@@ -3,6 +3,8 @@
 // QAP evaluations at tau into query scalars.  Mirrors what `Groth16::circuit_specific_setup` does in the reference's
 // drivers (/root/reference/groth16/examples/sha256.rs:133-137, mpc-api/src/main.rs:148-152) with the CircomReduction
 // h-query of ark-circom/src/circom/qap.rs:94-110; orchestration in distributed_groth16_b200/groth16/setup.py.
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace b200zk {
@@ -89,6 +91,135 @@ __global__ void k_spmv(const uint32_t* ptr, const uint32_t* idx, const Fr* val, 
     Fr acc = Fr::zero();
     for (uint32_t k = ptr[r], e = ptr[r + 1]; k < e; ++k) acc = Fr::add(acc, Fr::mul(lds(val + k), lds(x + idx[k])));
     sts(out + r, acc);
+}
+
+// ---- CSR product over points: out[r] = sum_k val[k] * points[idx[k]]  (snarkjs `zkey new`) -----------------------
+// The rows are very skewed (the constant wire's column of A holds 17 896 of the sha256 circuit's 106 808 non-zeros, every
+// other column <= 64), so the work is split per non-zero: one variable-base scalar multiplication per thread into a
+// product array, then a per-row sum over it.  Rows longer than SPMV_MSM_ROW go through the MSM instead, which bounds the
+// per-row sum at SPMV_MSM_ROW additions -- about the cost of one scalar multiplication.
+// A 64-bit signed path for short coefficients (v or r - v below 2^64, e.g. -1) was measured and dropped: a warp runs as
+// long as its longest scalar and nearly every warp holds a full-width one, so the products kernel took the same time
+// (2^20-constraint synthetic circuit on an H100 80GB HBM3 at 400 W: 1787 ms with it, 1766 ms without).
+constexpr uint32_t SPMV_MSM_ROW = 256;
+
+template <class F>
+__global__ void __launch_bounds__(128) k_points_spmv_products(const uint32_t* idx, const Fr* val, const affine_t<F>* points,
+                                                              size_t lo, size_t hi, xyzz_t<F>* prod) {
+    size_t k = lo + (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= hi) return;
+    const Fr v = Fr::from_mont(lds(val + k));
+    int top = 7;
+    while (top >= 0 && v.l[top] == 0) --top;
+    xyzz_t<F> acc = xyzz_t<F>::identity();
+    if (top >= 0) {
+        const affine_t<F> p = lds(points + idx[k]);
+        for (int bit = 32 * top + 31 - __clz(v.l[top]); bit >= 0; --bit) {     // double-and-add from the top set bit
+            acc = xyzz_t<F>::dbl(acc);
+            if ((v.l[bit >> 5] >> (bit & 31)) & 1) xyzz_t<F>::madd(acc, p, false);
+        }
+    }
+    sts(prod + k, acc);
+}
+
+// rows of at most SPMV_MSM_ROW entries: sum of their products, normalised; longer rows are left to the MSM path
+template <class F>
+__global__ void __launch_bounds__(128) k_points_spmv_sum(const uint32_t* ptr, const xyzz_t<F>* prod, size_t n_rows, affine_t<F>* out) {
+    size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_rows) return;
+    const uint32_t b = ptr[r], e = ptr[r + 1];
+    if (e - b > SPMV_MSM_ROW) return;
+    xyzz_t<F> acc = xyzz_t<F>::identity();
+    for (uint32_t k = b; k < e; ++k) acc = xyzz_t<F>::add(acc, lds(prod + k));
+    sts(out + r, xyzz_t<F>::to_affine(acc));
+}
+
+template <class F>
+__global__ void k_points_gather(const uint32_t* idx, const affine_t<F>* points, size_t n, affine_t<F>* out) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) sts(out + i, lds(points + idx[i]));
+}
+
+template <class F>
+__global__ void k_xyzz_to_affine_one(const xyzz_t<F>* in, affine_t<F>* out) {
+    if (threadIdx.x == 0) sts(out, xyzz_t<F>::to_affine(lds(in)));
+}
+
+template <class F>
+static int points_spmv_impl(b200zk_ctx* ctx, Slot& sl, const uint32_t* d_ptr, const uint32_t* d_idx, const Fr* d_val,
+                            const affine_t<F>* d_points, size_t n_rows, affine_t<F>* d_out) {
+    cudaStream_t st = sl.stream;
+    // the row pointers decide which rows take the MSM path: read them once on the host (index work only)
+    std::vector<uint32_t> ptr(n_rows + 1);
+    B2_CUDA_OK(ctx, cudaMemcpyAsync(ptr.data(), d_ptr, (n_rows + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    B2_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    const size_t nnz = ptr[n_rows];
+    std::vector<size_t> long_rows;
+    for (size_t r = 0; r < n_rows; ++r) {
+        if (ptr[r + 1] < ptr[r]) return set_error(ctx, B200ZK_ERR_ARG, "points_spmv: row pointers decrease");
+        if (ptr[r + 1] - ptr[r] > SPMV_MSM_ROW) long_rows.push_back(r);
+    }
+    xyzz_t<F>* prod = nullptr;
+    affine_t<F>* gathered = nullptr;
+    void* msm_out = nullptr;
+    size_t longest = 0;
+    for (size_t r : long_rows) longest = std::max(longest, (size_t)(ptr[r + 1] - ptr[r]));
+    int rc = B200ZK_OK;
+    auto run = [&]() -> int {
+        B2_CUDA_OK(ctx, cudaMalloc(&prod, (nnz ? nnz : 1) * sizeof(xyzz_t<F>)));
+        // products of every non-zero outside the long rows: one launch per gap between them
+        size_t lo = 0;
+        for (size_t i = 0; i <= long_rows.size(); ++i) {
+            const size_t hi = i < long_rows.size() ? ptr[long_rows[i]] : nnz;
+            if (hi > lo) {
+                LaunchScope ls(ctx, st, "points_spmv_products");
+                k_points_spmv_products<F><<<(unsigned)((hi - lo + 127) / 128), 128, 0, st>>>(d_idx, d_val, d_points, lo, hi, prod);
+            }
+            B2_TRY(check_launch(ctx, "k_points_spmv_products"));
+            if (i < long_rows.size()) lo = ptr[long_rows[i] + 1];
+        }
+        {
+            LaunchScope ls(ctx, st, "points_spmv_sum");
+            k_points_spmv_sum<F><<<(unsigned)((n_rows + 127) / 128), 128, 0, st>>>(d_ptr, prod, n_rows, d_out);
+        }
+        B2_TRY(check_launch(ctx, "k_points_spmv_sum"));
+        if (long_rows.empty()) return B200ZK_OK;
+        B2_CUDA_OK(ctx, cudaMalloc(&gathered, longest * sizeof(affine_t<F>)));
+        B2_CUDA_OK(ctx, cudaMalloc(&msm_out, sizeof(xyzz_t<F>)));
+        for (size_t r : long_rows) {
+            const size_t b = ptr[r], len = ptr[r + 1] - ptr[r];
+            {
+                LaunchScope ls(ctx, st, "points_gather");
+                k_points_gather<F><<<(unsigned)((len + 255) / 256), 256, 0, st>>>(d_idx + b, d_points, len, gathered);
+            }
+            B2_TRY(check_launch(ctx, "k_points_gather"));
+            B2_TRY(sizeof(F) > 32 ? msm_g2_dev(ctx, sl, gathered, d_val + b, len, msm_out)
+                                  : msm_g1_dev(ctx, sl, gathered, d_val + b, len, msm_out));
+            {
+                LaunchScope ls(ctx, st, "xyzz_to_affine");
+                k_xyzz_to_affine_one<F><<<1, 32, 0, st>>>(reinterpret_cast<const xyzz_t<F>*>(msm_out), d_out + r);
+            }
+            B2_TRY(check_launch(ctx, "k_xyzz_to_affine_one"));
+        }
+        return B200ZK_OK;
+    };
+    rc = run();
+    cudaError_t e = cudaStreamSynchronize(st);        // the temporaries are freed below
+    cudaFree(prod);
+    cudaFree(gathered);
+    cudaFree(msm_out);
+    if (rc != B200ZK_OK) return rc;
+    B2_CUDA_OK(ctx, e);
+    return B200ZK_OK;
+}
+
+int points_spmv_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* ptr, const void* idx, const void* val, const void* points,
+                    size_t n_rows, void* out) {
+    if (n_rows == 0) return B200ZK_OK;
+    return g2 ? points_spmv_impl<Fq2>(ctx, sl, (const uint32_t*)ptr, (const uint32_t*)idx, (const Fr*)val,
+                                      (const affine_t<Fq2>*)points, n_rows, (affine_t<Fq2>*)out)
+              : points_spmv_impl<Fq>(ctx, sl, (const uint32_t*)ptr, (const uint32_t*)idx, (const Fr*)val,
+                                     (const affine_t<Fq>*)points, n_rows, (affine_t<Fq>*)out);
 }
 
 // out[i] = (a[i] * s[0] + b[i] * s[1] + c[i] * s[2]) * s[3]

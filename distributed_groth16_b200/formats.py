@@ -134,6 +134,156 @@ def read_zkey(buf: bytes) -> ZKey:
                 coef_val_r2=rec["v"].copy())
 
 
+_COEF = np.dtype([("m", "<u4"), ("c", "<u4"), ("s", "<u4"), ("v", "<u8", (4,))])
+_ZKEY_ORDER = (1, 2, 4, 3, 9, 8, 5, 6, 7, 10)            # the section order snarkjs writes
+_R2_LIMBS = np.array([((1 << 512) % FR_MODULUS >> (64 * i)) & 0xFFFFFFFFFFFFFFFF for i in range(4)], dtype=np.uint64)
+
+
+def zkey_cir_power(n_constraints: int, n_public: int) -> int:
+    """log2 of the zkey domain, ceil(log2(n_constraints + n_public + 1)): the constraints and the n_public + 1
+    input-consistency rows must fit."""
+    return (n_constraints + n_public).bit_length()
+
+
+def zkey_coefficients(n_public: int, n_constraints: int, a, b):
+    """The coefficient section (4) of a zkey as (matrix, constraint, signal, value * R^2) arrays, in snarkjs order: by
+    constraint, A before B, then the input-consistency rows (0, n_constraints + j, j, 1) for j <= n_public.  a, b: (rows,
+    cols, values already multiplied by R^2 as (n, 4) u64 limbs) of the r1cs A and B matrices.  Index work only."""
+    m = [np.zeros(len(a[0]), np.uint32), np.ones(len(b[0]), np.uint32), np.zeros(n_public + 1, np.uint32)]
+    c = [np.asarray(a[0], np.uint32), np.asarray(b[0], np.uint32), np.arange(n_constraints, n_constraints + n_public + 1, dtype=np.uint32)]
+    s = [np.asarray(a[1], np.uint32), np.asarray(b[1], np.uint32), np.arange(n_public + 1, dtype=np.uint32)]
+    v = [np.asarray(a[2], np.uint64).reshape(-1, 4), np.asarray(b[2], np.uint64).reshape(-1, 4), np.tile(_R2_LIMBS, (n_public + 1, 1))]
+    m, c, s, v = (np.concatenate(x) for x in (m, c, s, v))
+    order = np.argsort(c, kind="stable")
+    return m[order], c[order], s[order], v[order]
+
+
+def write_zkey(zk: ZKey, section10: bytes | None = None) -> bytes:
+    """A Groth16 .zkey (snarkjs layout, the one read_zkey and ark-circom/src/zkey.rs read) with sections 1-10 in snarkjs
+    order.  section10 defaults to a zero csHash (64 bytes) and zero phase-2 contributions: the real csHash hashes the
+    ceremony's tau powers in snarkjs's order, which this writer does not compute, so `snarkjs zkey verify` rejects such a
+    file while ark-circom's reader (and read_zkey) ignore the section."""
+    hdr = struct.pack("<I", 32) + FQ_MODULUS.to_bytes(32, "little") + struct.pack("<I", 32) + FR_MODULUS.to_bytes(32, "little")
+    hdr += struct.pack("<III", zk.n_vars, zk.n_public, zk.domain_size)
+    pts = lambda a, w: np.ascontiguousarray(a, dtype="<u8").reshape(-1, w).tobytes()
+    hdr += b"".join(pts(p, w) for p, w in ((zk.alpha_g1, 8), (zk.beta_g1, 8), (zk.beta_g2, 16), (zk.gamma_g2, 16),
+                                            (zk.delta_g1, 8), (zk.delta_g2, 16)))
+    rec = np.empty(len(zk.coef_matrix), dtype=_COEF)
+    rec["m"], rec["c"], rec["s"], rec["v"] = zk.coef_matrix, zk.coef_row, zk.coef_col, np.asarray(zk.coef_val_r2).reshape(-1, 4)
+    secs = {1: struct.pack("<I", 1), 2: hdr, 3: pts(zk.ic, 8), 4: struct.pack("<I", len(rec)) + rec.tobytes(),
+            5: pts(zk.a_query, 8), 6: pts(zk.b_g1_query, 8), 7: pts(zk.b_g2_query, 16), 8: pts(zk.l_query, 8),
+            9: pts(zk.h_query, 8), 10: bytes(64) + struct.pack("<I", 0) if section10 is None else bytes(section10)}
+    return b"zkey" + struct.pack("<II", 1, len(_ZKEY_ORDER)) + b"".join(
+        struct.pack("<IQ", sid, len(secs[sid])) + secs[sid] for sid in _ZKEY_ORDER)
+
+
+class PTau:
+    """A prepared Powers-of-Tau file (snarkjs `powersoftau prepare phase2`), memory-mapped: only the points a circuit needs
+    are ever read (a 2^28 ceremony is hundreds of GB, a 2^20 circuit needs well under 1 GB of it).
+
+    Layout (restated from snarkjs; points are Montgomery little-endian affine, infinity all-zero): section 1 = n8, q,
+    power, ceremonyPower; 4 / 5 / 6 = alpha tau^i G1, beta tau^i G1, beta G2 (their first points are alpha_1, beta_1,
+    beta_2); 12 / 13 / 14 / 15 = the Lagrange bases L G1, L G2, alpha L G1, beta L G1 of every domain 2^k, level k starting
+    at point 2^k - 1 -- levels 0..power + 1 in section 12, 0..power in the others."""
+
+    _LAGRANGE = {12: 8, 13: 16, 14: 8, 15: 8}      # section -> u64 limbs per point
+
+    def __init__(self, path: str):
+        import mmap
+        self._f = open(path, "rb")
+        try:
+            size = self._f.seek(0, 2)
+            if size < 12:
+                raise FormatError("ptau file too short (%d bytes)" % size)
+            self._mm = mmap.mmap(self._f.fileno(), 0, access=mmap.ACCESS_READ)
+            self._parse(size)
+        except BaseException:
+            self.close()
+            raise
+
+    def _parse(self, size: int):
+        mm = self._mm
+        if mm[:4] != b"ptau":
+            raise FormatError("bad magic %r (expected b'ptau')" % mm[:4])
+        _version, nsec = struct.unpack_from("<II", mm, 4)
+        off, secs = 12, {}
+        for _ in range(nsec):
+            if off + 12 > size:
+                raise FormatError("ptau section table runs past the end of the file")
+            sid, ln = struct.unpack_from("<IQ", mm, off)
+            off += 12
+            if off + ln > size:
+                raise FormatError("ptau section %d runs past the end of the file" % sid)
+            secs.setdefault(sid, (off, ln))
+            off += ln
+        self._secs = secs
+        if 1 not in secs or secs[1][1] < 4:
+            raise FormatError("ptau header section 1 missing")
+        o1, l1 = secs[1]
+        n8 = struct.unpack_from("<I", mm, o1)[0]
+        if n8 != 32 or l1 < 4 + n8 + 8:
+            raise FormatError("ptau is not over BN254 (n8 = %d)" % n8)
+        if int.from_bytes(mm[o1 + 4:o1 + 4 + n8], "little") != FQ_MODULUS:
+            raise FormatError("ptau is not over BN254 (wrong q)")
+        self.power, self.ceremony_power = struct.unpack_from("<II", mm, o1 + 4 + n8)
+        missing = [sid for sid in (12, 13, 14, 15) if sid not in secs]
+        if missing:
+            raise FormatError("ptau has no Lagrange sections %s: it is not prepared for phase 2 (run snarkjs powersoftau "
+                              "prepare phase2 on it first)" % missing)
+        need = {4: 64, 5: 64, 6: 128}
+        for sid, w in self._LAGRANGE.items():
+            need[sid] = ((1 << (self.power + (2 if sid == 12 else 1))) - 1) * w * 8
+        for sid, ln in need.items():
+            if sid not in secs:
+                raise FormatError("ptau section %d missing" % sid)
+            if secs[sid][1] < ln:
+                raise FormatError("ptau section %d too short for power %d (%d < %d bytes)" % (sid, self.power, secs[sid][1], ln))
+
+    def _points(self, sid: int, first: int, count: int, width: int) -> np.ndarray:
+        off = self._secs[sid][0] + first * width * 8
+        return np.frombuffer(self._mm, dtype="<u8", count=count * width, offset=off).reshape(count, width).copy()
+
+    @property
+    def alpha_g1(self) -> np.ndarray:
+        return self._points(4, 0, 1, 8)[0]
+
+    @property
+    def beta_g1(self) -> np.ndarray:
+        return self._points(5, 0, 1, 8)[0]
+
+    @property
+    def beta_g2(self) -> np.ndarray:
+        return self._points(6, 0, 1, 16)[0]
+
+    def lagrange(self, sid: int, level: int) -> np.ndarray:
+        """Level `level` (2^level points) of Lagrange section sid (12, 13, 14 or 15) as (2^level, 8 | 16) u64 limbs."""
+        top = self.power + (1 if sid == 12 else 0)
+        if level > top:
+            raise FormatError("the circuit needs Lagrange level %d of ptau section %d, the ceremony (power %d) has levels up "
+                              "to %d: the circuit is too big for it" % (level, sid, self.power, top))
+        return self._points(sid, (1 << level) - 1, 1 << level, self._LAGRANGE[sid])
+
+    def close(self):
+        mm, self._mm = getattr(self, "_mm", None), None
+        if mm is not None:
+            mm.close()
+        f, self._f = getattr(self, "_f", None), None
+        if f is not None:
+            f.close()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+def read_ptau(path: str) -> PTau:
+    """Open a prepared .ptau (memory-mapped; see PTau).  Raises FormatError for a file that is not a BN254 ptau, is not
+    prepared for phase 2 or whose sections are shorter than its stated power."""
+    return PTau(path)
+
+
 def read_wtns(buf: bytes) -> np.ndarray:
     """(n, 4) u64 canonical (non-Montgomery) witness values."""
     secs = _sections(buf, b"wtns")

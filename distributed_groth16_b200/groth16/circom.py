@@ -25,6 +25,31 @@ def load_zkey(net: Net, zkey_bytes: bytes):
     return pk, mats, zk
 
 
+def zkey_new(net: Net, r1cs_bytes: bytes, ptau_path: str) -> bytes:
+    """snarkjs `zkey new <r1cs> <ptau>` on the GPU (scripts/phase2_proving_key.sh, ark-circom/test-vectors/complex-circuit/
+    build.sh:11): the .zkey bytes of the circuit's proving key from a prepared Powers-of-Tau file.  The key has delta = 1
+    and a zero csHash (formats.write_zkey): it needs a phase-2 contribution before production use."""
+    with formats.read_ptau(ptau_path) as pt:
+        return zkey_from_r1cs(net, formats.read_r1cs(r1cs_bytes), pt)
+
+
+def zkey_from_r1cs(net: Net, r1: formats.R1CS, pt: formats.PTau) -> bytes:
+    """zkey_new on a parsed r1cs and an open ceremony file."""
+    from .setup import ptau_key_points
+    q = ptau_key_points(net, r1, pt)
+    r2 = lambda i: net.fr_convert(net.to_device(np.ascontiguousarray(r1.vals[i], dtype=np.uint64).reshape(-1, 4)),
+                                  to_mont=True, times=2).cpu().numpy().view(np.uint64)     # value * R^2, on the device
+    mi, ci, si, vi = formats.zkey_coefficients(q["n_public"], r1.n_constraints, (r1.rows[0], r1.cols[0], r2(0)),
+                                               (r1.rows[1], r1.cols[1], r2(1)))
+    host = lambda t: t.cpu().numpy().view(np.uint64)
+    zk = formats.ZKey(n_vars=q["n_vars"], n_public=q["n_public"], domain_size=q["domain_size"], alpha_g1=q["alpha_g1"],
+                      beta_g1=q["beta_g1"], beta_g2=q["beta_g2"], gamma_g2=q["gamma_g2"], delta_g1=q["delta_g1"],
+                      delta_g2=q["delta_g2"], ic=host(q["ic"]), a_query=host(q["a_query"]), b_g1_query=host(q["b_g1_query"]),
+                      b_g2_query=host(q["b_g2_query"]), l_query=host(q["l_query"]), h_query=host(q["h_query"]),
+                      coef_matrix=mi, coef_row=ci, coef_col=si, coef_val_r2=vi)
+    return formats.write_zkey(zk)
+
+
 def load_witness(net: Net, wtns_bytes: bytes):
     """.wtns -> full assignment z on the device in Montgomery form (wire index == witness index: the reference
     disables the wire mapping, ark-circom/src/circom/builder.rs:63-64)."""

@@ -88,6 +88,83 @@ def _transpose_csr(net, rows, cols, vals_dev_order, n_cols, extra=None):
     return net.to_device(ptr.view(np.int32)), net.to_device(idx.view(np.int32)), vals_dev_order[d_order].contiguous()
 
 
+def _points_spmv(net, csr, points, n_rows: int, g2=False):
+    """out[r] = sum_k val[k] * points[idx[k]] over a CSR (ptr, idx, val) on the device (b200zk_points_spmv_dev)."""
+    import torch
+    ptr, idx, val = csr
+    out = torch.empty((n_rows, 16 if g2 else 8), dtype=torch.int64, device=points.device)
+    net.check(net._lib.b200zk_points_spmv_dev(net._h, 0, int(g2), c_vp(ptr.data_ptr()), c_vp(idx.data_ptr()),
+                                              c_vp(val.data_ptr()), c_vp(points.data_ptr()), n_rows, c_vp(out.data_ptr())))
+    return out
+
+
+def ptau_key_points(net, r1cs, ptau) -> dict:
+    """What snarkjs `zkey new` computes from an r1cs (formats.R1CS) and a prepared Powers-of-Tau file (formats.PTau), as
+    CUDA tensors (the query vectors, ic) and host limb arrays (the six header points).  With L, L2, alpha L, beta L the
+    Lagrange bases of the circuit's domain 2^k and H those of 2^(k+1):
+
+      a_query[s] = sum_c A[c,s] L_c (+ L_{nc+s} for s <= n_public: the input-consistency rows, groth16/src/qap.rs:69-73)
+      b_g1_query[s] / b_g2_query[s] = sum_c B[c,s] L_c / L2_c
+      K[s] = sum_c (A[c,s] beta L_c + B[c,s] alpha L_c + C[c,s] L_c)  ->  ic = K[:n_public + 1], l_query = K[n_public + 1:]
+      h_query[i] = H_{2i+1}   (ark-circom/src/circom/qap.rs:11-15, 94-110)
+
+    alpha_1, beta_1, beta_2 come from the ceremony, gamma_2 = delta_2 and delta_1 are the generators: gamma = delta = 1
+    until a phase-2 contribution.  Every product runs as b200zk_points_spmv_dev over one CSR per query (K over the stacked
+    points [L | alpha L | beta L]); the host only reorders indices and moves the needed ceremony levels to the device."""
+    import torch
+    from .. import formats
+    n_vars, nc = int(r1cs.n_wires), int(r1cs.n_constraints)
+    n_public = int(r1cs.n_pub_out + r1cs.n_pub_in)
+    n_inputs = n_public + 1
+    k = formats.zkey_cir_power(nc, n_public)
+    m = 1 << k
+    net.use_torch_stream(0)
+    lag, lag2, alag, blag = (net.to_device(ptau.lagrange(sid, k)) for sid in (12, 13, 14, 15))
+    h_query = net.to_device(np.ascontiguousarray(ptau.lagrange(12, k + 1)[1::2]))
+    dev = lag.device
+    one = torch.from_numpy(_mont_limbs(1).view(np.int64)).to(dev).reshape(1, 4)
+
+    def coo(i):
+        rows, cols = np.asarray(r1cs.rows[i], np.int64), np.asarray(r1cs.cols[i], np.int64)
+        vals = net.fr_convert(net.to_device(np.ascontiguousarray(r1cs.vals[i], dtype=np.uint64).reshape(-1, 4)), to_mont=True)
+        return rows, cols, vals
+
+    (ar, ac, av), (br, bc, bv), (cr, cc, cv) = coo(0), coo(1), coo(2)
+    ar = np.concatenate([ar, np.arange(nc, nc + n_inputs)])          # input-consistency rows a[nc + j] = z[j]
+    ac = np.concatenate([ac, np.arange(n_inputs)])
+    av = torch.cat([av, one.expand(n_inputs, 4)], dim=0).contiguous()
+    a_csr = _transpose_csr(net, ar, ac, av, n_vars)
+    b_csr = _transpose_csr(net, br, bc, bv, n_vars)
+    k_csr = _transpose_csr(net, np.concatenate([cr, br + m, ar + 2 * m]), np.concatenate([cc, bc, ac]),
+                           torch.cat([cv, bv, av], dim=0), n_vars)
+    a_query = _points_spmv(net, a_csr, lag, n_vars)
+    b_g1_query = _points_spmv(net, b_csr, lag, n_vars)
+    b_g2_query = _points_spmv(net, b_csr, lag2, n_vars, g2=True)
+    kq = _points_spmv(net, k_csr, torch.cat([lag, alag, blag], dim=0), n_vars)
+    g1 = _fixed_base(net, one).cpu().numpy().view(np.uint64)[0]
+    g2 = _fixed_base(net, one, g2=True).cpu().numpy().view(np.uint64)[0]
+    return dict(n_vars=n_vars, n_public=n_public, domain_size=m, a_query=a_query, b_g1_query=b_g1_query,
+                b_g2_query=b_g2_query, ic=kq[:n_inputs].contiguous(), l_query=kq[n_inputs:].contiguous(), h_query=h_query,
+                alpha_g1=ptau.alpha_g1, beta_g1=ptau.beta_g1, beta_g2=ptau.beta_g2, gamma_g2=g2, delta_g1=g1, delta_g2=g2)
+
+
+def setup_from_ptau(net, r1cs, ptau):
+    """Groth16 setup from a ceremony instead of known toxic waste: snarkjs `zkey new` (what the reference's
+    scripts/phase2_proving_key.sh runs before proving) on the GPU.  r1cs: formats.R1CS; ptau: formats.PTau (read_ptau).
+    Returns (ProvingKey on the device, VerifyingKey as host limb arrays, ConstraintMatrices) like circuit_specific_setup.
+    The key has delta = 1: it needs a phase-2 contribution before production use."""
+    q = ptau_key_points(net, r1cs, ptau)
+    n_inputs = q["n_public"] + 1
+    vk_points = np.concatenate([q["alpha_g1"], q["beta_g1"], q["delta_g1"], q["beta_g2"], q["delta_g2"]])
+    pk = ProvingKey.from_device(net, q["a_query"], q["b_g1_query"], q["b_g2_query"], q["l_query"], q["h_query"], n_inputs,
+                                vk_points)
+    vk = VerifyingKey(alpha_g1=q["alpha_g1"], beta_g2=q["beta_g2"], gamma_g2=q["gamma_g2"], delta_g2=q["delta_g2"],
+                      gamma_abc_g1=q["ic"].cpu().numpy().view(np.uint64))
+    coo = lambda i: (r1cs.rows[i], r1cs.cols[i], r1cs.vals[i])
+    mats = ConstraintMatrices(net, n_inputs, int(r1cs.n_constraints), coo(0), coo(1), values_montgomery_depth=-1)
+    return pk, vk, mats
+
+
 def circuit_specific_setup(net, n_vars: int, n_inputs: int, num_constraints: int, a_coo, b_coo, c_coo, toxic,
                            values_montgomery_depth: int = -1, g1_generator=None, g2_generator=None):
     """a_coo / b_coo / c_coo: (rows, cols, vals (nnz, 4) u64) of the R1CS matrices; toxic = (tau, alpha, beta, gamma, delta)

@@ -243,6 +243,14 @@ int b200zk_fr_powers_dev(b200zk_ctx* ctx, const uint64_t base[4], const uint64_t
 /* Generic CSR mat-vec over Fr: out[r] = sum val[k] x[idx[k]], k in [ptr[r], ptr[r+1]). */
 int b200zk_fr_spmv_dev(b200zk_ctx* ctx, const void* d_ptr, const void* d_idx, const void* d_val, const void* d_x,
                        size_t n_rows, void* d_out);
+/* The same CSR product over group elements: out[r] = sum val[k] points[idx[k]], k in [ptr[r], ptr[r+1]) -- the step of
+ * snarkjs `zkey new` that turns a Powers-of-Tau file's Lagrange bases into the query vectors, and (over the odd points of
+ * the doubled domain) the h-query convention of ark-circom/src/circom/qap.rs:11-15.  Conventions as
+ * b200zk_fr_spmv_dev: ptr n_rows + 1 x u32, idx nnz x u32, val nnz x 4 limbs Montgomery; points / out affine (g2 = 0: G1,
+ * 8 u64 limbs; 1: G2, 16), infinity all-zero, an empty row gives infinity.  Rows of more than 256 entries go through the
+ * MSM.  Reads ptr to the host and returns once out is complete; temporary device memory: nnz XYZZ points. */
+int b200zk_points_spmv_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_ptr, const void* d_idx, const void* d_val,
+                           const void* d_points, size_t n_rows, void* d_out);
 /* out[i] = (a[i] s0 + b[i] s1 + c[i] s2) s3   (s: 16 limbs = 4 Montgomery scalars, host). */
 int b200zk_fr_lincomb_dev(b200zk_ctx* ctx, const void* d_a, const void* d_b, const void* d_c, const uint64_t s[16], size_t n,
                           void* d_out);
