@@ -712,6 +712,14 @@ int b200zk_points_spmv_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_pt
     B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
     return points_spmv_dev(ctx, sl, g2, d_ptr, d_idx, d_val, d_points, n_rows, d_out);
 }
+int b200zk_points_scale_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_points, size_t n, const uint64_t k[4],
+                            void* d_out) {
+    if (!ctx || !k || !valid_slot(stream) || (n && (!d_points || !d_out))) return B200ZK_ERR_ARG;
+    Slot& sl = ctx->slots[stream];
+    std::lock_guard<std::mutex> g(sl.mu);
+    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
+    return points_scale_dev(ctx, sl, g2, d_points, n, k, d_out);
+}
 int b200zk_fr_lincomb_dev(b200zk_ctx* ctx, const void* d_a, const void* d_b, const void* d_c, const uint64_t s[16], size_t n,
                           void* d_out) {
     if (!ctx || !s || (n && (!d_a || !d_b || !d_c || !d_out))) return B200ZK_ERR_ARG;

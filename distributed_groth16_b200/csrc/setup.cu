@@ -6,6 +6,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "glv.cuh"
 
 namespace b200zk {
 
@@ -297,6 +298,200 @@ int fr_lincomb_dev(b200zk_ctx* ctx, Slot& sl, const void* a, const void* b, cons
     B2_TRY(check_launch(ctx, "k_fr_lincomb"));
     B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
     return B200ZK_OK;
+}
+
+// ---- one scalar times many points: out[i] = k * points[i]  (snarkjs `zkey contribute`: L and H times delta^-1) ------
+// The phase-2 step the reference's scripts/phase2_proving_key.sh runs after `zkey new`; orchestration in groth16/phase2.py.
+// G1: k is reduced mod r and split once per launch, k = k1 + k2 lambda (glv.cuh), and both halves are recoded on the
+// host into width-5 NAF digits (odd, |d| <= 15, at least four zeros after each non-zero).  The digits travel as a kernel
+// parameter and are the same for every thread, so the digit loop has no divergence: per point about 128 doublings and
+// ~43 mixed additions from a per-thread table of the odd multiples P, 3P, .., 15P (phi(jP) = (beta x, y) is applied on
+// the fly).  The table entries and the results are normalised to affine with block-batched inversions (Montgomery's
+// trick over a block-wide prefix / suffix product): 8 field inversions per block of 64 points, not one per point.
+constexpr int SCALE_BLOCK = 64;
+constexpr int SCALE_NAF = 130;            // |k1|, |k2| < 2^127: at most 128 NAF digits
+constexpr int SCALE_TAB = 8;              // P, 3P, .., 15P
+
+struct ScaleDigits {
+    int8_t d[2][SCALE_NAF];               // d[h][i]: digit i (weight 2^i) of k1 (h = 0) / k2 (h = 1), signs folded in
+    int top;                              // highest index with a non-zero digit in either half; -1: k = 0 mod r
+};
+
+// a^-1 for every thread's a (a != 0) of the block, with one F::inv: inclusive prefix and suffix products
+// (Hillis-Steele, log2(B) steps), then a_t^-1 = (a_0 .. a_{B-1})^-1 * prefix_{t-1} * suffix_{t+1}.  All threads call it.
+template <class F, int B>
+__device__ F block_batch_inv(const F& a, F* pre, F* suf, F* tot) {
+    const int t = threadIdx.x;
+    F p = a, s = a;
+    pre[t] = p;
+    suf[t] = s;
+    __syncthreads();
+#pragma unroll 1
+    for (int off = 1; off < B; off <<= 1) {
+        F pp = t >= off ? pre[t - off] : F::one();
+        F ss = t + off < B ? suf[t + off] : F::one();
+        __syncthreads();
+        if (t >= off) p = F::mul(p, pp);
+        if (t + off < B) s = F::mul(s, ss);
+        pre[t] = p;
+        suf[t] = s;
+        __syncthreads();
+    }
+    if (t == 0) *tot = F::inv(pre[B - 1]);
+    __syncthreads();
+    F r = *tot;
+    if (t > 0) r = F::mul(r, pre[t - 1]);
+    if (t < B - 1) r = F::mul(r, suf[t + 1]);
+    __syncthreads();                      // pre / suf / tot are reused by the next call
+    return r;
+}
+
+// table entry j of this thread, stored as 4 uint4 per point, [entry][chunk][thread]: conflict-free shared accesses
+__device__ __forceinline__ void scale_tab_put(uint4* tab, int j, const affine_t<Fq>& p) {
+    const uint4* s = reinterpret_cast<const uint4*>(&p);
+#pragma unroll
+    for (int c = 0; c < 4; ++c) tab[(j * 4 + c) * SCALE_BLOCK + threadIdx.x] = s[c];
+}
+__device__ __forceinline__ affine_t<Fq> scale_tab_get(const uint4* tab, int j) {
+    affine_t<Fq> p;
+    uint4* d = reinterpret_cast<uint4*>(&p);
+#pragma unroll
+    for (int c = 0; c < 4; ++c) d[c] = tab[(j * 4 + c) * SCALE_BLOCK + threadIdx.x];
+    return p;
+}
+
+__global__ void __launch_bounds__(SCALE_BLOCK) k_points_scale_g1(const __grid_constant__ ScaleDigits dg,
+                                                                  const affine_t<Fq>* points, size_t n, affine_t<Fq>* out) {
+    __shared__ uint4 tab[SCALE_TAB * 4 * SCALE_BLOCK];
+    __shared__ Fq pre[SCALE_BLOCK], suf[SCALE_BLOCK], tot;
+    const size_t i = (size_t)blockIdx.x * SCALE_BLOCK + threadIdx.x;
+    const affine_t<Fq> P = i < n ? lds(points + i) : affine_t<Fq>::infinity();
+    const bool inf = P.is_inf();
+    // the odd multiples, (2j + 1) P = (2j - 1) P + 2P in XYZZ, each normalised as it is made (one block-batched
+    // inverse per entry: only the running entry and 2P are live)
+    scale_tab_put(tab, 0, P);
+    {
+        const xyzz_t<Fq> two = inf ? xyzz_t<Fq>::identity() : xyzz_t<Fq>::dbl_affine(P.x, P.y);
+        xyzz_t<Fq> odd = xyzz_t<Fq>::from_affine(P);
+#pragma unroll 1
+        for (int j = 1; j < SCALE_TAB; ++j) {
+            odd = xyzz_t<Fq>::add(odd, two);
+            const Fq izzz = block_batch_inv<Fq, SCALE_BLOCK>(inf ? Fq::one() : odd.zzz, pre, suf, &tot);
+            affine_t<Fq> a = affine_t<Fq>::infinity();
+            if (!inf) {
+                const Fq izz = Fq::sqr(Fq::mul(izzz, odd.zz));                    // ZZ^3 = ZZZ^2  =>  1/ZZ = (ZZ/ZZZ)^2
+                a.x = Fq::mul(odd.x, izz);
+                a.y = Fq::mul(odd.y, izzz);
+            }
+            scale_tab_put(tab, j, a);
+        }
+    }
+    Fq beta;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) beta.l[j] = GlvParams::beta(j);
+    xyzz_t<Fq> acc = xyzz_t<Fq>::identity();
+    if (!inf) {
+#pragma unroll 1
+        for (int b = dg.top; b >= 0; --b) {
+            acc = xyzz_t<Fq>::dbl(acc);
+            const int d1 = dg.d[0][b], d2 = dg.d[1][b];
+            if (d1) xyzz_t<Fq>::madd(acc, scale_tab_get(tab, (d1 < 0 ? -d1 : d1) >> 1), d1 < 0);
+            if (d2) {
+                affine_t<Fq> q = scale_tab_get(tab, (d2 < 0 ? -d2 : d2) >> 1);
+                q.x = Fq::mul(q.x, beta);                                          // phi(jP) = (beta x, y)
+                xyzz_t<Fq>::madd(acc, q, d2 < 0);
+            }
+        }
+    }
+    const bool res_inf = acc.is_inf();
+    const Fq izzz = block_batch_inv<Fq, SCALE_BLOCK>(res_inf ? Fq::one() : acc.zzz, pre, suf, &tot);
+    if (i >= n) return;
+    affine_t<Fq> r = affine_t<Fq>::infinity();
+    if (!res_inf) {
+        const Fq izz = Fq::sqr(Fq::mul(izzz, acc.zz));
+        r.x = Fq::mul(acc.x, izz);
+        r.y = Fq::mul(acc.y, izzz);
+    }
+    sts(out + i, r);
+}
+
+// G2 (single points: delta_2, g2_spx, the cofactor of hash-to-G2): the plain 256-bit ladder, no reduction mod r, so that
+// it is right for twist points outside the order-r subgroup too
+struct ScaleK { uint32_t k[8]; };
+
+__global__ void __launch_bounds__(128) k_points_scale_g2_ladder(const __grid_constant__ ScaleK k, const affine_t<Fq2>* points,
+                                                                size_t n, affine_t<Fq2>* out) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const affine_t<Fq2> p = lds(points + i);
+    sts(out + i, xyzz_t<Fq2>::to_affine(xyzz_t<Fq2>::mul_scalar(xyzz_t<Fq2>::from_affine(p), k.k)));
+}
+
+// width-5 NAF of a non-negative k < 2^127 into d (digits odd in [-15, 15]); returns the highest non-zero index or -1
+static int naf5(unsigned __int128 k, int8_t* d) {
+    int top = -1;
+    for (int i = 0; i < SCALE_NAF; ++i) {
+        int v = 0;
+        if (k & 1) {
+            v = (int)(k & 31);
+            if (v >= 16) v -= 32;
+            if (v > 0) k -= (unsigned)v;
+            else k += (unsigned)(-v);
+            top = i;
+        }
+        d[i] = (int8_t)v;
+        k >>= 1;
+    }
+    return top;
+}
+
+int points_scale_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_points, size_t n, const uint64_t k64[4], void* d_out) {
+    if (n == 0) return B200ZK_OK;
+    uint32_t k[8];
+    for (int i = 0; i < 4; ++i) { k[2 * i] = (uint32_t)k64[i]; k[2 * i + 1] = (uint32_t)(k64[i] >> 32); }
+    if (g2) {
+        ScaleK sk;
+        memcpy(sk.k, k, sizeof(k));
+        {
+            LaunchScope ls(ctx, sl.stream, "points_scale_g2");
+            k_points_scale_g2_ladder<<<(unsigned)((n + 127) / 128), 128, 0, sl.stream>>>(
+                sk, reinterpret_cast<const affine_t<Fq2>*>(d_points), n, reinterpret_cast<affine_t<Fq2>*>(d_out));
+        }
+        return check_launch(ctx, "k_points_scale_g2");
+    }
+    for (;;) {                                          // k mod r: k < 2^256 < 6 r
+        bool ge = true;
+        for (int i = 7; i >= 0; --i) {
+            if (k[i] != FrParams::mod(i)) { ge = k[i] > FrParams::mod(i); break; }
+        }
+        if (!ge) break;
+        int64_t br = 0;
+        for (int i = 0; i < 8; ++i) {
+            int64_t v = (int64_t)k[i] - (int64_t)FrParams::mod(i) + br;
+            k[i] = (uint32_t)v;
+            br = v >> 32;
+        }
+    }
+    const GlvSplit sp = glv_decompose(k);
+    ScaleDigits dg;
+    int top = -1;
+    for (int h = 0; h < 2; ++h) {
+        const uint32_t* w = h ? sp.k2 : sp.k1;
+        unsigned __int128 v = 0;
+        for (int i = 3; i >= 0; --i) v = (v << 32) | w[i];
+        const int t = naf5(v, dg.d[h]);
+        if (h ? sp.neg2 : sp.neg1)
+            for (int i = 0; i < SCALE_NAF; ++i) dg.d[h][i] = (int8_t)-dg.d[h][i];
+        top = t > top ? t : top;
+    }
+    dg.top = top;
+    if (n >= ((size_t)1 << 31) * SCALE_BLOCK) return set_error(ctx, B200ZK_ERR_ARG, "points_scale: too many points");
+    {
+        LaunchScope ls(ctx, sl.stream, "points_scale_g1");
+        k_points_scale_g1<<<(unsigned)((n + SCALE_BLOCK - 1) / SCALE_BLOCK), SCALE_BLOCK, 0, sl.stream>>>(
+            dg, reinterpret_cast<const affine_t<Fq>*>(d_points), n, reinterpret_cast<affine_t<Fq>*>(d_out));
+    }
+    return check_launch(ctx, "k_points_scale_g1");
 }
 
 }  // namespace b200zk

@@ -284,6 +284,124 @@ def read_ptau(path: str) -> PTau:
     return PTau(path)
 
 
+@dataclass
+class Contribution:
+    """One phase-2 record of a zkey's section 10 (snarkjs `zkey contribute` / `zkey beacon`).  Points are Montgomery
+    little-endian affine limb arrays like the other sections (G1 8, G2 16 u64 limbs; infinity all-zero)."""
+    delta_after: np.ndarray        # delta_1 after this contribution
+    g1_s: np.ndarray
+    g1_sx: np.ndarray              # x g1_s
+    g2_spx: np.ndarray             # x hashToG2(transcript)
+    transcript: bytes              # 64 bytes
+    type: int = 0                  # 0 = contribution, 1 = beacon
+    name: str | None = None
+    num_iterations_exp: int | None = None
+    beacon_hash: bytes | None = None
+
+
+@dataclass
+class MPCParams:
+    """Section 10 of a zkey: the circuit hash and the phase-2 contributions, oldest first."""
+    cs_hash: bytes
+    contributions: list
+
+
+_MPC_NAME_MAX = 64
+
+
+def parse_mpc_params(sec: bytes) -> MPCParams:
+    """Section 10 bytes -> MPCParams.  Layout (restated from snarkjs zkey_utils read/writeMPCParams): csHash (64 bytes),
+    u32 count, then per contribution deltaAfter, g1_s, g1_sx (G1), g2_spx (G2), transcript (64 bytes), u32 type, u32 byte
+    length of a key / value stream: 1 = name (u8 length + UTF-8, at most 64 bytes), 2 = numIterationsExp (u8), 3 =
+    beaconHash (u8 length + bytes).  Raises FormatError for a truncated section, a count that runs past it, an unknown
+    parameter key or an over-long name."""
+    sec = bytes(sec)
+
+    def need(off, n, what):
+        if off + n > len(sec):
+            raise FormatError("zkey section 10 ends inside %s (%d + %d > %d bytes)" % (what, off, n, len(sec)))
+
+    need(0, 68, "the csHash and contribution count")
+    cs_hash, count = sec[:64], struct.unpack_from("<I", sec, 64)[0]
+    rec = 3 * 64 + 128 + 64 + 8                     # fixed part of one contribution
+    if 68 + count * rec > len(sec):
+        raise FormatError("zkey section 10 claims %d contributions, more than its %d bytes hold" % (count, len(sec)))
+    off, out = 68, []
+    for i in range(count):
+        need(off, rec, "contribution %d" % i)
+        pts = np.frombuffer(sec, dtype="<u8", count=40, offset=off).copy()
+        off += 320
+        transcript = sec[off:off + 64]
+        ctype, plen = struct.unpack_from("<II", sec, off + 64)
+        off += 72
+        need(off, plen, "the parameters of contribution %d" % i)
+        p, end = off, off + plen
+        c = Contribution(delta_after=pts[:8], g1_s=pts[8:16], g1_sx=pts[16:24], g2_spx=pts[24:40], transcript=transcript,
+                         type=ctype)
+        while p < end:
+            key = sec[p]
+            if key == 1:
+                if p + 2 > end or p + 2 + sec[p + 1] > end:
+                    raise FormatError("contribution %d: name runs past its parameters" % i)
+                ln = sec[p + 1]
+                if ln > _MPC_NAME_MAX:
+                    raise FormatError("contribution %d: name of %d bytes (at most %d)" % (i, ln, _MPC_NAME_MAX))
+                try:
+                    c.name = sec[p + 2:p + 2 + ln].decode("utf-8")
+                except UnicodeDecodeError as e:
+                    raise FormatError("contribution %d: name is not UTF-8 (%s)" % (i, e)) from None
+                p += 2 + ln
+            elif key == 2:
+                if p + 2 > end:
+                    raise FormatError("contribution %d: numIterationsExp runs past its parameters" % i)
+                c.num_iterations_exp = sec[p + 1]
+                p += 2
+            elif key == 3:
+                if p + 2 > end or p + 2 + sec[p + 1] > end:
+                    raise FormatError("contribution %d: beacon hash runs past its parameters" % i)
+                c.beacon_hash = sec[p + 2:p + 2 + sec[p + 1]]
+                p += 2 + sec[p + 1]
+            else:
+                raise FormatError("contribution %d: unknown parameter key %d" % (i, key))
+        off = end
+        out.append(c)
+    return MPCParams(cs_hash=cs_hash, contributions=out)
+
+
+def read_mpc_params(zkey_bytes: bytes) -> MPCParams:
+    """The phase-2 parameters (section 10) of a zkey; see parse_mpc_params."""
+    secs = _sections(zkey_bytes, b"zkey")
+    if 10 not in secs:
+        raise FormatError("zkey section 10 missing")
+    off, ln = secs[10][0]
+    if off + ln > len(zkey_bytes):
+        raise FormatError("zkey section 10 runs past the end of the file")
+    return parse_mpc_params(zkey_bytes[off:off + ln])
+
+
+def mpc_params_bytes(params: MPCParams) -> bytes:
+    """MPCParams -> section 10 bytes (the inverse of parse_mpc_params; feed them to write_zkey(zk, section10=...))."""
+    if len(params.cs_hash) != 64:
+        raise FormatError("csHash must be 64 bytes, got %d" % len(params.cs_hash))
+    out = [bytes(params.cs_hash), struct.pack("<I", len(params.contributions))]
+    for c in params.contributions:
+        pts = [np.ascontiguousarray(a, dtype="<u8").reshape(-1) for a in (c.delta_after, c.g1_s, c.g1_sx, c.g2_spx)]
+        if [p.size for p in pts] != [8, 8, 8, 16] or len(c.transcript) != 64:
+            raise FormatError("contribution points must be 8, 8, 8 and 16 limbs and the transcript 64 bytes")
+        prm = b""
+        if c.name:
+            name = c.name.encode("utf-8")
+            if len(name) > _MPC_NAME_MAX:
+                raise FormatError("contribution name of %d bytes (at most %d)" % (len(name), _MPC_NAME_MAX))
+            prm += bytes([1, len(name)]) + name
+        if c.type == 1:
+            if c.num_iterations_exp is None or c.beacon_hash is None or len(c.beacon_hash) > 255:
+                raise FormatError("a beacon record needs numIterationsExp and a beacon hash of at most 255 bytes")
+            prm += bytes([2, c.num_iterations_exp, 3, len(c.beacon_hash)]) + bytes(c.beacon_hash)
+        out += [b"".join(p.tobytes() for p in pts), bytes(c.transcript), struct.pack("<II", c.type, len(prm)), prm]
+    return b"".join(out)
+
+
 def read_wtns(buf: bytes) -> np.ndarray:
     """(n, 4) u64 canonical (non-Montgomery) witness values."""
     secs = _sections(buf, b"wtns")

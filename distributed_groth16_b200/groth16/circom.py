@@ -33,6 +33,49 @@ def zkey_new(net: Net, r1cs_bytes: bytes, ptau_path: str) -> bytes:
         return zkey_from_r1cs(net, formats.read_r1cs(r1cs_bytes), pt)
 
 
+def _random_scalar(entropy: bytes) -> int:
+    """A non-zero scalar mod r from os.urandom mixed with the caller's entropy through Blake2b-512."""
+    import hashlib
+    import os
+    while True:
+        v = int.from_bytes(hashlib.blake2b(os.urandom(64) + bytes(entropy), digest_size=64).digest(), "little") % formats.FR_MODULUS
+        if v:
+            return v
+
+
+def zkey_contribute(net: Net, zkey_bytes: bytes, name: str | None = None, entropy: bytes = b""):
+    """snarkjs `zkey contribute` on the GPU (scripts/phase2_proving_key.sh): a phase-2 contribution with a fresh secret x
+    (os.urandom mixed with `entropy` through Blake2b) and proof-of-knowledge base g1_s = s G for a fresh s.  L and H are
+    multiplied by x^-1 on the device.  The secrets are dropped on return.  Returns (zkey bytes, contribution hash)."""
+    from . import phase2
+    x, s = _random_scalar(entropy), _random_scalar(entropy)
+    g1_s = phase2._scale_one(net, np.concatenate([_fq_mont_limbs(1), _fq_mont_limbs(2)]), s)
+    return phase2.contribute(net, zkey_bytes, x, g1_s, name=name)
+
+
+def _fq_mont_limbs(v: int) -> np.ndarray:
+    x = v * (1 << 256) % formats.FQ_MODULUS
+    return np.array([(x >> (64 * i)) & 0xFFFFFFFFFFFFFFFF for i in range(4)], dtype=np.uint64)
+
+
+def zkey_beacon(net: Net, zkey_bytes: bytes, beacon_hash: bytes, num_iterations_exp: int, name: str | None = None):
+    """snarkjs `zkey beacon`: the final, publicly reproducible contribution from a beacon value (2^num_iterations_exp
+    SHA-256 rounds on the host, so large exponents take long).  Returns (zkey bytes, contribution hash)."""
+    from . import phase2
+    if not 10 <= int(num_iterations_exp) <= 63:
+        raise ValueError("num_iterations_exp must be in 10..63, got %d" % num_iterations_exp)
+    if len(beacon_hash) > 255:
+        raise ValueError("beacon hash longer than 255 bytes")
+    return phase2.beacon(net, zkey_bytes, bytes(beacon_hash), int(num_iterations_exp), name=name)
+
+
+def zkey_verify(net: Net, r1cs_bytes: bytes, ptau_path: str, zkey_bytes: bytes):
+    """snarkjs `zkey verify <r1cs> <ptau> <zkey>`: -> phase2.Phase2Report (ok, failure reasons, per contribution its name,
+    type and hash, and the csHash found in the file, which is not recomputed)."""
+    from . import phase2
+    return phase2.verify(net, r1cs_bytes, ptau_path, zkey_bytes)
+
+
 def zkey_from_r1cs(net: Net, r1: formats.R1CS, pt: formats.PTau) -> bytes:
     """zkey_new on a parsed r1cs and an open ceremony file."""
     from .setup import ptau_key_points

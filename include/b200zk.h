@@ -251,6 +251,13 @@ int b200zk_fr_spmv_dev(b200zk_ctx* ctx, const void* d_ptr, const void* d_idx, co
  * MSM.  Reads ptr to the host and returns once out is complete; temporary device memory: nnz XYZZ points. */
 int b200zk_points_spmv_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_ptr, const void* d_idx, const void* d_val,
                            const void* d_points, size_t n_rows, void* d_out);
+/* One scalar times many points, out[i] = k * points[i] -- the step of a snarkjs `zkey contribute` / `zkey beacon` that
+ * multiplies the L and H sections by delta^-1.  k: 4 u64 limbs, a plain little-endian integer (not Montgomery, not
+ * reduced), host.  Affine in and out (G1 8 / G2 16 u64 limbs, Montgomery), infinity all-zero; out may equal points.
+ * G1 reduces k mod r and uses the GLV split (every G1 point has order r); G2 runs the plain 256-bit ladder on k as given,
+ * so it is right for twist points outside the order-r subgroup too (cofactor clearing).  Enqueued on the slot's stream. */
+int b200zk_points_scale_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_points, size_t n, const uint64_t k[4],
+                            void* d_out);
 /* out[i] = (a[i] s0 + b[i] s1 + c[i] s2) s3   (s: 16 limbs = 4 Montgomery scalars, host). */
 int b200zk_fr_lincomb_dev(b200zk_ctx* ctx, const void* d_a, const void* d_b, const void* d_c, const uint64_t s[16], size_t n,
                           void* d_out);
