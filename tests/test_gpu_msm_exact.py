@@ -1,0 +1,377 @@
+"""The MSM (csrc/msm.cu) against exact answers at every window width, pipeline switch and size up to 2^26.
+
+The bases are generated with known discrete logs, P_i = k_i G (tests/dlog_oracle.py), so MSM(P, s) = (sum_i k_i s_i) G
+is known exactly at any size without running another MSM.  Covered here:
+  - the default configuration at 2^20 .. 2^26 (device-resident, host-staged in parts, fixed-base table), with the
+    generated points themselves spot-checked against k_i G;
+  - every window width B200ZK_MSM_WINDOW = 2..23 on G1 and 2..20 on G2 (read on every call), each with digit-pattern
+    scalar families that put B, B + 1 or 2^c - 1 into every window of k (plain path) or of both GLV halves; at 2^20 the
+    small widths (c <= 8) also run task lengths above 128 and block-level merges of the giant buckets.  Width 24 needs
+    about 33 GB of G1 bucket workspace (10^8 buckets with their task sums) and is left out;
+  - the same sweep without GLV, and every MSM switch (segment length, window groups and their explicit sizes, input
+    parts with empty ones, part weights, thread reduction, long tasks, G2 without GLV), one fresh process each;
+  - adversarial bucket contents: one point n times, P and -P, s and r - s, and +-G bases whose bucket counts make a
+    running sum of the segment reduction hit the identity and equal the bucket it adds (quad and thread reduction);
+  - the W * n >= 2^32 guard, which must refuse before any allocation.
+A failure names the configuration, the family and the size.
+
+Measured on one H100 80GB HBM3 at a 700 W power limit: 279 s for the file, host oracle and subprocess start-up included."""
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+import pytest
+
+from oracle import bn254 as o, layout
+
+import dlog_oracle as dl
+
+pytestmark = pytest.mark.gpu
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HERE = os.path.dirname(os.path.abspath(__file__))
+
+G1_WINDOWS = list(range(2, 24))
+G2_WINDOWS = list(range(2, 21))
+
+
+# ---- helpers ----------------------------------------------------------------------------------------------------
+def _host(t):
+    return t.cpu().numpy().view(np.uint64)
+
+
+def _assert_canonical(sh):
+    """every Montgomery scalar read back from the device is < r"""
+    r = np.array([(o.R >> (64 * i)) & dl.MASK64 for i in range(4)], dtype=np.uint64)
+    lt = np.zeros(sh.shape[0], dtype=bool)
+    eq = np.ones(sh.shape[0], dtype=bool)
+    for i in (3, 2, 1, 0):
+        lt |= eq & (sh[:, i] < r[i])
+        eq &= sh[:, i] == r[i]
+    assert lt.all(), "scalar >= r at %s" % np.nonzero(~lt)[0][:8]
+
+
+def _msm_dev(net, bases, scalars, g2):
+    return net.sum_points_dev(net.msm_dev(bases, scalars, g2=g2), 1, g2=g2)
+
+
+def _check_point(got, want, what):
+    (gp, ginf), (wp, winf) = got, want
+    assert ginf == winf and (np.asarray(gp) == wp).all(), "MSM mismatch: %s (got inf=%s, want inf=%s)" % (what, ginf, winf)
+
+
+def _check_generated(net, seed, n, g2, what, staged=False):
+    """device-generated bases and scalars, exact answer from the logs"""
+    bases = net.generate_g2(seed, n) if g2 else net.generate_g1(seed, n)
+    scalars = net.generate_fr(seed ^ 0x5CA1A4, n)
+    sh = _host(scalars)
+    _assert_canonical(sh)
+    want = dl.expected_msm(seed, sh, g2)
+    got = net.msm(_host(bases), sh, g2=g2) if staged else _msm_dev(net, bases, scalars, g2)
+    _check_point(got, want, what)
+    return bases
+
+
+def _family_scalars(c, glv):
+    fams = dl.digit_families(c, glv)
+    if glv:
+        fams["glv_halves"] = [dl.glv_compose(a, b) for a, b in dl.glv_designed_halves()] + list(_extremes())
+    return fams
+
+
+_EXT = []
+
+
+def _extremes():
+    if not _EXT:
+        _EXT.extend(dl.glv_extremes(1 << 14))
+    return _EXT
+
+
+def _check_families(net, c, g2, glv, what):
+    """one MSM per scalar family on the first generated bases; for GLV the designed halves are confirmed first"""
+    import torch
+    fams = _family_scalars(c, glv)
+    if glv:
+        for a, b in dl.glv_designed_halves():
+            assert dl.glv_decompose(dl.glv_compose(a, b)) == (a, b)
+    seed = 0xFA000000 + c
+    m = max(len(v) for v in fams.values())
+    bases = net.generate_g2(seed, m) if g2 else net.generate_g1(seed, m)
+    for name, ks in fams.items():
+        sc = layout.fr_to_arr(ks)
+        want = dl.expected_msm(seed, sc, g2)
+        got = _msm_dev(net, bases[: len(ks)].contiguous(), torch.from_numpy(sc.view(np.int64)).to(bases.device), g2)
+        _check_point(got, want, "%s family %s" % (what, name))
+
+
+def _sweep_one(net, c, g2, glv, big=True):
+    os.environ["B200ZK_MSM_WINDOW"] = str(c)
+    try:
+        what = "%s c=%d glv=%s" % ("G2" if g2 else "G1", c, glv)
+        for n in (3001, 40000) + (((1 << 20),) if big and c <= 8 else ()):
+            _check_generated(net, 0xC0000000 + 1000 * c + n % 997, n, g2, "%s n=%d" % (what, n))
+        _check_families(net, c, g2, glv, what)
+    finally:
+        del os.environ["B200ZK_MSM_WINDOW"]
+
+
+def _g_arr(g2, neg=False):
+    curve, gen = (o.G2, o.G2_GEN) if g2 else (o.G1, o.G1_GEN)
+    return (layout.g2_to_arr if g2 else layout.g1_to_arr)([curve.neg(gen) if neg else gen])[0]
+
+
+# Bucket counts m_d (multiples of G in bucket d) of the +-G collision case, top bucket of every 8-bucket block first: the
+# running sum of the segment reduction goes 1, 0 (identity: G + (-G)), 1, 2 (doubling: G + G), 2, 4, 0 (4G + (-4G)), 3, ...
+COLLIDE_BLOCK = [1, -1, 1, 1, 0, 2, -4, 3]
+
+
+def collision_counts(B):
+    m = [0] * (B + 1)                                   # m[d], digit d = 1..B
+    for b in range(B):                                   # bucket b holds digit b + 1; blocks of 8 from the top down
+        j = 7 - (b % 8)
+        m[b + 1] = COLLIDE_BLOCK[j]
+    return m
+
+
+def simulate_segments(m, B, seg_len):
+    """(identity hits, doubling hits) of run = run + bucket in k_msm_reduce_segments(_quad), buckets of G multiples"""
+    ident = dbl = 0
+    for lo in range(0, B, seg_len):
+        run = 0
+        for b in range(lo + seg_len - 1, lo - 1, -1):
+            mb = m[b + 1]
+            if run and mb and run + mb == 0:
+                ident += 1
+            if run and run == mb:
+                dbl += 1
+            run += mb
+    return ident, dbl
+
+
+def check_collisions(net, g2, seg_len, c=5):
+    """+-G bases with scalars 1..B at window c: every bucket is a known multiple of G (k = d < 2^c: window 0 only, and the
+    GLV split leaves k2 = 0)."""
+    import torch
+    B = 1 << (c - 1)
+    m = collision_counts(B)
+    ident, dbl = simulate_segments(m, B, seg_len)
+    assert ident > 0 and dbl > 0, (ident, dbl)
+    logs, scal, rows = [], [], []
+    gp, gn = _g_arr(g2), _g_arr(g2, True)
+    for d in range(1, B + 1):
+        for _ in range(abs(m[d])):
+            rows.append(gp if m[d] > 0 else gn)
+            logs.append(1 if m[d] > 0 else -1)
+            scal.append(d)
+    sc = layout.fr_to_arr(scal)
+    want = dl.expected_from_logs(logs, sc, g2)
+    assert want[0].any() and not want[1]
+    os.environ["B200ZK_MSM_WINDOW"] = str(c)
+    try:
+        got = _msm_dev(net, torch.from_numpy(np.stack(rows).view(np.int64)).cuda(), torch.from_numpy(sc.view(np.int64)).cuda(), g2)
+    finally:
+        del os.environ["B200ZK_MSM_WINDOW"]
+    _check_point(got, want, "+-G bucket collisions %s seg_len=%d" % ("G2" if g2 else "G1", seg_len))
+
+
+# ---- 1. size ladder, default configuration ------------------------------------------------------------------------
+def _spot_check_points(bases, seed, g2):
+    n = bases.shape[0]
+    rng = np.random.default_rng(n)
+    cnt = 64 if g2 else 256
+    idx = np.unique(np.concatenate([[0, n - 1], rng.integers(0, n, cnt - 2)]))
+    import torch
+    got = _host(bases[torch.from_numpy(idx).to(bases.device)])
+    logs = dl.base_logs(seed, n)[idx]
+    curve, gen = (o.G2, o.G2_GEN) if g2 else (o.G1, o.G1_GEN)
+    want = (layout.g2_to_arr if g2 else layout.g1_to_arr)([curve.mul(gen, int(k)) for k in logs])
+    assert (got == want).all()
+
+
+@pytest.mark.parametrize("g2,n", [(False, 1 << 20), (False, (1 << 22) + 1), (False, (1 << 23) - 1), (False, 1 << 24),
+                                  (False, 1 << 26), (True, 1 << 20), (True, 1 << 22)])
+def test_size_ladder_device_resident(net, g2, n):
+    import torch
+    seed = 0xA1000000 + n
+    bases = _check_generated(net, seed, n, g2, "default %s n=%d" % ("G2" if g2 else "G1", n))
+    _spot_check_points(bases, seed, g2)
+    del bases
+    torch.cuda.empty_cache()
+
+
+@pytest.mark.parametrize("g2", [False, True])
+@pytest.mark.parametrize("log_n", [20, 22])
+def test_size_ladder_host_staged(net, g2, log_n):
+    """b200zk_msm_g1/g2 on host buffers: five input parts adding into one bucket set"""
+    net.profile(True)
+    net.profile_reset()
+    _check_generated(net, 0xA2000000 + log_n, 1 << log_n, g2, "host-staged log_n=%d" % log_n, staged=True)
+    rep = net.profile_report()
+    net.profile(False)
+    assert rep["msm_digits"]["launches"] == 5                 # one sort per part
+
+
+def test_fixed_base_table_2_22_c20(net):
+    import torch
+    n, seed = 1 << 22, 0xA3000022
+    bases = net.generate_g1(seed, n)
+    scalars = net.generate_fr(seed, n)
+    sh = _host(scalars)
+    _assert_canonical(sh)
+    table = net.msm_table_build(bases, 20)
+    del bases
+    got = net.sum_points_dev(net.msm_table_dev(table, scalars, 20), 1)
+    _check_point(got, dl.expected_msm(seed, sh), "fixed-base table n=2^22 c=20")
+    del table
+    torch.cuda.empty_cache()
+
+
+# ---- 2. window sweep ------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("c", G1_WINDOWS)
+def test_window_sweep_g1(net, c):
+    _sweep_one(net, c, False, True)
+
+
+@pytest.mark.parametrize("c", G2_WINDOWS)
+def test_window_sweep_g2(net, c):
+    _sweep_one(net, c, True, True, big=False)
+
+
+# ---- 3. adversarial bucket contents ---------------------------------------------------------------------------------
+@pytest.mark.parametrize("g2", [False, True])
+def test_one_point_many_times(net, g2):
+    """one point 2^16 + 5 times with one scalar: one giant bucket per window whose tasks all have the same sum"""
+    import torch
+    n, seed = (1 << 16) + 5, 0xA4000001
+    p = net.generate_g2(seed, 1) if g2 else net.generate_g1(seed, 1)
+    s = net.generate_fr(seed, 1)
+    bases, scalars = p.repeat(n, 1).contiguous(), s.repeat(n, 1).contiguous()
+    k0 = dl.base_logs(seed, 1)
+    want = dl.point_from_exponent(dl.exponent(np.repeat(k0, n), _host(scalars)), g2)
+    _check_point(_msm_dev(net, bases, scalars, g2), want, "one point n times")
+    # the same point with alternating P, -P and one scalar, and with s, r - s: both sum to infinity
+    neg = torch.from_numpy(_neg_points(_host(p), g2).view(np.int64)).to(p.device)
+    alt = torch.cat([p, neg]).repeat(n // 2, 1).contiguous()
+    got = _msm_dev(net, alt, s.repeat(alt.shape[0], 1).contiguous(), g2)
+    assert got[1], "P and -P with one scalar must give infinity"
+    sv = layout.arr_to_fr(_host(s))[0]
+    pair = torch.from_numpy(layout.fr_to_arr([sv, o.R - sv]).view(np.int64)).to(p.device)
+    got = _msm_dev(net, bases[: 2 * (n // 2)].contiguous(), pair.repeat(n // 2, 1).contiguous(), g2)
+    assert got[1], "s and r - s on one point must give infinity"
+
+
+def _neg_points(arr, g2):
+    pts = (layout.arr_to_g2 if g2 else layout.arr_to_g1)(arr)
+    curve = o.G2 if g2 else o.G1
+    return (layout.g2_to_arr if g2 else layout.g1_to_arr)([curve.neg(q) for q in pts])
+
+
+@pytest.mark.parametrize("g2", [False, True])
+def test_bucket_running_sum_collisions_quad_reduce(net, g2):
+    check_collisions(net, g2, seg_len=8)                  # small bucket sets: one quad per 8-bucket segment
+
+
+def test_size_guard_refuses_before_launch(net, monkeypatch):
+    """c = 2 gives W = 128 digit windows: 2^25 points make W * n = 2^32 entries, past the 32-bit offsets"""
+    import torch
+    from distributed_groth16_b200 import B200zkError
+    n = 1 << 25
+    bases = net.generate_g1(7, n)
+    scalars = net.generate_fr(7, n)
+    monkeypatch.setenv("B200ZK_MSM_WINDOW", "2")
+    with pytest.raises(B200zkError):
+        net.msm_dev(bases, scalars)
+    del bases, scalars
+    torch.cuda.empty_cache()
+
+
+# ---- 4. switches: one fresh process each ------------------------------------------------------------------------------
+def run_switch_checks(spec):
+    """Body of one switch subprocess: G1 and G2 at two sizes, device-resident and host-staged, the +-G collision case, and
+    the effect the switch must have (window groups, input parts) read from the profile."""
+    import torch
+    from distributed_groth16_b200 import Net
+    net = Net(0)
+    net.use_torch_stream(0)
+    if spec.get("sweep_glv0"):
+        for c in G1_WINDOWS:
+            _sweep_one(net, c, False, False)
+        torch.cuda.synchronize()
+        net.close()
+        return
+    if "window" in spec:
+        os.environ["B200ZK_MSM_WINDOW"] = str(spec["window"])
+    for g2 in (False, True):
+        for n in spec.get("sizes", (3001, (1 << 17) + 3)):
+            what = "%s %s n=%d" % (spec["name"], "G2" if g2 else "G1", n)
+            net.profile(True)
+            net.profile_reset()
+            _check_generated(net, 0xB0000000 + n, n, g2, what + " device")
+            rep = net.profile_report()
+            if "groups" in spec and not g2:
+                assert rep["msm_combine"]["launches"] == spec["groups"], (what, rep["msm_combine"])
+            net.profile_reset()
+            _check_generated(net, 0xB1000000 + n, n, g2, what + " host-staged", staged=True)
+            rep = net.profile_report()
+            if "parts" in spec:
+                assert rep["msm_digits"]["launches"] == min(spec["parts"], n), (what, rep["msm_digits"])
+            net.profile(False)
+    for n in spec.get("tiny", ()):
+        for g2 in (False, True):
+            _check_generated(net, 0xB2000000 + n, n, g2, "%s tiny n=%d host-staged" % (spec["name"], n), staged=True)
+    os.environ.pop("B200ZK_MSM_WINDOW", None)
+    for g2 in (False, True):
+        check_collisions(net, g2, spec.get("seg_len", 8))
+    torch.cuda.synchronize()
+    net.close()
+
+
+# seg_len: the segment length the +-G collision case (c = 5, B = 16) runs with under the switch; a forced length above B is
+# ignored there, and the small bucket set keeps its 8-bucket quads
+SWITCHES = [
+    ({"B200ZK_MSM_SEG": "2"}, {"seg_len": 2}),
+    ({"B200ZK_MSM_SEG": "4"}, {"seg_len": 4}),
+    ({"B200ZK_MSM_SEG": "32"}, {"seg_len": 8}),
+    ({"B200ZK_MSM_SEG": "64"}, {"seg_len": 8}),
+    ({"B200ZK_MSM_GROUPS": "2"}, {"groups": 2}),
+    ({"B200ZK_MSM_GROUPS": "3"}, {"groups": 3}),
+    ({"B200ZK_MSM_GROUPS": "7"}, {"groups": 7}),
+    ({"B200ZK_MSM_GROUP_UNITS": "7,1"}, {"window": 16, "groups": 2}),
+    ({"B200ZK_MSM_GROUP_UNITS": ",".join(["1"] * 10)}, {"window": 13, "groups": 10}),
+    ({"B200ZK_MSM_PARTS": "2"}, {"parts": 2}),
+    ({"B200ZK_MSM_PARTS": "7"}, {"parts": 7}),
+    ({"B200ZK_MSM_PARTS": "16"}, {"parts": 16, "tiny": (1, 5, 15)}),
+    ({"B200ZK_MSM_PART_WEIGHTS": "1,3"}, {"parts": 2}),
+    ({"B200ZK_MSM_PART_WEIGHTS": "5,1,1"}, {"parts": 3}),
+    ({"B200ZK_MSM_QUAD_REDUCE": "0"}, {"seg_len": 16}),
+    ({"B200ZK_MSM_SHORT_TASKS": "0"}, {}),
+    ({"B200ZK_MSM_GLV_G2": "0"}, {}),
+    ({"B200ZK_MSM_GLV": "0"}, {"sweep_glv0": True}),
+]
+
+
+def _switch_id(env):
+    return "-".join("%s=%s" % (k.replace("B200ZK_MSM_", "").lower(), v if len(v) < 8 else "1x10") for k, v in env.items())
+
+
+SCRIPT = r"""
+import json, sys
+sys.path.insert(0, %r)
+sys.path.insert(0, %r)
+import test_gpu_msm_exact as t
+t.run_switch_checks(json.loads(%r))
+print("switch checks ok")
+"""
+
+
+@pytest.mark.parametrize("env,spec", SWITCHES, ids=[_switch_id(e) for e, _ in SWITCHES])
+def test_switch_matrix(env, spec):
+    spec = dict(spec, name=_switch_id(env))
+    e = dict(os.environ)
+    e.pop("B200ZK_MSM_WINDOW", None)
+    e.update(env)
+    r = subprocess.run([sys.executable, "-c", SCRIPT % (ROOT, HERE, json.dumps(spec))], env=e, capture_output=True, text=True,
+                       timeout=900, cwd=ROOT)
+    assert r.returncode == 0 and "switch checks ok" in r.stdout, r.stdout[-2000:] + r.stderr[-4000:]
