@@ -720,6 +720,15 @@ int b200zk_points_scale_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_p
     B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
     return points_scale_dev(ctx, sl, g2, d_points, n, k, d_out);
 }
+int b200zk_points_intt_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_in, unsigned log_n, void* d_out) {
+    if (!ctx) return B200ZK_ERR_ARG;
+    if (!valid_slot(stream) || !d_in || !d_out) return set_error(ctx, B200ZK_ERR_ARG, "points_intt: null pointer or bad stream slot");
+    if (log_n > 28) return set_error(ctx, B200ZK_ERR_DOMAIN, "points_intt: log_n > 28 (the two-adicity of Fr)");
+    Slot& sl = ctx->slots[stream];
+    std::lock_guard<std::mutex> g(sl.mu);
+    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
+    return points_intt_dev(ctx, sl, g2, d_in, log_n, d_out);
+}
 int b200zk_fr_lincomb_dev(b200zk_ctx* ctx, const void* d_a, const void* d_b, const void* d_c, const uint64_t s[16], size_t n,
                           void* d_out) {
     if (!ctx || !s || (n && (!d_a || !d_b || !d_c || !d_out))) return B200ZK_ERR_ARG;

@@ -71,18 +71,21 @@ __global__ void __launch_bounds__(128) k_fixed_base_mul(const affine_t<F>* table
     sts(out + i, xyzz_t<F>::to_affine(acc));
 }
 
-// out[i] = scale * base^i
-__global__ void k_fr_powers(const Fr* consts /* base, scale */, size_t n, Fr* out) {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    Fr b = consts[0], res = consts[1];
-    uint64_t e = i;
+// res * b^e by square-and-multiply
+__device__ __forceinline__ Fr fr_pow_scaled(Fr b, Fr res, uint64_t e) {
     while (e) {
         if (e & 1) res = Fr::mul(res, b);
         b = Fr::sqr(b);
         e >>= 1;
     }
-    sts(out + i, res);
+    return res;
+}
+
+// out[i] = scale * base^i
+__global__ void k_fr_powers(const Fr* consts /* base, scale */, size_t n, Fr* out) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    sts(out + i, fr_pow_scaled(consts[0], consts[1], i));
 }
 
 // out[r] = sum_k val[k] * x[idx[k]],  k in [ptr[r], ptr[r+1])
@@ -346,17 +349,22 @@ __device__ F block_batch_inv(const F& a, F* pre, F* suf, F* tot) {
     return r;
 }
 
-// table entry j of this thread, stored as 4 uint4 per point, [entry][chunk][thread]: conflict-free shared accesses
-__device__ __forceinline__ void scale_tab_put(uint4* tab, int j, const affine_t<Fq>& p) {
+// table entry j of this thread, stored as C = sizeof(point) / 16 uint4 per point, [entry][chunk][thread]: conflict-free
+// shared accesses for a block of B threads
+template <class F, int B>
+__device__ __forceinline__ void tab_put(uint4* tab, int j, const affine_t<F>& p) {
+    constexpr int C = sizeof(affine_t<F>) / 16;
     const uint4* s = reinterpret_cast<const uint4*>(&p);
 #pragma unroll
-    for (int c = 0; c < 4; ++c) tab[(j * 4 + c) * SCALE_BLOCK + threadIdx.x] = s[c];
+    for (int c = 0; c < C; ++c) tab[(j * C + c) * B + threadIdx.x] = s[c];
 }
-__device__ __forceinline__ affine_t<Fq> scale_tab_get(const uint4* tab, int j) {
-    affine_t<Fq> p;
+template <class F, int B>
+__device__ __forceinline__ affine_t<F> tab_get(const uint4* tab, int j) {
+    constexpr int C = sizeof(affine_t<F>) / 16;
+    affine_t<F> p;
     uint4* d = reinterpret_cast<uint4*>(&p);
 #pragma unroll
-    for (int c = 0; c < 4; ++c) d[c] = tab[(j * 4 + c) * SCALE_BLOCK + threadIdx.x];
+    for (int c = 0; c < C; ++c) d[c] = tab[(j * C + c) * B + threadIdx.x];
     return p;
 }
 
@@ -369,7 +377,7 @@ __global__ void __launch_bounds__(SCALE_BLOCK) k_points_scale_g1(const __grid_co
     const bool inf = P.is_inf();
     // the odd multiples, (2j + 1) P = (2j - 1) P + 2P in XYZZ, each normalised as it is made (one block-batched
     // inverse per entry: only the running entry and 2P are live)
-    scale_tab_put(tab, 0, P);
+    tab_put<Fq, SCALE_BLOCK>(tab, 0, P);
     {
         const xyzz_t<Fq> two = inf ? xyzz_t<Fq>::identity() : xyzz_t<Fq>::dbl_affine(P.x, P.y);
         xyzz_t<Fq> odd = xyzz_t<Fq>::from_affine(P);
@@ -383,7 +391,7 @@ __global__ void __launch_bounds__(SCALE_BLOCK) k_points_scale_g1(const __grid_co
                 a.x = Fq::mul(odd.x, izz);
                 a.y = Fq::mul(odd.y, izzz);
             }
-            scale_tab_put(tab, j, a);
+            tab_put<Fq, SCALE_BLOCK>(tab, j, a);
         }
     }
     Fq beta;
@@ -395,9 +403,9 @@ __global__ void __launch_bounds__(SCALE_BLOCK) k_points_scale_g1(const __grid_co
         for (int b = dg.top; b >= 0; --b) {
             acc = xyzz_t<Fq>::dbl(acc);
             const int d1 = dg.d[0][b], d2 = dg.d[1][b];
-            if (d1) xyzz_t<Fq>::madd(acc, scale_tab_get(tab, (d1 < 0 ? -d1 : d1) >> 1), d1 < 0);
+            if (d1) xyzz_t<Fq>::madd(acc, tab_get<Fq, SCALE_BLOCK>(tab, (d1 < 0 ? -d1 : d1) >> 1), d1 < 0);
             if (d2) {
-                affine_t<Fq> q = scale_tab_get(tab, (d2 < 0 ? -d2 : d2) >> 1);
+                affine_t<Fq> q = tab_get<Fq, SCALE_BLOCK>(tab, (d2 < 0 ? -d2 : d2) >> 1);
                 q.x = Fq::mul(q.x, beta);                                          // phi(jP) = (beta x, y)
                 xyzz_t<Fq>::madd(acc, q, d2 < 0);
             }
@@ -492,6 +500,249 @@ int points_scale_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_points, si
             dg, reinterpret_cast<const affine_t<Fq>*>(d_points), n, reinterpret_cast<affine_t<Fq>*>(d_out));
     }
     return check_launch(ctx, "k_points_scale_g1");
+}
+
+// ---- inverse NTT over points: out[i] = n^-1 sum_j w_n^(-i j) in[j]  (snarkjs `powersoftau prepare phase2`) ----------
+// The Lagrange levels of a prepared Powers-of-Tau file; orchestration in groth16/ptau.py.  Radix-2 decimation in time:
+// one bit-reversal pass, then log_n in-place butterfly passes over global memory, then n^-1 by points_scale_dev.  Each
+// butterfly costs one full scalar multiplication (w^-j P) against a handful of point additions, so the passes are plain
+// and the work per thread is made uniform instead:
+//   * the twiddles w_n^-i, i < n / 2, are computed once per transform on the device, split with GLV (glv.cuh; on G2
+//     phi = (beta^2 x, y), right for points of the order-r subgroup) and recoded into 32 signed 4-bit windows per half,
+//     digits in [-7, 8] (|k1|, |k2| < 2^127 leave no carry out of the top window).  Every thread runs the same
+//     32 x (4 doublings + 2 mixed additions) from a per-thread table P, 2P, .., 8P in shared memory (normalised with
+//     block-batched inversions like points_scale);
+//   * butterflies are numbered twiddle-major, so consecutive threads share a twiddle whenever a pass has >= 32
+//     butterflies per twiddle: a warp reads one digit string, and the blocks whose twiddle is w^0 skip the product;
+//   * U + wP and U - wP share one block-batched inversion (of the product of their ZZZ).
+constexpr int INTT_WINDOWS = 32;
+constexpr int INTT_TAB = 8;               // P, 2P, .., 8P
+constexpr int INTT_BLOCK_G1 = 64;
+constexpr int INTT_BLOCK_G2 = 32;         // the G2 table (8 x 128 B per thread) fills 32 KB of shared memory at 32 threads
+
+struct __align__(16) TwiddleDigits {
+    int8_t d[2][INTT_WINDOWS];            // d[h][w]: window w (weight 16^w) of k1 (h = 0) / k2 (h = 1), signs folded in
+};
+
+// digits of w_n^-i for i < count
+__global__ void k_intt_twiddle_digits(unsigned log_n, size_t count, TwiddleDigits* out) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    Fr w;
+#pragma unroll
+    for (int l = 0; l < 8; ++l) w.l[l] = FrParams::root28_inv(l);
+    for (unsigned k = log_n; k < 28; ++k) w = Fr::sqr(w);            // the root the field NTT uses (ntt.cu k_plan_consts)
+    const Fr t = Fr::from_mont(fr_pow_scaled(w, Fr::one(), i));
+    const GlvSplit sp = glv_decompose(t.l);
+    TwiddleDigits dg;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const uint32_t* k = h ? sp.k2 : sp.k1;
+        const bool neg = h ? sp.neg2 : sp.neg1;
+        int carry = 0;
+#pragma unroll
+        for (int q = 0; q < INTT_WINDOWS; ++q) {
+            int v = (int)((k[q >> 3] >> ((q & 7) * 4)) & 15) + carry;
+            carry = v > 8;
+            if (carry) v -= 16;
+            dg.d[h][q] = (int8_t)(neg ? -v : v);
+        }
+    }
+    sts(out + i, dg);
+}
+
+template <class F> __device__ __forceinline__ void apply_endo(affine_t<F>& p);
+template <> __device__ __forceinline__ void apply_endo<Fq>(affine_t<Fq>& p) {
+    Fq b;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) b.l[i] = GlvParams::beta(i);
+    p.x = Fq::mul(p.x, b);
+}
+template <> __device__ __forceinline__ void apply_endo<Fq2>(affine_t<Fq2>& p) {
+    Fq b;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) b.l[i] = GlvParams::beta_g2(i);
+    p.x.c0 = Fq::mul(p.x.c0, b);
+    p.x.c1 = Fq::mul(p.x.c1, b);
+}
+
+// affine form of a given 1 / a.zzz
+template <class F>
+__device__ __forceinline__ affine_t<F> affine_with(const xyzz_t<F>& a, const F& izzz) {
+    affine_t<F> r = affine_t<F>::infinity();
+    if (!a.is_inf()) {
+        const F izz = F::sqr(F::mul(izzz, a.zz));
+        r.x = F::mul(a.x, izz);
+        r.y = F::mul(a.y, izzz);
+    }
+    return r;
+}
+
+// out[i] = in[bitrev(i)]; each pair is handled by one thread that reads both before writing, so out may equal in
+template <class F>
+__global__ void k_points_bitrev(const affine_t<F>* in, affine_t<F>* out, unsigned log_n) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >> log_n) return;
+    const size_t r = log_n ? (size_t)(__brevll((unsigned long long)i) >> (64 - log_n)) : 0;
+    if (r < i) return;
+    const affine_t<F> x = lds(in + i), y = lds(in + r);
+    sts(out + i, y);
+    if (r != i) sts(out + r, x);
+}
+
+// pass with half-size m = 2^log_m: butterfly t = (j, g), j = t >> lg, g = t mod 2^lg (lg = log2(n / 2m)), on the
+// elements g 2m + j and g 2m + j + m with twiddle w_2m^-j = w_n^-(j << lg)
+template <class F, int B>
+__global__ void __launch_bounds__(B) k_points_intt_pass(affine_t<F>* a, const TwiddleDigits* __restrict__ tw, unsigned log_n,
+                                                        unsigned log_m) {
+    constexpr int C = sizeof(affine_t<F>) / 16;
+    __shared__ uint4 tab[INTT_TAB * C * B];
+    __shared__ F pre[B], suf[B], tot;
+    const unsigned lg = log_n - 1 - log_m;
+    const size_t t = (size_t)blockIdx.x * B + threadIdx.x;
+    const bool live = (t >> (log_n - 1)) == 0;
+    const size_t j = t >> lg;
+    const size_t ia = ((t & (((size_t)1 << lg) - 1)) << (log_m + 1)) + j, ib = ia + ((size_t)1 << log_m);
+    bool mul = false;
+    if (!__syncthreads_and(!live || j == 0)) {                           // block-uniform
+        // the table is built from shared memory copies only: P and the products stay out of registers during the loop
+        {
+            const affine_t<F> P = live ? lds(a + ib) : affine_t<F>::infinity();
+            mul = live && j != 0 && !P.is_inf();
+            tab_put<F, B>(tab, 0, P);
+        }
+        xyzz_t<F> run = xyzz_t<F>::identity();
+#pragma unroll 1
+        for (int e = 1; e < INTT_TAB; ++e) {                             // (e + 1) P
+            if (mul) {
+                const affine_t<F> P = tab_get<F, B>(tab, 0);
+                if (e == 1) run = xyzz_t<F>::dbl_affine(P.x, P.y);
+                else xyzz_t<F>::madd(run, P, false);
+            }
+            const F izzz = block_batch_inv<F, B>(mul ? run.zzz : F::one(), pre, suf, &tot);
+            tab_put<F, B>(tab, e, mul ? affine_with(run, izzz) : affine_t<F>::infinity());
+        }
+    }
+    xyzz_t<F> prod;
+    if (mul) {
+        const int8_t* d = tw[j << lg].d[0];
+        prod = xyzz_t<F>::identity();
+#pragma unroll 1
+        for (int q = INTT_WINDOWS - 1; q >= 0; --q) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) prod = xyzz_t<F>::dbl(prod);
+            const int d1 = d[q], d2 = d[INTT_WINDOWS + q];
+            if (d1) xyzz_t<F>::madd(prod, tab_get<F, B>(tab, (d1 < 0 ? -d1 : d1) - 1), d1 < 0);
+            if (d2) {
+                affine_t<F> p = tab_get<F, B>(tab, (d2 < 0 ? -d2 : d2) - 1);
+                apply_endo(p);
+                xyzz_t<F>::madd(prod, p, d2 < 0);
+            }
+        }
+    } else {
+        prod = xyzz_t<F>::from_affine(live ? lds(a + ib) : affine_t<F>::infinity());      // w^0 P, or P = infinity
+    }
+    // T = w P in affine form, then U + T and U - T as affine additions that share one inverse: the denominator is
+    // x_T - x_U, or 2 y_U when T = +-U (then one result is infinity and the other 2U), or 1 when T or U is infinity
+    const affine_t<F> T = affine_with(prod, block_batch_inv<F, B>(prod.is_inf() ? F::one() : prod.zzz, pre, suf, &tot));
+    const affine_t<F> U = live ? lds(a + ia) : affine_t<F>::infinity();
+    const bool edge = T.is_inf() || U.is_inf();
+    const F dx = F::sub(T.x, U.x);
+    const bool dbl = !edge && dx.is_zero();
+    const F inv = block_batch_inv<F, B>(edge ? F::one() : dbl ? F::dbl(U.y) : dx, pre, suf, &tot);
+    if (!live) return;
+    affine_t<F> s, df;
+    if (T.is_inf()) {
+        s = U;
+        df = U;
+    } else if (U.is_inf()) {
+        s = T;
+        df = T;
+        df.y = F::neg(T.y);
+    } else {
+        auto finish = [&](const F& lam, const F& x_other) {                  // U + Q from the slope, x_Q = x_other
+            affine_t<F> r;
+            r.x = F::sub(F::sub(F::sqr(lam), U.x), x_other);
+            r.y = F::sub(F::mul(lam, F::sub(U.x, r.x)), U.y);
+            return r;
+        };
+        if (dbl) {                                                           // T = U or T = -U
+            const F x2 = F::sqr(U.x);
+            const affine_t<F> two = finish(F::mul(F::add(F::dbl(x2), x2), inv), U.x);
+            const bool same = F::sub(T.y, U.y).is_zero();
+            s = same ? two : affine_t<F>::infinity();
+            df = same ? affine_t<F>::infinity() : two;
+        } else {
+            s = finish(F::mul(F::sub(T.y, U.y), inv), T.x);
+            df = finish(F::mul(F::neg(F::add(T.y, U.y)), inv), T.x);
+        }
+    }
+    sts(a + ia, s);
+    sts(a + ib, df);
+}
+
+template <class F, int B>
+static int points_intt_impl(b200zk_ctx* ctx, Slot& sl, int g2, const affine_t<F>* d_in, unsigned log_n, affine_t<F>* d_out) {
+    cudaStream_t st = sl.stream;
+    const size_t n = (size_t)1 << log_n, half = n >> 1;
+    TwiddleDigits* tw = nullptr;
+    if (half) {
+        const cudaError_t e = cudaMalloc(&tw, half * sizeof(TwiddleDigits));
+        if (e != cudaSuccess) {
+            cudaGetLastError();                                           // nothing was launched: leave no error behind
+            char b[256];
+            snprintf(b, sizeof(b), "points_intt: the twiddle digits of 2^%u points (%zu MB of device memory) do not fit: %s",
+                     log_n, half * sizeof(TwiddleDigits) >> 20, cudaGetErrorString(e));
+            return set_error(ctx, e == cudaErrorMemoryAllocation ? B200ZK_ERR_OOM : B200ZK_ERR_CUDA, b);
+        }
+    }
+    auto run = [&]() -> int {
+        {
+            LaunchScope ls(ctx, st, "points_intt_bitrev");
+            k_points_bitrev<F><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_in, d_out, log_n);
+        }
+        B2_TRY(check_launch(ctx, "k_points_bitrev"));
+        if (!half) return B200ZK_OK;
+        {
+            LaunchScope ls(ctx, st, "points_intt_twiddles");
+            k_intt_twiddle_digits<<<(unsigned)((half + 255) / 256), 256, 0, st>>>(log_n, half, tw);
+        }
+        B2_TRY(check_launch(ctx, "k_intt_twiddle_digits"));
+        for (unsigned log_m = 0; log_m < log_n; ++log_m) {
+            {
+                LaunchScope ls(ctx, st, g2 ? "points_intt_pass_g2" : "points_intt_pass_g1");
+                k_points_intt_pass<F, B><<<(unsigned)((half + B - 1) / B), B, 0, st>>>(d_out, tw, log_n, log_m);
+            }
+            B2_TRY(check_launch(ctx, "k_points_intt_pass"));
+        }
+        // n^-1 mod r = r - (r - 1) / n  (n divides r - 1)
+        uint32_t q[8], ninv32[8];
+        for (int i = 0; i < 8; ++i) q[i] = FrParams::mod(i) & (i ? ~0u : ~1u);
+        for (int i = 0; i < 8; ++i) {
+            const uint64_t hi = i < 7 ? (uint64_t)q[i + 1] : 0;
+            q[i] = (uint32_t)((((hi << 32) | q[i]) >> log_n));
+        }
+        int64_t br = 0;
+        for (int i = 0; i < 8; ++i) {
+            const int64_t v = (int64_t)FrParams::mod(i) - (int64_t)q[i] + br;
+            ninv32[i] = (uint32_t)v;
+            br = v >> 32;
+        }
+        uint64_t ninv[4];
+        for (int i = 0; i < 4; ++i) ninv[i] = (uint64_t)ninv32[2 * i] | ((uint64_t)ninv32[2 * i + 1] << 32);
+        return points_scale_dev(ctx, sl, g2, d_out, n, ninv, d_out);
+    };
+    const int rc = run();
+    const cudaError_t e = cudaStreamSynchronize(st);                     // the twiddle digits are freed below
+    cudaFree(tw);
+    if (rc != B200ZK_OK) return rc;
+    B2_CUDA_OK(ctx, e);
+    return B200ZK_OK;
+}
+
+int points_intt_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_in, unsigned log_n, void* d_out) {
+    return g2 ? points_intt_impl<Fq2, INTT_BLOCK_G2>(ctx, sl, 1, (const affine_t<Fq2>*)d_in, log_n, (affine_t<Fq2>*)d_out)
+              : points_intt_impl<Fq, INTT_BLOCK_G1>(ctx, sl, 0, (const affine_t<Fq>*)d_in, log_n, (affine_t<Fq>*)d_out);
 }
 
 }  // namespace b200zk

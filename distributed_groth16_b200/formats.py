@@ -184,12 +184,19 @@ class PTau:
     Layout (restated from snarkjs; points are Montgomery little-endian affine, infinity all-zero): section 1 = n8, q,
     power, ceremonyPower; 4 / 5 / 6 = alpha tau^i G1, beta tau^i G1, beta G2 (their first points are alpha_1, beta_1,
     beta_2); 12 / 13 / 14 / 15 = the Lagrange bases L G1, L G2, alpha L G1, beta L G1 of every domain 2^k, level k starting
-    at point 2^k - 1 -- levels 0..power + 1 in section 12, 0..power in the others."""
+    at point 2^k - 1 -- levels 0..power + 1 in section 12, 0..power in the others.
+
+    prepared=False opens the output of a phase-1 ceremony instead (snarkjs `powersoftau prepare phase2` input): sections
+    2-7 must be present and as long as the power requires (2 = tau^i G1, 2^(power+1) - 1 points; 3 = tau^i G2, 4, 5:
+    2^power points each; 6: one point; 7 = the contribution records, any length), the power must be at most 27 (the top
+    Lagrange level, power + 1, must fit the 2^28 domain of Fr), and sections 12-15 are neither required nor read."""
 
     _LAGRANGE = {12: 8, 13: 16, 14: 8, 15: 8}      # section -> u64 limbs per point
+    MAX_UNPREPARED_POWER = 27
 
-    def __init__(self, path: str):
+    def __init__(self, path: str, prepared: bool = True):
         import mmap
+        self._prepared = prepared
         self._f = open(path, "rb")
         try:
             size = self._f.seek(0, 2)
@@ -226,6 +233,16 @@ class PTau:
         if int.from_bytes(mm[o1 + 4:o1 + 4 + n8], "little") != FQ_MODULUS:
             raise FormatError("ptau is not over BN254 (wrong q)")
         self.power, self.ceremony_power = struct.unpack_from("<II", mm, o1 + 4 + n8)
+        if not self._prepared:
+            if self.power > self.MAX_UNPREPARED_POWER:
+                raise FormatError("ptau power %d above %d: its top Lagrange level (2^%d points) exceeds the 2^28 domain of Fr"
+                                  % (self.power, self.MAX_UNPREPARED_POWER, self.power + 1))
+            for sid, ln in self.tau_section_bytes(self.power).items():
+                if sid not in secs:
+                    raise FormatError("ptau section %d missing" % sid)
+                if secs[sid][1] < ln:
+                    raise FormatError("ptau section %d too short for power %d (%d < %d bytes)" % (sid, self.power, secs[sid][1], ln))
+            return
         missing = [sid for sid in (12, 13, 14, 15) if sid not in secs]
         if missing:
             raise FormatError("ptau has no Lagrange sections %s: it is not prepared for phase 2 (run snarkjs powersoftau "
@@ -238,6 +255,32 @@ class PTau:
                 raise FormatError("ptau section %d missing" % sid)
             if secs[sid][1] < ln:
                 raise FormatError("ptau section %d too short for power %d (%d < %d bytes)" % (sid, self.power, secs[sid][1], ln))
+
+    @staticmethod
+    def tau_section_bytes(power: int) -> dict:
+        """Least length in bytes of sections 2-7 for a ceremony of this power."""
+        n = 1 << power
+        return {2: (2 * n - 1) * 64, 3: n * 128, 4: n * 64, 5: n * 64, 6: 128, 7: 0}
+
+    @classmethod
+    def lagrange_section_bytes(cls, power: int) -> dict:
+        """Length in bytes of sections 12-15 of a prepared file of this power (levels 0..power + 1 in 12, 0..power in the
+        others: 2^(top + 1) - 1 points)."""
+        return {sid: ((1 << (power + (2 if sid == 12 else 1))) - 1) * w * 8 for sid, w in cls._LAGRANGE.items()}
+
+    def section_span(self, sid: int):
+        """(byte offset, length) of section sid in the file."""
+        return self._secs[sid]
+
+    def section_chunks(self, sid: int, chunk: int = 1 << 26):
+        """The bytes of section sid, in copies of at most `chunk` bytes."""
+        off, ln = self._secs[sid]
+        for lo in range(0, ln, chunk):
+            yield self._mm[off + lo:off + min(ln, lo + chunk)]
+
+    def points(self, sid: int, first: int, count: int, width: int) -> np.ndarray:
+        """count points of section sid from point `first` as (count, width) u64 limbs (width 8: G1, 16: G2)."""
+        return self._points(sid, first, count, width)
 
     def _points(self, sid: int, first: int, count: int, width: int) -> np.ndarray:
         off = self._secs[sid][0] + first * width * 8
@@ -282,6 +325,66 @@ def read_ptau(path: str) -> PTau:
     """Open a prepared .ptau (memory-mapped; see PTau).  Raises FormatError for a file that is not a BN254 ptau, is not
     prepared for phase 2 or whose sections are shorter than its stated power."""
     return PTau(path)
+
+
+class PreparedPTauWriter:
+    """Streams the output of snarkjs `powersoftau prepare phase2` for an open ceremony `src` (a PTau, prepared or not) to
+    `path`: 11 sections in the order 1, 2-7, 12-15.  Section 1 is restated as (n8, q, power, ceremonyPower = power) -- what
+    snarkjs' writePTauHeader(curve, power) writes as far as is known here; sections 2-7 are copied byte for byte (section 7
+    with any contribution records).  The Lagrange sections follow level by level through write_level(), in the order
+    `levels()` lists, so the host holds one level at a time; every length is known in advance and checked."""
+
+    def __init__(self, path: str, src: PTau):
+        self.power = src.power
+        self._lengths = PTau.lagrange_section_bytes(self.power)
+        self._order = [(sid, k) for sid in (12, 13, 14, 15) for k in range(self.power + (2 if sid == 12 else 1))]
+        self._next = 0
+        self._f = open(path, "wb")
+        try:
+            s1 = struct.pack("<I", 32) + FQ_MODULUS.to_bytes(32, "little") + struct.pack("<II", self.power, self.power)
+            self._f.write(b"ptau" + struct.pack("<II", 1, 11) + struct.pack("<IQ", 1, len(s1)) + s1)
+            for sid in (2, 3, 4, 5, 6, 7):
+                self._f.write(struct.pack("<IQ", sid, src.section_span(sid)[1]))
+                for part in src.section_chunks(sid):
+                    self._f.write(part)
+        except BaseException:
+            self._f.close()
+            raise
+
+    def levels(self) -> list:
+        """[(section, level)] in file order."""
+        return list(self._order)
+
+    def write_level(self, sid: int, level: int, data) -> None:
+        """Level `level` of Lagrange section sid: 2^level points (8 or 16 u64 limbs each) as bytes or a u64 array."""
+        if self._next >= len(self._order) or self._order[self._next] != (sid, level):
+            raise ValueError("Lagrange level (%d, %d) out of order: expected %r" % (
+                sid, level, self._order[self._next] if self._next < len(self._order) else None))
+        data = memoryview(np.ascontiguousarray(data) if isinstance(data, np.ndarray) else data).cast("B")
+        want = (1 << level) * PTau._LAGRANGE[sid] * 8
+        if data.nbytes != want:
+            raise ValueError("Lagrange level (%d, %d) has %d bytes, expected %d" % (sid, level, data.nbytes, want))
+        if level == 0:
+            self._f.write(struct.pack("<IQ", sid, self._lengths[sid]))
+        self._f.write(data)
+        self._next += 1
+
+    def close(self) -> None:
+        """Finish the file; raises ValueError (and leaves it truncated) if levels are missing."""
+        f, self._f = self._f, None
+        if f is None:
+            return
+        f.close()
+        if self._next != len(self._order):
+            raise ValueError("prepared ptau incomplete: %d of %d Lagrange levels written" % (self._next, len(self._order)))
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        f, self._f = self._f, None
+        if f is not None:
+            f.close()
 
 
 @dataclass

@@ -25,6 +25,20 @@ def load_zkey(net: Net, zkey_bytes: bytes):
     return pk, mats, zk
 
 
+def ptau_prepare_phase2(net: Net, src_path: str, dst_path: str) -> None:
+    """snarkjs `powersoftau prepare phase2 <src> <dst>` on the GPU: the Lagrange sections 12-15 that zkey_new reads, computed
+    from the tau-power sections of a phase-1 ceremony file and streamed to dst_path (ptau.prepare_phase2)."""
+    from . import ptau
+    ptau.prepare_phase2(net, src_path, dst_path)
+
+
+def ptau_check_lagrange(net: Net, ptau_path: str):
+    """The Lagrange part of snarkjs `powersoftau verify` on a prepared file: -> ptau.LagrangeReport (ok, one failure line
+    per section and level that does not check).  Needs no toxic waste."""
+    from . import ptau
+    return ptau.check_lagrange(net, ptau_path)
+
+
 def zkey_new(net: Net, r1cs_bytes: bytes, ptau_path: str) -> bytes:
     """snarkjs `zkey new <r1cs> <ptau>` on the GPU (scripts/phase2_proving_key.sh, ark-circom/test-vectors/complex-circuit/
     build.sh:11): the .zkey bytes of the circuit's proving key from a prepared Powers-of-Tau file.  The key has delta = 1

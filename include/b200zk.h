@@ -258,6 +258,14 @@ int b200zk_points_spmv_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_pt
  * so it is right for twist points outside the order-r subgroup too (cofactor clearing).  Enqueued on the slot's stream. */
 int b200zk_points_scale_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_points, size_t n, const uint64_t k[4],
                             void* d_out);
+/* out[i] = n^-1 * sum_j omega_n^(-i j) * in[j],  n = 2^log_n: the Lagrange basis in the exponent that snarkjs
+ * `powersoftau prepare phase2` writes.  Affine Montgomery points in natural order, infinity all-zero (also as input).
+ * omega_n is the root of unity of b200zk_ntt_fr_dev, so points_intt(k_j G) == fixed_base_mul(ntt(k, inverse)) point for
+ * point.  g2 = 0: G1 (8 u64 limbs per point), 1: G2 (16); the points must lie in the order-r subgroup (every G1 point
+ * does; the GLV split is used on both groups).  d_out may equal d_in (in place); no other overlap is allowed.
+ * Temporary device memory: 2^(log_n - 1) x 64 bytes, allocated before anything is launched (B200ZK_ERR_OOM with a message
+ * when it does not fit).  log_n > 28: B200ZK_ERR_DOMAIN; a null pointer: B200ZK_ERR_ARG.  Returns once out is complete. */
+int b200zk_points_intt_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_in, unsigned log_n, void* d_out);
 /* out[i] = (a[i] s0 + b[i] s1 + c[i] s2) s3   (s: 16 limbs = 4 Montgomery scalars, host). */
 int b200zk_fr_lincomb_dev(b200zk_ctx* ctx, const void* d_a, const void* d_b, const void* d_c, const uint64_t s[16], size_t n,
                           void* d_out);
