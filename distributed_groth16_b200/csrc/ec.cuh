@@ -183,15 +183,18 @@ struct xyzz_t {
 
     B2_HD static xyzz_t neg(const xyzz_t& a) { xyzz_t r = a; r.y = F::neg(a.y); return r; }
 
-    // canonical affine (x = X/ZZ, y = Y/ZZZ); infinity -> (0,0)
-    B2_HD_NI static affine_t<F> to_affine(const xyzz_t& a) {
-        if (a.is_inf()) return affine_t<F>::infinity();
-        F izzz = F::inv(a.zzz);                      // 1/ZZZ
+    // canonical affine (x = X/ZZ, y = Y/ZZZ) of a finite a from a known izzz = 1/ZZZ
+    B2_HD static affine_t<F> to_affine(const xyzz_t& a, const F& izzz) {
         F izz = F::sqr(F::mul(izzz, a.zz));          // ZZ^3 = ZZZ^2  =>  1/ZZ = (ZZ/ZZZ)^2
         affine_t<F> r;
         r.x = F::mul(a.x, izz);
         r.y = F::mul(a.y, izzz);
         return r;
+    }
+    // the same with its own inversion; infinity -> (0,0)
+    B2_HD_NI static affine_t<F> to_affine(const xyzz_t& a) {
+        if (a.is_inf()) return affine_t<F>::infinity();
+        return to_affine(a, F::inv(a.zzz));
     }
 
     // k * p for a 256-bit canonical (non-Montgomery) scalar k given as 8 x u32
@@ -204,6 +207,22 @@ struct xyzz_t {
         return acc;
     }
 };
+
+// the fixed generator of G1 (F = Fq) or G2 (F = Fq2), Montgomery form
+template <class F> B2_HD affine_t<F> curve_generator();
+template <> B2_HD affine_t<Fq> curve_generator<Fq>() {
+    affine_t<Fq> g;
+    for (int i = 0; i < 8; ++i) { g.x.l[i] = CurveConst::g1_gen_x(i); g.y.l[i] = CurveConst::g1_gen_y(i); }
+    return g;
+}
+template <> B2_HD affine_t<Fq2> curve_generator<Fq2>() {
+    affine_t<Fq2> g;
+    for (int i = 0; i < 8; ++i) {
+        g.x.c0.l[i] = CurveConst::g2_gen_x0(i); g.x.c1.l[i] = CurveConst::g2_gen_x1(i);
+        g.y.c0.l[i] = CurveConst::g2_gen_y0(i); g.y.c1.l[i] = CurveConst::g2_gen_y1(i);
+    }
+    return g;
+}
 
 #ifdef __CUDACC__
 // ---------------------------------------------------------------------------------------------
@@ -230,20 +249,6 @@ struct quad_ops {
     // Shuffles were measured slower here: with data-dependent branches upstream every SHFL gets wrapped in a
     // WARPSYNC/collective sequence (576 SHFL + 320 WARPSYNC per doubling+addition in SASS).
     struct xch_t { F p[2][4]; };
-    __device__ __forceinline__ static void put(F* dst, const F& v) {
-        const uint4* s4 = reinterpret_cast<const uint4*>(&v);
-        uint4* d4 = reinterpret_cast<uint4*>(dst);
-#pragma unroll
-        for (int i = 0; i < (int)(sizeof(F) / 16); ++i) d4[i] = s4[i];
-    }
-    __device__ __forceinline__ static F get(const F* src) {
-        F r;
-        const uint4* s4 = reinterpret_cast<const uint4*>(src);
-        uint4* d4 = reinterpret_cast<uint4*>(&r);
-#pragma unroll
-        for (int i = 0; i < (int)(sizeof(F) / 16); ++i) d4[i] = s4[i];
-        return r;
-    }
     __device__ __forceinline__ static F sel(int q, const F& a0, const F& a1, const F& a2, const F& a3) {
         F r;
         const uint32_t* p0 = reinterpret_cast<const uint32_t*>(&a0);
@@ -261,9 +266,9 @@ struct quad_ops {
         const int q = quad_lane();
         F a = sel(q, a0, a1, a2, a3), b = sel(q, b0, b1, b2, b3);
         F p = F::mul(a, b);
-        put(&x->p[buf][q], p);
+        st16(&x->p[buf][q], p);
         __syncwarp(quad_mask());
-        p0 = get(&x->p[buf][0]); p1 = get(&x->p[buf][1]); p2 = get(&x->p[buf][2]); p3 = get(&x->p[buf][3]);
+        p0 = ld16(&x->p[buf][0]); p1 = ld16(&x->p[buf][1]); p2 = ld16(&x->p[buf][2]); p3 = ld16(&x->p[buf][3]);
     }
 
     __device__ static xyzz_t<F> dbl(xch_t* x, const xyzz_t<F>& p) {

@@ -491,6 +491,15 @@ struct Fp {
         x[7] = cc::addc(x[7], y[7]);
     }
     B2_HD static Fp from_u32(uint32_t v) { Fp o = zero(); o.l[0] = v; return to_mont(o); }
+    // start * base^e by square-and-multiply
+    B2_HD static Fp pow_u64(Fp base, uint64_t e, Fp start = one()) {
+        while (e) {
+            if (e & 1) start = mul(start, base);
+            base = sqr(base);
+            e >>= 1;
+        }
+        return start;
+    }
 };
 
 typedef Fp<FqParams> Fq;
@@ -574,5 +583,39 @@ struct Fq2 {
         Fq2 r; r.c0 = Fq::mul(a.c0, n); r.c1 = Fq::neg(Fq::mul(a.c1, n)); return r;
     }
 };
+
+#ifdef __CUDACC__
+// 16-byte vector load / store of a field element, a point or any other T whose size is a multiple of 16 bytes
+template <class T>
+__device__ __forceinline__ T ld16(const T* p) {
+    static_assert(sizeof(T) % 16 == 0, "16-byte multiple");
+    T r;
+    const uint4* s = reinterpret_cast<const uint4*>(p);
+    uint4* d = reinterpret_cast<uint4*>(&r);
+#pragma unroll
+    for (int i = 0; i < (int)(sizeof(T) / 16); ++i) d[i] = s[i];
+    return r;
+}
+// the same at an untyped (16-byte aligned) address, e.g. a byte offset into a packed record
+template <class T>
+__device__ __forceinline__ T ld16(const void* p) { return ld16(static_cast<const T*>(p)); }
+template <class T>
+__device__ __forceinline__ void st16(T* p, const T& v) {
+    static_assert(sizeof(T) % 16 == 0, "16-byte multiple");
+    const uint4* s = reinterpret_cast<const uint4*>(&v);
+    uint4* d = reinterpret_cast<uint4*>(p);
+#pragma unroll
+    for (int i = 0; i < (int)(sizeof(T) / 16); ++i) d[i] = s[i];
+}
+
+// w_n, the primitive 2^log_n-th root of unity of the field NTT (its inverse if `inverse`), log_n <= 28
+__device__ __forceinline__ Fr fr_root_of_unity(unsigned log_n, bool inverse) {
+    Fr w;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) w.l[i] = inverse ? FrParams::root28_inv(i) : FrParams::root28(i);
+    for (unsigned k = log_n; k < 28; ++k) w = Fr::sqr(w);
+    return w;
+}
+#endif  // __CUDACC__
 
 }  // namespace b200zk

@@ -106,4 +106,20 @@ B2_HD GlvSplit glv_decompose(const uint32_t k[8]) {
     return s;
 }
 
+// the x coordinate of phi(P): beta x on G1, beta^2 x on the twist (the same lambda; tools/gen_constants.py checks both).
+// phi leaves y and the XYZZ denominators alone, so it applies to affine and XYZZ points alike.
+B2_HD void glv_phi_x(Fq& x) {
+    Fq beta;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) beta.l[i] = GlvParams::beta(i);
+    x = Fq::mul(x, beta);
+}
+B2_HD void glv_phi_x(Fq2& x) {
+    Fq beta;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) beta.l[i] = GlvParams::beta_g2(i);
+    x.c0 = Fq::mul(x.c0, beta);
+    x.c1 = Fq::mul(x.c1, beta);
+}
+
 }  // namespace b200zk

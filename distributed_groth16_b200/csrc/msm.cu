@@ -22,25 +22,6 @@ namespace b200zk {
 
 static const uint32_t KEY_NONE = 0xFFFFFFFFu;
 
-template <class T>
-__device__ __forceinline__ T ld16(const T* p) {
-    static_assert(sizeof(T) % 16 == 0, "16-byte multiple");
-    T r;
-    const uint4* s = reinterpret_cast<const uint4*>(p);
-    uint4* d = reinterpret_cast<uint4*>(&r);
-#pragma unroll
-    for (int i = 0; i < (int)(sizeof(T) / 16); ++i) d[i] = s[i];
-    return r;
-}
-template <class T>
-__device__ __forceinline__ void st16(T* p, const T& v) {
-    static_assert(sizeof(T) % 16 == 0, "16-byte multiple");
-    const uint4* s = reinterpret_cast<const uint4*>(&v);
-    uint4* d = reinterpret_cast<uint4*>(p);
-#pragma unroll
-    for (int i = 0; i < (int)(sizeof(T) / 16); ++i) d[i] = s[i];
-}
-
 // ---------------------------------------------------------------------------------------------
 // 1. digits + histogram
 // ---------------------------------------------------------------------------------------------
@@ -473,20 +454,7 @@ __global__ void __launch_bounds__(32) k_msm_horner(const xyzz_t<F>* wsum, uint32
 
 // GLV variant: quad 0 runs the chain of the |k1| windows (sets 2k), quad 1 that of the |k2| windows (sets 2k + 1) in
 // the same warp (half as many sequential doublings); result = H0 + phi(H1), phi(X, Y, ZZ, ZZZ) = (beta X, Y, ZZ, ZZZ) on G1 and
-// (beta^2 X, Y, ZZ, ZZZ) on the twist (the same lambda: tools/gen_constants.py checks both).
-__device__ __forceinline__ void glv_phi_x(Fq& x) {
-    Fq beta;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) beta.l[i] = GlvParams::beta(i);
-    x = Fq::mul(x, beta);
-}
-__device__ __forceinline__ void glv_phi_x(Fq2& x) {
-    Fq beta;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) beta.l[i] = GlvParams::beta_g2(i);
-    x.c0 = Fq::mul(x.c0, beta);
-    x.c1 = Fq::mul(x.c1, beta);
-}
+// (beta^2 X, Y, ZZ, ZZZ) on the twist (glv_phi_x).
 template <class F>
 __global__ void __launch_bounds__(32) k_msm_horner_glv(const xyzz_t<F>* wsum, uint32_t nwin, uint32_t c, uint32_t first, uint32_t last,
                                                        xyzz_t<F>* state, xyzz_t<F>* out) {
@@ -1216,21 +1184,6 @@ __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
     x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ULL;
     x = (x ^ (x >> 27)) * 0x94D049BB133111EBULL;
     return x ^ (x >> 31);
-}
-
-template <class F> __device__ affine_t<F> curve_generator();
-template <> __device__ affine_t<Fq> curve_generator<Fq>() {
-    affine_t<Fq> g;
-    for (int i = 0; i < 8; ++i) { g.x.l[i] = CurveConst::g1_gen_x(i); g.y.l[i] = CurveConst::g1_gen_y(i); }
-    return g;
-}
-template <> __device__ affine_t<Fq2> curve_generator<Fq2>() {
-    affine_t<Fq2> g;
-    for (int i = 0; i < 8; ++i) {
-        g.x.c0.l[i] = CurveConst::g2_gen_x0(i); g.x.c1.l[i] = CurveConst::g2_gen_x1(i);
-        g.y.c0.l[i] = CurveConst::g2_gen_y0(i); g.y.c1.l[i] = CurveConst::g2_gen_y1(i);
-    }
-    return g;
 }
 
 // P_i = k_i * G, k_i = splitmix64(seed + i) | 1

@@ -43,69 +43,34 @@ struct NttPlan {
     std::vector<void*> allocs;
 };
 
-__device__ __forceinline__ Fr ld_fr(const Fr* p) {
-    const uint4* q = reinterpret_cast<const uint4*>(p);
-    uint4 a = q[0], b = q[1];
-    Fr r;
-    r.l[0] = a.x; r.l[1] = a.y; r.l[2] = a.z; r.l[3] = a.w;
-    r.l[4] = b.x; r.l[5] = b.y; r.l[6] = b.z; r.l[7] = b.w;
-    return r;
-}
-__device__ __forceinline__ void st_fr(Fr* p, const Fr& v) {
-    uint4* q = reinterpret_cast<uint4*>(p);
-    q[0] = make_uint4(v.l[0], v.l[1], v.l[2], v.l[3]);
-    q[1] = make_uint4(v.l[4], v.l[5], v.l[6], v.l[7]);
-}
-
 __device__ __forceinline__ Fr powtab_get(const PowTab& t, uint64_t e) {
-    Fr lo = ld_fr(t.lo + (e & ((1ull << t.lo_bits) - 1)));
+    Fr lo = ld16(t.lo + (e & ((1ull << t.lo_bits) - 1)));
     uint64_t hi_i = e >> t.lo_bits;
     if (hi_i == 0) return lo;
-    return Fr::mul(lo, ld_fr(t.hi + hi_i));
-}
-
-__device__ Fr fr_pow_u64(Fr base, uint64_t e) {
-    Fr res = Fr::one();
-    while (e) {
-        if (e & 1) res = Fr::mul(res, base);
-        base = Fr::sqr(base);
-        e >>= 1;
-    }
-    return res;
+    return Fr::mul(lo, ld16(t.hi + hi_i));
 }
 
 // consts[0] = w_N (or its inverse), [1] = N^-1, [2] = g (or g^-1), [3] = w_2N (forward; one if log_n = 28)
 __global__ void k_plan_consts(unsigned log_n, int inverse, Fr* consts) {
     if (threadIdx.x != 0 || blockIdx.x != 0) return;
-    Fr w, g;
-    for (int i = 0; i < 8; ++i) {
-        w.l[i] = inverse ? FrParams::root28_inv(i) : FrParams::root28(i);
-        g.l[i] = inverse ? FrParams::gen_inv(i) : FrParams::gen(i);
-    }
-    for (unsigned k = log_n; k < 28; ++k) w = Fr::sqr(w);
-    consts[0] = w;
+    Fr g;
+    for (int i = 0; i < 8; ++i) g.l[i] = inverse ? FrParams::gen_inv(i) : FrParams::gen(i);
+    consts[0] = fr_root_of_unity(log_n, inverse);
     Fr two = Fr::add(Fr::one(), Fr::one());
     Fr n = Fr::one();
     for (unsigned k = 0; k < log_n; ++k) n = Fr::mul(n, two);
     consts[1] = Fr::inv(n);
     consts[2] = g;
-    Fr w2;
-    for (int i = 0; i < 8; ++i) w2.l[i] = FrParams::root28(i);
-    if (log_n + 1 <= 28) {
-        for (unsigned k = log_n + 1; k < 28; ++k) w2 = Fr::sqr(w2);
-    } else {
-        w2 = Fr::one();
-    }
-    consts[3] = w2;
+    consts[3] = log_n < 28 ? fr_root_of_unity(log_n + 1, false) : Fr::one();
 }
 
 // out[i] = base^(i << shift) (* scale, if given)
 __global__ void k_build_pow(const Fr* base_ptr, Fr* out, uint32_t count, uint32_t shift, const Fr* scale = nullptr) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;
-    Fr v = fr_pow_u64(*base_ptr, (uint64_t)i << shift);
+    Fr v = Fr::pow_u64(*base_ptr, (uint64_t)i << shift);
     if (scale) v = Fr::mul(v, *scale);
-    st_fr(out + i, v);
+    st16(out + i, v);
 }
 
 struct PassParams {
@@ -160,7 +125,7 @@ __global__ void __launch_bounds__(512, B2_NTT_MINBLOCKS) k_ntt_pass(PassParams p
         uint64_t q = p.batch_tile ? q0 : q0 + c, j = q >> p.logM, n2 = q & Mmask;
         uint64_t addr = (j << (p.logR + p.logM)) + ((uint64_t)ns << p.logM) + n2;
         const Fr* in = p.in + (size_t)(p.batch_tile ? b0 + c : b0) * p.batch_stride;
-        Fr v = ld_fr(in + addr);
+        Fr v = ld16(in + addr);
         if (p.apply_pre) v = Fr::mul(v, powtab_get(p.pre, addr));
         uint32_t slot = p.logR ? (__brev(ns) >> (32 - p.logR)) : 0;
         uint32_t e = c * R + slot;
@@ -174,13 +139,13 @@ __global__ void __launch_bounds__(512, B2_NTT_MINBLOCKS) k_ntt_pass(PassParams p
     // stores them back: the same 4 twiddle products as two radix-2 stages (a prime field has no free multiplication by i),
     // but one shared-memory round trip and one barrier instead of two, and four independent products in flight per thread.
     // An odd number of stages starts with the single unit-twiddle stage s = 1.
-    auto lds = [&](uint32_t i) {
+    auto ld_split = [&](uint32_t i) {
         uint4 lo = s_lo[i], hi = s_hi[i];
         Fr v;
         v.l[0] = lo.x; v.l[1] = lo.y; v.l[2] = lo.z; v.l[3] = lo.w; v.l[4] = hi.x; v.l[5] = hi.y; v.l[6] = hi.z; v.l[7] = hi.w;
         return v;
     };
-    auto sts = [&](uint32_t i, const Fr& v) {
+    auto st_split = [&](uint32_t i, const Fr& v) {
         s_lo[i] = make_uint4(v.l[0], v.l[1], v.l[2], v.l[3]);
         s_hi[i] = make_uint4(v.l[4], v.l[5], v.l[6], v.l[7]);
     };
@@ -196,9 +161,9 @@ __global__ void __launch_bounds__(512, B2_NTT_MINBLOCKS) k_ntt_pass(PassParams p
         for (uint32_t b = tid; b < nbf; b += nt) {
             const uint32_t c = b >> (p.logR - 1), bb = b & (R / 2 - 1);
             const uint32_t i0 = c * R + (bb << 1), i1 = i0 + 1;
-            const Fr u = lds(i0), v = lds(i1);
-            sts(i0, Fr::add(u, v));
-            sts(i1, Fr::sub(u, v));
+            const Fr u = ld_split(i0), v = ld_split(i1);
+            st_split(i0, Fr::add(u, v));
+            st_split(i1, Fr::sub(u, v));
         }
         __syncthreads();
         s = 2;
@@ -210,7 +175,7 @@ __global__ void __launch_bounds__(512, B2_NTT_MINBLOCKS) k_ntt_pass(PassParams p
             const uint32_t c = b >> (p.logR - 2), bb = b & (R / 4 - 1);
             const uint32_t jj = bb & (half - 1);
             const uint32_t e0 = c * R + (((bb >> (s - 1)) << (s + 1)) | jj);
-            Fr x0 = lds(e0), x1 = lds(e0 + half), x2 = lds(e0 + 2 * half), x3 = lds(e0 + 3 * half);
+            Fr x0 = ld_split(e0), x1 = ld_split(e0 + half), x2 = ld_split(e0 + 2 * half), x3 = ld_split(e0 + 3 * half);
             if (s > 1) {                    // stage s twiddle w_R^(jj 2^(logR - s)), the same for both pairs
                 const Fr t = twd(jj << (p.logR - s));
                 x1 = Fr::mul(x1, t);
@@ -220,10 +185,10 @@ __global__ void __launch_bounds__(512, B2_NTT_MINBLOCKS) k_ntt_pass(PassParams p
             // stage s + 1: pairs (y0, y2) at index jj and (y1, y3) at index jj + half of a 2^s-point group
             if (s > 1) y2 = Fr::mul(y2, twd(jj << (p.logR - s - 1)));      // s = 1: jj = 0, unit twiddle
             y3 = Fr::mul(y3, twd((jj + half) << (p.logR - s - 1)));
-            sts(e0, Fr::add(y0, y2));
-            sts(e0 + 2 * half, Fr::sub(y0, y2));
-            sts(e0 + half, Fr::add(y1, y3));
-            sts(e0 + 3 * half, Fr::sub(y1, y3));
+            st_split(e0, Fr::add(y0, y2));
+            st_split(e0 + 2 * half, Fr::sub(y0, y2));
+            st_split(e0 + half, Fr::add(y1, y3));
+            st_split(e0 + 3 * half, Fr::sub(y1, y3));
         }
         __syncthreads();
     }
@@ -246,12 +211,12 @@ __global__ void __launch_bounds__(512, B2_NTT_MINBLOCKS) k_ntt_pass(PassParams p
             uint64_t ex = (bidx + p.post_b0) * (p.post_alpha * oaddr + p.post_beta) + p.post_gamma * oaddr;
             if (ex) v = Fr::mul(v, powtab_get(p.post, ex));
         }
-        if (p.apply_post_const) v = Fr::mul(v, ld_fr(p.post_const));
+        if (p.apply_post_const) v = Fr::mul(v, ld16(p.post_const));
         if (p.p2p) {
             Fr* dst = p.peer_out[oaddr >> p.log_rl] + ((oaddr & ((1ull << p.log_rl) - 1)) << p.log_cols_total) + p.col0 + bidx;
-            st_fr(dst, v);
+            st16(dst, v);
         } else {
-            st_fr(out + oaddr, v);
+            st16(out + oaddr, v);
         }
     }
 }
@@ -260,14 +225,14 @@ __global__ void k_bitrev(const Fr* in, Fr* out, unsigned log_n) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= ((size_t)1 << log_n)) return;
     size_t j = log_n ? (size_t)(__brevll((unsigned long long)i) >> (64 - log_n)) : 0;
-    st_fr(out + j, ld_fr(in + i));
+    st16(out + j, ld16(in + i));
 }
 
 // h[i] = a[i]*b[i] - c[i]
 __global__ void k_h_pointwise(const Fr* a, const Fr* b, const Fr* c, Fr* h, size_t m) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m) return;
-    st_fr(h + i, Fr::sub(Fr::mul(ld_fr(a + i), ld_fr(b + i)), ld_fr(c + i)));
+    st16(h + i, Fr::sub(Fr::mul(ld16(a + i), ld16(b + i)), ld16(c + i)));
 }
 
 static int build_powtab(b200zk_ctx* ctx, cudaStream_t st, NttPlan* pl, const Fr* base, unsigned log_range, PowTab* out) {

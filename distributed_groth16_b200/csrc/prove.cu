@@ -13,16 +13,6 @@
 
 namespace b200zk {
 
-template <class T>
-__device__ __forceinline__ T ldp(const void* p) {
-    T r;
-    const uint4* s = reinterpret_cast<const uint4*>(p);
-    uint4* d = reinterpret_cast<uint4*>(&r);
-#pragma unroll
-    for (int i = 0; i < (int)(sizeof(T) / 16); ++i) d[i] = s[i];
-    return r;
-}
-
 __device__ bool fq_is_neg(const Fq& y) {       // arkworks: y > -y  (canonical integers)
     Fq a = Fq::from_mont(y), b = Fq::from_mont(Fq::neg(y));
     for (int i = 7; i >= 0; --i) {
@@ -74,20 +64,20 @@ __global__ void __launch_bounds__(96) k_prove_finalize(FinalizeArgs f) {
     bool r_zero = r.is_zero(), s_zero = s.is_zero();
 
     if (role == 1) {
-        affine_t<Fq2> beta2 = ldp<affine_t<Fq2>>(vk + 192), delta2 = ldp<affine_t<Fq2>>(vk + 320);
-        xyzz_t<Fq2> Bp = ldp<xyzz_t<Fq2>>(f.msm_b2);
-        if (f.add_zero_terms) xyzz_t<Fq2>::madd(Bp, ldp<affine_t<Fq2>>(f.b2_0), false);
+        affine_t<Fq2> beta2 = ld16<affine_t<Fq2>>(vk + 192), delta2 = ld16<affine_t<Fq2>>(vk + 320);
+        xyzz_t<Fq2> Bp = ld16<xyzz_t<Fq2>>(f.msm_b2);
+        if (f.add_zero_terms) xyzz_t<Fq2>::madd(Bp, ld16<affine_t<Fq2>>(f.b2_0), false);
         xyzz_t<Fq2>::madd(Bp, beta2, false);
         if (!s_zero) Bp = xyzz_t<Fq2>::add(Bp, xyzz_t<Fq2>::mul_scalar(xyzz_t<Fq2>::from_affine(delta2), s.l));
         compress_g2(Bp, f.out + 32);
         return;
     }
-    affine_t<Fq> alpha = ldp<affine_t<Fq>>(vk), beta1 = ldp<affine_t<Fq>>(vk + 64), delta1 = ldp<affine_t<Fq>>(vk + 128);
+    affine_t<Fq> alpha = ld16<affine_t<Fq>>(vk), beta1 = ld16<affine_t<Fq>>(vk + 64), delta1 = ld16<affine_t<Fq>>(vk + 128);
     xyzz_t<Fq> d1 = xyzz_t<Fq>::from_affine(delta1);
     xyzz_t<Fq> A = xyzz_t<Fq>::identity();
     if (role == 0 || !s_zero) {
-        A = ldp<xyzz_t<Fq>>(f.msm_a);
-        if (f.add_zero_terms) xyzz_t<Fq>::madd(A, ldp<affine_t<Fq>>(f.a0), false);
+        A = ld16<xyzz_t<Fq>>(f.msm_a);
+        if (f.add_zero_terms) xyzz_t<Fq>::madd(A, ld16<affine_t<Fq>>(f.a0), false);
         xyzz_t<Fq>::madd(A, alpha, false);
         if (!r_zero) A = xyzz_t<Fq>::add(A, xyzz_t<Fq>::mul_scalar(d1, r.l));
     }
@@ -96,11 +86,11 @@ __global__ void __launch_bounds__(96) k_prove_finalize(FinalizeArgs f) {
         return;
     }
     Fr rs = Fr::from_mont(Fr::mul(f.rs[0], f.rs[1]));
-    xyzz_t<Fq> C = xyzz_t<Fq>::add(ldp<xyzz_t<Fq>>(f.msm_l), ldp<xyzz_t<Fq>>(f.msm_h));
+    xyzz_t<Fq> C = xyzz_t<Fq>::add(ld16<xyzz_t<Fq>>(f.msm_l), ld16<xyzz_t<Fq>>(f.msm_h));
     if (!s_zero) C = xyzz_t<Fq>::add(C, xyzz_t<Fq>::mul_scalar(A, s.l));
     if (!r_zero) {
-        xyzz_t<Fq> B1 = ldp<xyzz_t<Fq>>(f.msm_b1);
-        if (f.add_zero_terms) xyzz_t<Fq>::madd(B1, ldp<affine_t<Fq>>(f.b1_0), false);
+        xyzz_t<Fq> B1 = ld16<xyzz_t<Fq>>(f.msm_b1);
+        if (f.add_zero_terms) xyzz_t<Fq>::madd(B1, ld16<affine_t<Fq>>(f.b1_0), false);
         xyzz_t<Fq>::madd(B1, beta1, false);
         if (!s_zero) B1 = xyzz_t<Fq>::add(B1, xyzz_t<Fq>::mul_scalar(d1, s.l));
         C = xyzz_t<Fq>::add(C, xyzz_t<Fq>::mul_scalar(B1, r.l));

@@ -10,30 +10,17 @@
 
 namespace b200zk {
 
-__device__ __forceinline__ Fr ldq(const Fr* p) {
-    const uint4* q = reinterpret_cast<const uint4*>(p);
-    uint4 a = q[0], b = q[1];
-    Fr r;
-    r.l[0] = a.x; r.l[1] = a.y; r.l[2] = a.z; r.l[3] = a.w; r.l[4] = b.x; r.l[5] = b.y; r.l[6] = b.z; r.l[7] = b.w;
-    return r;
-}
-__device__ __forceinline__ void stq(Fr* p, const Fr& v) {
-    uint4* q = reinterpret_cast<uint4*>(p);
-    q[0] = make_uint4(v.l[0], v.l[1], v.l[2], v.l[3]);
-    q[1] = make_uint4(v.l[4], v.l[5], v.l[6], v.l[7]);
-}
-
 __global__ void k_fr_convert(const Fr* in, Fr* out, size_t n, int to_mont, int times) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    Fr v = ldq(in + i);
+    Fr v = ld16(in + i);
     for (int t = 0; t < times; ++t) v = to_mont ? Fr::to_mont(v) : Fr::from_mont(v);
-    stq(out + i, v);
+    st16(out + i, v);
 }
 
 __device__ __forceinline__ Fr row_dot(const uint32_t* ptr, const uint32_t* col, const Fr* val, const Fr* z, uint32_t i) {
     Fr acc = Fr::zero();
-    for (uint32_t k = ptr[i], e = ptr[i + 1]; k < e; ++k) acc = Fr::add(acc, Fr::mul(ldq(val + k), ldq(z + col[k])));
+    for (uint32_t k = ptr[i], e = ptr[i + 1]; k < e; ++k) acc = Fr::add(acc, Fr::mul(ld16(val + k), ld16(z + col[k])));
     return acc;
 }
 
@@ -47,9 +34,9 @@ __global__ void k_qap(const uint32_t* a_ptr, const uint32_t* a_col, const Fr* a_
         vb = row_dot(b_ptr, b_col, b_val, z, i);
         vc = Fr::mul(va, vb);
     } else if (i < nc + n_inputs) {
-        va = ldq(z + (i - nc));
+        va = ld16(z + (i - nc));
     }
-    stq(a + i, va); stq(b + i, vb); stq(c + i, vc);
+    st16(a + i, va); st16(b + i, vb); st16(c + i, vc);
 }
 
 // One warp per row: the lanes stride over the row's non-zeros and the partial sums meet in a shuffle tree.  Small circuits have
@@ -67,7 +54,7 @@ __device__ __forceinline__ Fr warp_sum(Fr v) {
 }
 __device__ __forceinline__ Fr row_dot_warp(const uint32_t* ptr, const uint32_t* col, const Fr* val, const Fr* z, uint32_t i, uint32_t lane) {
     Fr acc = Fr::zero();
-    for (uint32_t k = ptr[i] + lane, e = ptr[i + 1]; k < e; k += 32) acc = Fr::add(acc, Fr::mul(ldq(val + k), ldq(z + col[k])));
+    for (uint32_t k = ptr[i] + lane, e = ptr[i + 1]; k < e; k += 32) acc = Fr::add(acc, Fr::mul(ld16(val + k), ld16(z + col[k])));
     return warp_sum(acc);
 }
 __global__ void __launch_bounds__(256) k_qap_warp(const uint32_t* a_ptr, const uint32_t* a_col, const Fr* a_val, const uint32_t* b_ptr,
@@ -81,9 +68,9 @@ __global__ void __launch_bounds__(256) k_qap_warp(const uint32_t* a_ptr, const u
         vb = row_dot_warp(b_ptr, b_col, b_val, z, i, lane);
         vc = Fr::mul(va, vb);
     } else if (i < nc + n_inputs) {
-        va = ldq(z + (i - nc));
+        va = ld16(z + (i - nc));
     }
-    if (lane == 0) { stq(a + i, va); stq(b + i, vb); stq(c + i, vc); }
+    if (lane == 0) { st16(a + i, va); st16(b + i, vb); st16(c + i, vc); }
 }
 
 int fr_convert_dev(b200zk_ctx* ctx, Slot& sl, const void* d_in, void* d_out, size_t n, int to_mont, int times) {

@@ -10,50 +10,18 @@
 
 namespace b200zk {
 
-template <class T>
-__device__ __forceinline__ T lds(const T* p) {
-    T r;
-    const uint4* s = reinterpret_cast<const uint4*>(p);
-    uint4* d = reinterpret_cast<uint4*>(&r);
-#pragma unroll
-    for (int i = 0; i < (int)(sizeof(T) / 16); ++i) d[i] = s[i];
-    return r;
-}
-template <class T>
-__device__ __forceinline__ void sts(T* p, const T& v) {
-    const uint4* s = reinterpret_cast<const uint4*>(&v);
-    uint4* d = reinterpret_cast<uint4*>(p);
-#pragma unroll
-    for (int i = 0; i < (int)(sizeof(T) / 16); ++i) d[i] = s[i];
-}
-
-template <class F> __device__ affine_t<F> generator_of();
-template <> __device__ affine_t<Fq> generator_of<Fq>() {
-    affine_t<Fq> g;
-    for (int i = 0; i < 8; ++i) { g.x.l[i] = CurveConst::g1_gen_x(i); g.y.l[i] = CurveConst::g1_gen_y(i); }
-    return g;
-}
-template <> __device__ affine_t<Fq2> generator_of<Fq2>() {
-    affine_t<Fq2> g;
-    for (int i = 0; i < 8; ++i) {
-        g.x.c0.l[i] = CurveConst::g2_gen_x0(i); g.x.c1.l[i] = CurveConst::g2_gen_x1(i);
-        g.y.c0.l[i] = CurveConst::g2_gen_y0(i); g.y.c1.l[i] = CurveConst::g2_gen_y1(i);
-    }
-    return g;
-}
-
 // table[w * 15 + (d - 1)] = d * 16^w * G,  w < 64, d in 1..15 (affine).  64 threads: thread w first walks to 16^w G.
 template <class F>
 __global__ void k_fixed_base_table(affine_t<F>* table) {
     uint32_t w = blockIdx.x * blockDim.x + threadIdx.x;
     if (w >= 64) return;
-    xyzz_t<F> base = xyzz_t<F>::from_affine(generator_of<F>());
+    xyzz_t<F> base = xyzz_t<F>::from_affine(curve_generator<F>());
     for (uint32_t k = 0; k < 4 * w; ++k) base = xyzz_t<F>::dbl(base);
     affine_t<F> b = xyzz_t<F>::to_affine(base);
     xyzz_t<F> acc = xyzz_t<F>::identity();
     for (uint32_t d = 1; d <= 15; ++d) {
         xyzz_t<F>::madd(acc, b, false);
-        sts(table + w * 15 + (d - 1), xyzz_t<F>::to_affine(acc));
+        st16(table + w * 15 + (d - 1), xyzz_t<F>::to_affine(acc));
     }
 }
 
@@ -62,30 +30,20 @@ template <class F>
 __global__ void __launch_bounds__(128) k_fixed_base_mul(const affine_t<F>* table, const Fr* scalars, size_t n, affine_t<F>* out) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    Fr k = Fr::from_mont(lds(scalars + i));
+    Fr k = Fr::from_mont(ld16(scalars + i));
     xyzz_t<F> acc = xyzz_t<F>::identity();
     for (uint32_t w = 0; w < 64; ++w) {
         uint32_t d = (k.l[w >> 3] >> ((w & 7) * 4)) & 15;
-        if (d) xyzz_t<F>::madd(acc, lds(table + w * 15 + (d - 1)), false);
+        if (d) xyzz_t<F>::madd(acc, ld16(table + w * 15 + (d - 1)), false);
     }
-    sts(out + i, xyzz_t<F>::to_affine(acc));
-}
-
-// res * b^e by square-and-multiply
-__device__ __forceinline__ Fr fr_pow_scaled(Fr b, Fr res, uint64_t e) {
-    while (e) {
-        if (e & 1) res = Fr::mul(res, b);
-        b = Fr::sqr(b);
-        e >>= 1;
-    }
-    return res;
+    st16(out + i, xyzz_t<F>::to_affine(acc));
 }
 
 // out[i] = scale * base^i
 __global__ void k_fr_powers(const Fr* consts /* base, scale */, size_t n, Fr* out) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    sts(out + i, fr_pow_scaled(consts[0], consts[1], i));
+    st16(out + i, Fr::pow_u64(consts[0], i, consts[1]));
 }
 
 // out[r] = sum_k val[k] * x[idx[k]],  k in [ptr[r], ptr[r+1])
@@ -93,8 +51,8 @@ __global__ void k_spmv(const uint32_t* ptr, const uint32_t* idx, const Fr* val, 
     size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n_rows) return;
     Fr acc = Fr::zero();
-    for (uint32_t k = ptr[r], e = ptr[r + 1]; k < e; ++k) acc = Fr::add(acc, Fr::mul(lds(val + k), lds(x + idx[k])));
-    sts(out + r, acc);
+    for (uint32_t k = ptr[r], e = ptr[r + 1]; k < e; ++k) acc = Fr::add(acc, Fr::mul(ld16(val + k), ld16(x + idx[k])));
+    st16(out + r, acc);
 }
 
 // ---- CSR product over points: out[r] = sum_k val[k] * points[idx[k]]  (snarkjs `zkey new`) -----------------------
@@ -112,18 +70,18 @@ __global__ void __launch_bounds__(128) k_points_spmv_products(const uint32_t* id
                                                               size_t lo, size_t hi, xyzz_t<F>* prod) {
     size_t k = lo + (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= hi) return;
-    const Fr v = Fr::from_mont(lds(val + k));
+    const Fr v = Fr::from_mont(ld16(val + k));
     int top = 7;
     while (top >= 0 && v.l[top] == 0) --top;
     xyzz_t<F> acc = xyzz_t<F>::identity();
     if (top >= 0) {
-        const affine_t<F> p = lds(points + idx[k]);
+        const affine_t<F> p = ld16(points + idx[k]);
         for (int bit = 32 * top + 31 - __clz(v.l[top]); bit >= 0; --bit) {     // double-and-add from the top set bit
             acc = xyzz_t<F>::dbl(acc);
             if ((v.l[bit >> 5] >> (bit & 31)) & 1) xyzz_t<F>::madd(acc, p, false);
         }
     }
-    sts(prod + k, acc);
+    st16(prod + k, acc);
 }
 
 // rows of at most SPMV_MSM_ROW entries: sum of their products, normalised; longer rows are left to the MSM path
@@ -134,19 +92,19 @@ __global__ void __launch_bounds__(128) k_points_spmv_sum(const uint32_t* ptr, co
     const uint32_t b = ptr[r], e = ptr[r + 1];
     if (e - b > SPMV_MSM_ROW) return;
     xyzz_t<F> acc = xyzz_t<F>::identity();
-    for (uint32_t k = b; k < e; ++k) acc = xyzz_t<F>::add(acc, lds(prod + k));
-    sts(out + r, xyzz_t<F>::to_affine(acc));
+    for (uint32_t k = b; k < e; ++k) acc = xyzz_t<F>::add(acc, ld16(prod + k));
+    st16(out + r, xyzz_t<F>::to_affine(acc));
 }
 
 template <class F>
 __global__ void k_points_gather(const uint32_t* idx, const affine_t<F>* points, size_t n, affine_t<F>* out) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) sts(out + i, lds(points + idx[i]));
+    if (i < n) st16(out + i, ld16(points + idx[i]));
 }
 
 template <class F>
 __global__ void k_xyzz_to_affine_one(const xyzz_t<F>* in, affine_t<F>* out) {
-    if (threadIdx.x == 0) sts(out, xyzz_t<F>::to_affine(lds(in)));
+    if (threadIdx.x == 0) st16(out, xyzz_t<F>::to_affine(ld16(in)));
 }
 
 template <class F>
@@ -230,8 +188,8 @@ int points_spmv_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* ptr, const vo
 __global__ void k_fr_lincomb(const Fr* a, const Fr* b, const Fr* c, const Fr* s, size_t n, Fr* out) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    Fr v = Fr::add(Fr::add(Fr::mul(lds(a + i), s[0]), Fr::mul(lds(b + i), s[1])), Fr::mul(lds(c + i), s[2]));
-    sts(out + i, Fr::mul(v, s[3]));
+    Fr v = Fr::add(Fr::add(Fr::mul(ld16(a + i), s[0]), Fr::mul(ld16(b + i), s[1])), Fr::mul(ld16(c + i), s[2]));
+    st16(out + i, Fr::mul(v, s[3]));
 }
 
 template <class F>
@@ -307,7 +265,8 @@ int fr_lincomb_dev(b200zk_ctx* ctx, Slot& sl, const void* a, const void* b, cons
 // The phase-2 step the reference's scripts/phase2_proving_key.sh runs after `zkey new`; orchestration in groth16/phase2.py.
 // G1: k is reduced mod r and split once per launch, k = k1 + k2 lambda (glv.cuh), and both halves are recoded on the
 // host into width-5 NAF digits (odd, |d| <= 15, at least four zeros after each non-zero).  The digits travel as a kernel
-// parameter and are the same for every thread, so the digit loop has no divergence: per point about 128 doublings and
+// parameter and are the same for every thread, so the digit loop (glv_table_mul, shared with the point iNTT below) has
+// no divergence: per point about 128 doublings and
 // ~43 mixed additions from a per-thread table of the odd multiples P, 3P, .., 15P (phi(jP) = (beta x, y) is applied on
 // the fly).  The table entries and the results are normalised to affine with block-batched inversions (Montgomery's
 // trick over a block-wide prefix / suffix product): 8 field inversions per block of 64 points, not one per point.
@@ -316,7 +275,8 @@ constexpr int SCALE_NAF = 130;            // |k1|, |k2| < 2^127: at most 128 NAF
 constexpr int SCALE_TAB = 8;              // P, 3P, .., 15P
 
 struct ScaleDigits {
-    int8_t d[2][SCALE_NAF];               // d[h][i]: digit i (weight 2^i) of k1 (h = 0) / k2 (h = 1), signs folded in
+    int8_t d[2][SCALE_NAF];               // d[h][i]: digit i (weight 2^i) of k1 (h = 0) / k2 (h = 1) as a table position
+                                          // (glv_table_mul): NAF digit v -> +-(|v| + 1) / 2, signs folded in
     int top;                              // highest index with a non-zero digit in either half; -1: k = 0 mod r
 };
 
@@ -349,6 +309,14 @@ __device__ F block_batch_inv(const F& a, F* pre, F* suf, F* tot) {
     return r;
 }
 
+// every thread's a in affine form with one block_batch_inv over their ZZZ; finite = !a.is_inf(), passed in because the
+// caller often knows it more cheaply (a thread with finite = false gets infinity).  All threads call it.
+template <class F, int B>
+__device__ __forceinline__ affine_t<F> block_to_affine(const xyzz_t<F>& a, bool finite, F* pre, F* suf, F* tot) {
+    const F izzz = block_batch_inv<F, B>(finite ? a.zzz : F::one(), pre, suf, tot);
+    return finite ? xyzz_t<F>::to_affine(a, izzz) : affine_t<F>::infinity();
+}
+
 // table entry j of this thread, stored as C = sizeof(point) / 16 uint4 per point, [entry][chunk][thread]: conflict-free
 // shared accesses for a block of B threads
 template <class F, int B>
@@ -368,12 +336,31 @@ __device__ __forceinline__ affine_t<F> tab_get(const uint4* tab, int j) {
     return p;
 }
 
+// acc = 2^(DOUBLINGS (top + 1)) acc + sum_{q <= top} 2^(DOUBLINGS q) (d1[q] + d2[q] lambda) P by Horner from q = top, over
+// this thread's table of multiples of P: a digit is a signed table position, +-(j + 1) adds +-(entry j), 0 adds nothing;
+// the d2 entries go through phi (glv_phi_x).
+template <class F, int B, int DOUBLINGS>
+__device__ __forceinline__ void glv_table_mul(xyzz_t<F>& acc, const uint4* tab, const int8_t* d1, const int8_t* d2, int top) {
+#pragma unroll 1
+    for (int q = top; q >= 0; --q) {
+#pragma unroll
+        for (int k = 0; k < DOUBLINGS; ++k) acc = xyzz_t<F>::dbl(acc);
+        const int a = d1[q], b = d2[q];
+        if (a) xyzz_t<F>::madd(acc, tab_get<F, B>(tab, (a < 0 ? -a : a) - 1), a < 0);
+        if (b) {
+            affine_t<F> p = tab_get<F, B>(tab, (b < 0 ? -b : b) - 1);
+            glv_phi_x(p.x);
+            xyzz_t<F>::madd(acc, p, b < 0);
+        }
+    }
+}
+
 __global__ void __launch_bounds__(SCALE_BLOCK) k_points_scale_g1(const __grid_constant__ ScaleDigits dg,
                                                                   const affine_t<Fq>* points, size_t n, affine_t<Fq>* out) {
     __shared__ uint4 tab[SCALE_TAB * 4 * SCALE_BLOCK];
     __shared__ Fq pre[SCALE_BLOCK], suf[SCALE_BLOCK], tot;
     const size_t i = (size_t)blockIdx.x * SCALE_BLOCK + threadIdx.x;
-    const affine_t<Fq> P = i < n ? lds(points + i) : affine_t<Fq>::infinity();
+    const affine_t<Fq> P = i < n ? ld16(points + i) : affine_t<Fq>::infinity();
     const bool inf = P.is_inf();
     // the odd multiples, (2j + 1) P = (2j - 1) P + 2P in XYZZ, each normalised as it is made (one block-batched
     // inverse per entry: only the running entry and 2P are live)
@@ -384,43 +371,13 @@ __global__ void __launch_bounds__(SCALE_BLOCK) k_points_scale_g1(const __grid_co
 #pragma unroll 1
         for (int j = 1; j < SCALE_TAB; ++j) {
             odd = xyzz_t<Fq>::add(odd, two);
-            const Fq izzz = block_batch_inv<Fq, SCALE_BLOCK>(inf ? Fq::one() : odd.zzz, pre, suf, &tot);
-            affine_t<Fq> a = affine_t<Fq>::infinity();
-            if (!inf) {
-                const Fq izz = Fq::sqr(Fq::mul(izzz, odd.zz));                    // ZZ^3 = ZZZ^2  =>  1/ZZ = (ZZ/ZZZ)^2
-                a.x = Fq::mul(odd.x, izz);
-                a.y = Fq::mul(odd.y, izzz);
-            }
-            tab_put<Fq, SCALE_BLOCK>(tab, j, a);
+            tab_put<Fq, SCALE_BLOCK>(tab, j, block_to_affine<Fq, SCALE_BLOCK>(odd, !inf, pre, suf, &tot));
         }
     }
-    Fq beta;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) beta.l[j] = GlvParams::beta(j);
     xyzz_t<Fq> acc = xyzz_t<Fq>::identity();
-    if (!inf) {
-#pragma unroll 1
-        for (int b = dg.top; b >= 0; --b) {
-            acc = xyzz_t<Fq>::dbl(acc);
-            const int d1 = dg.d[0][b], d2 = dg.d[1][b];
-            if (d1) xyzz_t<Fq>::madd(acc, tab_get<Fq, SCALE_BLOCK>(tab, (d1 < 0 ? -d1 : d1) >> 1), d1 < 0);
-            if (d2) {
-                affine_t<Fq> q = tab_get<Fq, SCALE_BLOCK>(tab, (d2 < 0 ? -d2 : d2) >> 1);
-                q.x = Fq::mul(q.x, beta);                                          // phi(jP) = (beta x, y)
-                xyzz_t<Fq>::madd(acc, q, d2 < 0);
-            }
-        }
-    }
-    const bool res_inf = acc.is_inf();
-    const Fq izzz = block_batch_inv<Fq, SCALE_BLOCK>(res_inf ? Fq::one() : acc.zzz, pre, suf, &tot);
-    if (i >= n) return;
-    affine_t<Fq> r = affine_t<Fq>::infinity();
-    if (!res_inf) {
-        const Fq izz = Fq::sqr(Fq::mul(izzz, acc.zz));
-        r.x = Fq::mul(acc.x, izz);
-        r.y = Fq::mul(acc.y, izzz);
-    }
-    sts(out + i, r);
+    if (!inf) glv_table_mul<Fq, SCALE_BLOCK, 1>(acc, tab, dg.d[0], dg.d[1], dg.top);
+    const affine_t<Fq> r = block_to_affine<Fq, SCALE_BLOCK>(acc, !acc.is_inf(), pre, suf, &tot);
+    if (i < n) st16(out + i, r);
 }
 
 // G2 (single points: delta_2, g2_spx, the cofactor of hash-to-G2): the plain 256-bit ladder, no reduction mod r, so that
@@ -431,8 +388,8 @@ __global__ void __launch_bounds__(128) k_points_scale_g2_ladder(const __grid_con
                                                                 size_t n, affine_t<Fq2>* out) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const affine_t<Fq2> p = lds(points + i);
-    sts(out + i, xyzz_t<Fq2>::to_affine(xyzz_t<Fq2>::mul_scalar(xyzz_t<Fq2>::from_affine(p), k.k)));
+    const affine_t<Fq2> p = ld16(points + i);
+    st16(out + i, xyzz_t<Fq2>::to_affine(xyzz_t<Fq2>::mul_scalar(xyzz_t<Fq2>::from_affine(p), k.k)));
 }
 
 // width-5 NAF of a non-negative k < 2^127 into d (digits odd in [-15, 15]); returns the highest non-zero index or -1
@@ -488,8 +445,11 @@ int points_scale_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_points, si
         unsigned __int128 v = 0;
         for (int i = 3; i >= 0; --i) v = (v << 32) | w[i];
         const int t = naf5(v, dg.d[h]);
-        if (h ? sp.neg2 : sp.neg1)
-            for (int i = 0; i < SCALE_NAF; ++i) dg.d[h][i] = (int8_t)-dg.d[h][i];
+        const bool neg = h ? sp.neg2 : sp.neg1;
+        for (int i = 0; i < SCALE_NAF; ++i) {          // the table holds P, 3P, .., 15P: |v| P is entry (|v| - 1) / 2
+            const int v = neg ? -dg.d[h][i] : dg.d[h][i];
+            dg.d[h][i] = (int8_t)(v < 0 ? -((1 - v) / 2) : (v + 1) / 2);
+        }
         top = t > top ? t : top;
     }
     dg.top = top;
@@ -528,11 +488,7 @@ struct __align__(16) TwiddleDigits {
 __global__ void k_intt_twiddle_digits(unsigned log_n, size_t count, TwiddleDigits* out) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;
-    Fr w;
-#pragma unroll
-    for (int l = 0; l < 8; ++l) w.l[l] = FrParams::root28_inv(l);
-    for (unsigned k = log_n; k < 28; ++k) w = Fr::sqr(w);            // the root the field NTT uses (ntt.cu k_plan_consts)
-    const Fr t = Fr::from_mont(fr_pow_scaled(w, Fr::one(), i));
+    const Fr t = Fr::from_mont(Fr::pow_u64(fr_root_of_unity(log_n, true), i));
     const GlvSplit sp = glv_decompose(t.l);
     TwiddleDigits dg;
 #pragma unroll
@@ -548,34 +504,7 @@ __global__ void k_intt_twiddle_digits(unsigned log_n, size_t count, TwiddleDigit
             dg.d[h][q] = (int8_t)(neg ? -v : v);
         }
     }
-    sts(out + i, dg);
-}
-
-template <class F> __device__ __forceinline__ void apply_endo(affine_t<F>& p);
-template <> __device__ __forceinline__ void apply_endo<Fq>(affine_t<Fq>& p) {
-    Fq b;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) b.l[i] = GlvParams::beta(i);
-    p.x = Fq::mul(p.x, b);
-}
-template <> __device__ __forceinline__ void apply_endo<Fq2>(affine_t<Fq2>& p) {
-    Fq b;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) b.l[i] = GlvParams::beta_g2(i);
-    p.x.c0 = Fq::mul(p.x.c0, b);
-    p.x.c1 = Fq::mul(p.x.c1, b);
-}
-
-// affine form of a given 1 / a.zzz
-template <class F>
-__device__ __forceinline__ affine_t<F> affine_with(const xyzz_t<F>& a, const F& izzz) {
-    affine_t<F> r = affine_t<F>::infinity();
-    if (!a.is_inf()) {
-        const F izz = F::sqr(F::mul(izzz, a.zz));
-        r.x = F::mul(a.x, izz);
-        r.y = F::mul(a.y, izzz);
-    }
-    return r;
+    st16(out + i, dg);
 }
 
 // out[i] = in[bitrev(i)]; each pair is handled by one thread that reads both before writing, so out may equal in
@@ -585,9 +514,9 @@ __global__ void k_points_bitrev(const affine_t<F>* in, affine_t<F>* out, unsigne
     if (i >> log_n) return;
     const size_t r = log_n ? (size_t)(__brevll((unsigned long long)i) >> (64 - log_n)) : 0;
     if (r < i) return;
-    const affine_t<F> x = lds(in + i), y = lds(in + r);
-    sts(out + i, y);
-    if (r != i) sts(out + r, x);
+    const affine_t<F> x = ld16(in + i), y = ld16(in + r);
+    st16(out + i, y);
+    if (r != i) st16(out + r, x);
 }
 
 // pass with half-size m = 2^log_m: butterfly t = (j, g), j = t >> lg, g = t mod 2^lg (lg = log2(n / 2m)), on the
@@ -607,7 +536,7 @@ __global__ void __launch_bounds__(B) k_points_intt_pass(affine_t<F>* a, const Tw
     if (!__syncthreads_and(!live || j == 0)) {                           // block-uniform
         // the table is built from shared memory copies only: P and the products stay out of registers during the loop
         {
-            const affine_t<F> P = live ? lds(a + ib) : affine_t<F>::infinity();
+            const affine_t<F> P = live ? ld16(a + ib) : affine_t<F>::infinity();
             mul = live && j != 0 && !P.is_inf();
             tab_put<F, B>(tab, 0, P);
         }
@@ -619,33 +548,16 @@ __global__ void __launch_bounds__(B) k_points_intt_pass(affine_t<F>* a, const Tw
                 if (e == 1) run = xyzz_t<F>::dbl_affine(P.x, P.y);
                 else xyzz_t<F>::madd(run, P, false);
             }
-            const F izzz = block_batch_inv<F, B>(mul ? run.zzz : F::one(), pre, suf, &tot);
-            tab_put<F, B>(tab, e, mul ? affine_with(run, izzz) : affine_t<F>::infinity());
+            tab_put<F, B>(tab, e, block_to_affine<F, B>(run, mul, pre, suf, &tot));
         }
     }
-    xyzz_t<F> prod;
-    if (mul) {
-        const int8_t* d = tw[j << lg].d[0];
-        prod = xyzz_t<F>::identity();
-#pragma unroll 1
-        for (int q = INTT_WINDOWS - 1; q >= 0; --q) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) prod = xyzz_t<F>::dbl(prod);
-            const int d1 = d[q], d2 = d[INTT_WINDOWS + q];
-            if (d1) xyzz_t<F>::madd(prod, tab_get<F, B>(tab, (d1 < 0 ? -d1 : d1) - 1), d1 < 0);
-            if (d2) {
-                affine_t<F> p = tab_get<F, B>(tab, (d2 < 0 ? -d2 : d2) - 1);
-                apply_endo(p);
-                xyzz_t<F>::madd(prod, p, d2 < 0);
-            }
-        }
-    } else {
-        prod = xyzz_t<F>::from_affine(live ? lds(a + ib) : affine_t<F>::infinity());      // w^0 P, or P = infinity
-    }
+    xyzz_t<F> prod = xyzz_t<F>::identity();
+    if (mul) glv_table_mul<F, B, 4>(prod, tab, tw[j << lg].d[0], tw[j << lg].d[1], INTT_WINDOWS - 1);
+    else prod = xyzz_t<F>::from_affine(live ? ld16(a + ib) : affine_t<F>::infinity());      // w^0 P, or P = infinity
     // T = w P in affine form, then U + T and U - T as affine additions that share one inverse: the denominator is
     // x_T - x_U, or 2 y_U when T = +-U (then one result is infinity and the other 2U), or 1 when T or U is infinity
-    const affine_t<F> T = affine_with(prod, block_batch_inv<F, B>(prod.is_inf() ? F::one() : prod.zzz, pre, suf, &tot));
-    const affine_t<F> U = live ? lds(a + ia) : affine_t<F>::infinity();
+    const affine_t<F> T = block_to_affine<F, B>(prod, !prod.is_inf(), pre, suf, &tot);
+    const affine_t<F> U = live ? ld16(a + ia) : affine_t<F>::infinity();
     const bool edge = T.is_inf() || U.is_inf();
     const F dx = F::sub(T.x, U.x);
     const bool dbl = !edge && dx.is_zero();
@@ -677,8 +589,8 @@ __global__ void __launch_bounds__(B) k_points_intt_pass(affine_t<F>* a, const Tw
             df = finish(F::mul(F::neg(F::add(T.y, U.y)), inv), T.x);
         }
     }
-    sts(a + ia, s);
-    sts(a + ib, df);
+    st16(a + ia, s);
+    st16(a + ib, df);
 }
 
 template <class F, int B>
