@@ -12,10 +12,13 @@ is known exactly at any size without running another MSM.  Covered here:
     parts with empty ones, part weights, thread reduction, long tasks, G2 without GLV), one fresh process each;
   - adversarial bucket contents: one point n times, P and -P, s and r - s, and +-G bases whose bucket counts make a
     running sum of the segment reduction hit the identity and equal the bucket it adds (quad and thread reduction);
-  - the W * n >= 2^32 guard, which must refuse before any allocation.
+  - the W * n >= 2^32 guard, which must refuse before any allocation;
+  - fixed-base tables at every window c = 2..24 (G1) and 2..20 (G2) with digit-pattern families, reaching all three
+    `wsplit` branches, a G2 table at 2^20, and the fold path's W * n >= 2^31 guard.
 A failure names the configuration, the family and the size.
 
-Measured on one H100 80GB HBM3 at a 700 W power limit: 279 s for the file, host oracle and subprocess start-up included."""
+Measured on one H100 80GB HBM3 at a 700 W power limit: 279 s for the file, host oracle and subprocess start-up included.
+The table section added later takes about 10 s (H100 80GB HBM3, 400 W power limit)."""
 import json
 import os
 import subprocess
@@ -375,3 +378,93 @@ def test_switch_matrix(env, spec):
     r = subprocess.run([sys.executable, "-c", SCRIPT % (ROOT, HERE, json.dumps(spec))], env=e, capture_output=True, text=True,
                        timeout=900, cwd=ROOT)
     assert r.returncode == 0 and "switch checks ok" in r.stdout, r.stdout[-2000:] + r.stderr[-4000:]
+
+
+# ---- 5. fixed-base tables: window sweep, G2 at 2^20, the fold guard -----------------------------------------------------
+TABLE_G1_WINDOWS = list(range(2, 25))
+TABLE_G2_WINDOWS = list(range(2, 21))
+PROVER_TABLE_WINDOWS = (7, 16, 22)           # B200ZK_PK_TABLE_WINDOW in test_gpu_prove_exact.py (32-bucket segment hint)
+
+
+def table_seg_len(c, hint=0):
+    """segment length of a fixed-base table MSM (one bucket set), as msm_dev_impl picks it without B200ZK_MSM_SEG"""
+    B = 1 << (c - 1)
+    seg = min(B, 16)
+    if B // seg <= 8192:                     # quad reduction: 8-bucket segments whatever the hint
+        return min(B, 8)
+    return hint if hint and hint <= B else seg
+
+
+def table_wsplit(c, seg_len):
+    """blocks that sum the segment partials of the single bucket set (msm_dev_impl, `wsplit`)"""
+    nseg = (1 << (c - 1)) // seg_len
+    return 16 if nseg >= 16 * 256 else (4 if nseg >= 1024 else 1)
+
+
+def test_table_sweep_reaches_every_wsplit():
+    pairs = [(c, table_seg_len(c)) for c in TABLE_G1_WINDOWS] + [(c, table_seg_len(c, 32)) for c in PROVER_TABLE_WINDOWS]
+    assert {table_wsplit(c, s) for c, s in pairs} == {1, 4, 16}, pairs
+    assert {table_wsplit(c, table_seg_len(c)) for c in TABLE_G2_WINDOWS} == {1, 4, 16}
+
+
+def _table_msm(net, bases, scalars, c, g2):
+    table = net.msm_table_build(bases, c, g2=g2)
+    return net.sum_points_dev(net.msm_table_dev(table, scalars, c, g2=g2), 1, g2=g2)
+
+
+def _table_sweep_one(net, c, g2):
+    import torch
+    what = "table %s c=%d wsplit=%d" % ("G2" if g2 else "G1", c, table_wsplit(c, table_seg_len(c)))
+    for n in (3001, 40000):
+        seed = 0xD0000000 + 1000 * c + n % 997 + (1 << 20) * g2
+        bases = net.generate_g2(seed, n) if g2 else net.generate_g1(seed, n)
+        scalars = net.generate_fr(seed ^ 0x7AB1E, n)
+        _check_point(_table_msm(net, bases, scalars, c, g2), dl.expected_msm(seed, _host(scalars), g2), "%s n=%d" % (what, n))
+    fams = dl.digit_families(c, glv=False)
+    seed = 0xD8000000 + c + (1 << 20) * g2
+    cnt = max(len(v) for v in fams.values())
+    bases = net.generate_g2(seed, cnt) if g2 else net.generate_g1(seed, cnt)
+    for name, ks in fams.items():
+        sc = layout.fr_to_arr(ks)
+        got = _table_msm(net, bases[: len(ks)].contiguous(), torch.from_numpy(sc.view(np.int64)).to(bases.device), c, g2)
+        _check_point(got, dl.expected_msm(seed, sc, g2), "%s family %s" % (what, name))
+
+
+@pytest.mark.parametrize("c", TABLE_G1_WINDOWS)
+def test_table_window_sweep_g1(net, c):
+    _table_sweep_one(net, c, False)
+
+
+@pytest.mark.parametrize("c", TABLE_G2_WINDOWS)
+def test_table_window_sweep_g2(net, c):
+    _table_sweep_one(net, c, True)
+
+
+def test_fixed_base_table_g2_2_20_c20(net):
+    import torch
+    n, seed = 1 << 20, 0xA3000020
+    bases = net.generate_g2(seed, n)
+    scalars = net.generate_fr(seed, n)
+    got = _table_msm(net, bases, scalars, 20, True)
+    _check_point(got, dl.expected_msm(seed, _host(scalars), True), "fixed-base table G2 n=2^20 c=20")
+    del bases
+    torch.cuda.empty_cache()
+
+
+def test_table_fold_guard_refuses_before_launch(net):
+    """c = 2 has 128 windows: 2^24 scalars make W * n = 2^31 table entries, past the fold path's 31-bit entry indices.
+    msm_dev_impl refuses before it allocates or launches anything, so the table buffer here is a placeholder."""
+    import ctypes
+    import torch
+    from distributed_groth16_b200 import _native
+    n = 1 << 24
+    assert net.msm_table_windows(2) * n == 1 << 31
+    scalars = net.generate_fr(11, n)
+    table = torch.zeros((16, 8), dtype=torch.int64, device=scalars.device)
+    out = torch.empty(16, dtype=torch.int64, device=scalars.device)
+    rc = net._lib.b200zk_msm_table_dev(net._h, 0, 0, ctypes.c_void_p(table.data_ptr()), ctypes.c_void_p(scalars.data_ptr()), n, 2,
+                                       ctypes.c_void_p(out.data_ptr()))
+    assert rc == _native.ERR_ARG, rc
+    assert "W * n" in net._lib.b200zk_last_error(net._h).decode()
+    del scalars
+    torch.cuda.empty_cache()
