@@ -99,6 +99,11 @@ SIGNATURES = {
     "b200zk_points_spmv_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, c_vp, c_vp, c_vp, ctypes.c_size_t, c_vp]),
     "b200zk_points_scale_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, ctypes.c_size_t, c_vp, c_vp]),
     "b200zk_points_intt_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, ctypes.c_uint, c_vp]),
+    "b200zk_points_mul_powers_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, ctypes.c_size_t, c_vp, c_vp, c_vp]),
+    "b200zk_points_encode_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, ctypes.c_size_t, ctypes.c_int, c_vp]),
+    "b200zk_blake2b512_init": (ctypes.c_int, [c_vp]),
+    "b200zk_blake2b512_update": (ctypes.c_int, [c_vp, c_vp, ctypes.c_size_t]),
+    "b200zk_blake2b512_final": (ctypes.c_int, [c_vp, c_vp]),
     "b200zk_fr_lincomb_dev": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, ctypes.c_size_t, c_vp]),
     "b200zk_g1_generate_dev": (ctypes.c_int, [c_vp, ctypes.c_uint64, ctypes.c_size_t, c_vp]),
     "b200zk_g2_generate_dev": (ctypes.c_int, [c_vp, ctypes.c_uint64, ctypes.c_size_t, c_vp]),

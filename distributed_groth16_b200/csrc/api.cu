@@ -1,6 +1,7 @@
 // api.cu -- the extern "C" surface declared in include/b200zk.h.
 #include <sstream>
 
+#include "blake2b.cuh"
 #include "common.cuh"
 
 using namespace b200zk;
@@ -729,6 +730,50 @@ int b200zk_points_intt_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_in
     B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
     return points_intt_dev(ctx, sl, g2, d_in, log_n, d_out);
 }
+int b200zk_points_mul_powers_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_points, size_t n, const uint64_t first[4],
+                                 const uint64_t ratio[4], void* d_out) {
+    if (!ctx) return B200ZK_ERR_ARG;
+    if (!valid_slot(stream) || !first || !ratio || (n && (!d_points || !d_out)))
+        return set_error(ctx, B200ZK_ERR_ARG, "points_mul_powers: null pointer or bad stream slot");
+    Slot& sl = ctx->slots[stream];
+    std::lock_guard<std::mutex> g(sl.mu);
+    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
+    return points_mul_powers_dev(ctx, sl, g2, d_points, n, first, ratio, d_out);
+}
+int b200zk_points_encode_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_affine, size_t n, int fmt, void* d_bytes) {
+    if (!ctx) return B200ZK_ERR_ARG;
+    if (!valid_slot(stream) || (n && (!d_affine || !d_bytes)))
+        return set_error(ctx, B200ZK_ERR_ARG, "points_encode: null pointer or bad stream slot");
+    Slot& sl = ctx->slots[stream];
+    std::lock_guard<std::mutex> g(sl.mu);
+    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
+    return points_encode_dev(ctx, sl, g2, d_affine, n, fmt, d_bytes);
+}
+
+// ---- Blake2b-512 with an exported state (csrc/blake2b.cuh): host only, no context --------------------------------------
+int b200zk_blake2b512_init(uint8_t state[216]) {
+    if (!state) return B200ZK_ERR_ARG;
+    blake2b_ctx c;
+    blake2b_init(&c, 64);
+    blake2b_export(&c, state);
+    return B200ZK_OK;
+}
+int b200zk_blake2b512_update(uint8_t state[216], const void* data, size_t len) {
+    if (!state || (len && !data)) return B200ZK_ERR_ARG;
+    blake2b_ctx c;
+    if (!blake2b_import(&c, state)) return B200ZK_ERR_ARG;
+    blake2b_update(&c, data, len);
+    blake2b_export(&c, state);
+    return B200ZK_OK;
+}
+int b200zk_blake2b512_final(const uint8_t state[216], uint8_t out[64]) {
+    if (!state || !out) return B200ZK_ERR_ARG;
+    blake2b_ctx c;
+    if (!blake2b_import(&c, state) || c.outlen != 64) return B200ZK_ERR_ARG;
+    blake2b_final(&c, out);
+    return B200ZK_OK;
+}
+
 int b200zk_fr_lincomb_dev(b200zk_ctx* ctx, const void* d_a, const void* d_b, const void* d_c, const uint64_t s[16], size_t n,
                           void* d_out) {
     if (!ctx || !s || (n && (!d_a || !d_b || !d_c || !d_out))) return B200ZK_ERR_ARG;

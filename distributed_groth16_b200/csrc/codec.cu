@@ -63,6 +63,41 @@ int points_compress_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_affine,
     return check_launch(ctx, "k_compress");
 }
 
+// ffjavascript encodings (codec.cuh ffjs_encode): the bytes a phase-1 contribution hashes, about 2.4 GB at power 22 --
+// one thread per point, since leaving Montgomery form is a field product per coordinate
+template <class F, bool COMPRESSED>
+__global__ void __launch_bounds__(128) k_points_encode(const affine_t<F>* in, size_t n, uint8_t* out) {
+    constexpr int LEN = (COMPRESSED ? 1 : 2) * (int)sizeof(F);
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    __align__(16) uint8_t b[LEN];
+    ffjs_encode<F, COMPRESSED>(ld16(in + i), b);
+    uint4* o = reinterpret_cast<uint4*>(out + i * LEN);
+#pragma unroll
+    for (int k = 0; k < LEN / 16; ++k) o[k] = *reinterpret_cast<const uint4*>(b + 16 * k);
+}
+
+int points_encode_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_affine, size_t n, int fmt, void* d_bytes) {
+    if (fmt != 0 && fmt != 1) return set_error(ctx, B200ZK_ERR_ARG, "points_encode: fmt must be 0 (uncompressed) or 1 (compressed)");
+    if (n == 0) return B200ZK_OK;
+    if (n >= ((size_t)1 << 31) * 128) return set_error(ctx, B200ZK_ERR_ARG, "points_encode: too many points");
+    const unsigned grid = (unsigned)((n + 127) / 128);
+    {
+        LaunchScope ls(ctx, sl.stream, "points_encode");
+        uint8_t* out = (uint8_t*)d_bytes;
+        if (g2) {
+            const affine_t<Fq2>* in = reinterpret_cast<const affine_t<Fq2>*>(d_affine);
+            if (fmt) k_points_encode<Fq2, true><<<grid, 128, 0, sl.stream>>>(in, n, out);
+            else k_points_encode<Fq2, false><<<grid, 128, 0, sl.stream>>>(in, n, out);
+        } else {
+            const affine_t<Fq>* in = reinterpret_cast<const affine_t<Fq>*>(d_affine);
+            if (fmt) k_points_encode<Fq, true><<<grid, 128, 0, sl.stream>>>(in, n, out);
+            else k_points_encode<Fq, false><<<grid, 128, 0, sl.stream>>>(in, n, out);
+        }
+    }
+    return check_launch(ctx, "k_points_encode");
+}
+
 int points_decompress_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_bytes, size_t n, int check_subgroup, void* d_affine,
                           size_t* n_invalid) {
     if (n_invalid) *n_invalid = 0;

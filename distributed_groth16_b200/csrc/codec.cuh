@@ -165,6 +165,37 @@ B2_HD void g1_encode(const affine_t<Fq>& p, uint8_t* b) {
     if (fq_is_larger(p.y)) b[31] |= 0x80;
 }
 
+// ---- ffjavascript's encodings (toRprUncompressed / toRprCompressed), the bytes snarkjs hashes in a phase-1 ceremony -----
+// canonical big-endian; an Fq2 element as c1 then c0
+B2_HD void ffjs_put(const Fq& am, uint8_t* out) {
+    const Fq a = Fq::from_mont(am);
+    for (int i = 0; i < 32; ++i) out[31 - i] = (uint8_t)(a.l[i >> 2] >> (8 * (i & 3)));
+}
+B2_HD void ffjs_put(const Fq2& a, uint8_t* out) {
+    ffjs_put(a.c1, out);
+    ffjs_put(a.c0, out + 32);
+}
+B2_HD bool is_larger(const Fq& y) { return fq_is_larger(y); }
+B2_HD bool is_larger(const Fq2& y) { return fq2_is_larger(y); }
+
+// COMPRESSED = false: x || y (64 / 128 bytes); true: x with 0x80 in byte 0 when y is the larger of (y, -y) (32 / 64
+// bytes).  Infinity: 0x40 then zeros in both.
+template <class F, bool COMPRESSED>
+B2_HD void ffjs_encode(const affine_t<F>& p, uint8_t* b) {
+    constexpr int FB = (int)sizeof(F), LEN = COMPRESSED ? FB : 2 * FB;
+    if (p.is_inf()) {
+        for (int k = 0; k < LEN; ++k) b[k] = 0;
+        b[0] = 0x40;
+        return;
+    }
+    ffjs_put(p.x, b);
+    if (COMPRESSED) {
+        if (is_larger(p.y)) b[0] |= 0x80;
+    } else {
+        ffjs_put(p.y, b + FB);
+    }
+}
+
 B2_HD void g2_encode(const affine_t<Fq2>& p, uint8_t* b) {
     if (p.is_inf()) {
         for (int k = 0; k < 64; ++k) b[k] = 0;

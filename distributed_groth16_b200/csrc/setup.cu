@@ -410,21 +410,10 @@ static int naf5(unsigned __int128 k, int8_t* d) {
     return top;
 }
 
-int points_scale_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_points, size_t n, const uint64_t k64[4], void* d_out) {
-    if (n == 0) return B200ZK_OK;
-    uint32_t k[8];
+// 4 u64 limbs of a plain integer < 2^256 -> 8 u32 limbs of it mod r (k < 2^256 < 6 r)
+static void reduce_mod_r(const uint64_t k64[4], uint32_t k[8]) {
     for (int i = 0; i < 4; ++i) { k[2 * i] = (uint32_t)k64[i]; k[2 * i + 1] = (uint32_t)(k64[i] >> 32); }
-    if (g2) {
-        ScaleK sk;
-        memcpy(sk.k, k, sizeof(k));
-        {
-            LaunchScope ls(ctx, sl.stream, "points_scale_g2");
-            k_points_scale_g2_ladder<<<(unsigned)((n + 127) / 128), 128, 0, sl.stream>>>(
-                sk, reinterpret_cast<const affine_t<Fq2>*>(d_points), n, reinterpret_cast<affine_t<Fq2>*>(d_out));
-        }
-        return check_launch(ctx, "k_points_scale_g2");
-    }
-    for (;;) {                                          // k mod r: k < 2^256 < 6 r
+    for (;;) {
         bool ge = true;
         for (int i = 7; i >= 0; --i) {
             if (k[i] != FrParams::mod(i)) { ge = k[i] > FrParams::mod(i); break; }
@@ -437,6 +426,23 @@ int points_scale_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_points, si
             br = v >> 32;
         }
     }
+}
+
+int points_scale_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_points, size_t n, const uint64_t k64[4], void* d_out) {
+    if (n == 0) return B200ZK_OK;
+    uint32_t k[8];
+    if (g2) {
+        for (int i = 0; i < 4; ++i) { k[2 * i] = (uint32_t)k64[i]; k[2 * i + 1] = (uint32_t)(k64[i] >> 32); }
+        ScaleK sk;
+        memcpy(sk.k, k, sizeof(k));
+        {
+            LaunchScope ls(ctx, sl.stream, "points_scale_g2");
+            k_points_scale_g2_ladder<<<(unsigned)((n + 127) / 128), 128, 0, sl.stream>>>(
+                sk, reinterpret_cast<const affine_t<Fq2>*>(d_points), n, reinterpret_cast<affine_t<Fq2>*>(d_out));
+        }
+        return check_launch(ctx, "k_points_scale_g2");
+    }
+    reduce_mod_r(k64, k);
     const GlvSplit sp = glv_decompose(k);
     ScaleDigits dg;
     int top = -1;
@@ -480,31 +486,38 @@ constexpr int INTT_TAB = 8;               // P, 2P, .., 8P
 constexpr int INTT_BLOCK_G1 = 64;
 constexpr int INTT_BLOCK_G2 = 32;         // the G2 table (8 x 128 B per thread) fills 32 KB of shared memory at 32 threads
 
+// the scalar of one product of the point iNTT (a twiddle) or of points_mul_powers (first ratio^i) in the form
+// glv_table_mul<F, B, 4> takes
 struct __align__(16) TwiddleDigits {
     int8_t d[2][INTT_WINDOWS];            // d[h][w]: window w (weight 16^w) of k1 (h = 0) / k2 (h = 1), signs folded in
 };
 
-// digits of w_n^-i for i < count
-__global__ void k_intt_twiddle_digits(unsigned log_n, size_t count, TwiddleDigits* out) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= count) return;
-    const Fr t = Fr::from_mont(Fr::pow_u64(fr_root_of_unity(log_n, true), i));
-    const GlvSplit sp = glv_decompose(t.l);
+// k (canonical, < r) -> GLV halves, each recoded into 32 signed 4-bit windows in [-7, 8] (a window above 8 borrows 16 from
+// the next one; |k1|, |k2| < 2^127 leave no carry out of the top window)
+__device__ __forceinline__ TwiddleDigits glv_window_digits(const Fr& k) {
+    const GlvSplit sp = glv_decompose(k.l);
     TwiddleDigits dg;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-        const uint32_t* k = h ? sp.k2 : sp.k1;
+        const uint32_t* w = h ? sp.k2 : sp.k1;
         const bool neg = h ? sp.neg2 : sp.neg1;
         int carry = 0;
 #pragma unroll
         for (int q = 0; q < INTT_WINDOWS; ++q) {
-            int v = (int)((k[q >> 3] >> ((q & 7) * 4)) & 15) + carry;
+            int v = (int)((w[q >> 3] >> ((q & 7) * 4)) & 15) + carry;
             carry = v > 8;
             if (carry) v -= 16;
             dg.d[h][q] = (int8_t)(neg ? -v : v);
         }
     }
-    st16(out + i, dg);
+    return dg;
+}
+
+// digits of w_n^-i for i < count
+__global__ void k_intt_twiddle_digits(unsigned log_n, size_t count, TwiddleDigits* out) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    st16(out + i, glv_window_digits(Fr::from_mont(Fr::pow_u64(fr_root_of_unity(log_n, true), i))));
 }
 
 // out[i] = in[bitrev(i)]; each pair is handled by one thread that reads both before writing, so out may equal in
@@ -517,6 +530,24 @@ __global__ void k_points_bitrev(const affine_t<F>* in, affine_t<F>* out, unsigne
     const affine_t<F> x = ld16(in + i), y = ld16(in + r);
     st16(out + i, y);
     if (r != i) st16(out + r, x);
+}
+
+// this thread's table P, 2P, .., 8P for glv_table_mul<F, B, 4>, normalised with block-batched inversions; mul = false
+// leaves entries 1..7 at infinity (P is not multiplied).  The table is built from shared memory copies only: P and the
+// products stay out of registers during the loop.  All threads call it.
+template <class F, int B>
+__device__ __forceinline__ void build_mul_table(uint4* tab, const affine_t<F>& P, bool mul, F* pre, F* suf, F* tot) {
+    tab_put<F, B>(tab, 0, P);
+    xyzz_t<F> run = xyzz_t<F>::identity();
+#pragma unroll 1
+    for (int e = 1; e < INTT_TAB; ++e) {                                 // (e + 1) P
+        if (mul) {
+            const affine_t<F> Q = tab_get<F, B>(tab, 0);
+            if (e == 1) run = xyzz_t<F>::dbl_affine(Q.x, Q.y);
+            else xyzz_t<F>::madd(run, Q, false);
+        }
+        tab_put<F, B>(tab, e, block_to_affine<F, B>(run, mul, pre, suf, tot));
+    }
 }
 
 // pass with half-size m = 2^log_m: butterfly t = (j, g), j = t >> lg, g = t mod 2^lg (lg = log2(n / 2m)), on the
@@ -534,22 +565,9 @@ __global__ void __launch_bounds__(B) k_points_intt_pass(affine_t<F>* a, const Tw
     const size_t ia = ((t & (((size_t)1 << lg) - 1)) << (log_m + 1)) + j, ib = ia + ((size_t)1 << log_m);
     bool mul = false;
     if (!__syncthreads_and(!live || j == 0)) {                           // block-uniform
-        // the table is built from shared memory copies only: P and the products stay out of registers during the loop
-        {
-            const affine_t<F> P = live ? ld16(a + ib) : affine_t<F>::infinity();
-            mul = live && j != 0 && !P.is_inf();
-            tab_put<F, B>(tab, 0, P);
-        }
-        xyzz_t<F> run = xyzz_t<F>::identity();
-#pragma unroll 1
-        for (int e = 1; e < INTT_TAB; ++e) {                             // (e + 1) P
-            if (mul) {
-                const affine_t<F> P = tab_get<F, B>(tab, 0);
-                if (e == 1) run = xyzz_t<F>::dbl_affine(P.x, P.y);
-                else xyzz_t<F>::madd(run, P, false);
-            }
-            tab_put<F, B>(tab, e, block_to_affine<F, B>(run, mul, pre, suf, &tot));
-        }
+        const affine_t<F> P = live ? ld16(a + ib) : affine_t<F>::infinity();
+        mul = live && j != 0 && !P.is_inf();
+        build_mul_table<F, B>(tab, P, mul, pre, suf, &tot);
     }
     xyzz_t<F> prod = xyzz_t<F>::identity();
     if (mul) glv_table_mul<F, B, 4>(prod, tab, tw[j << lg].d[0], tw[j << lg].d[1], INTT_WINDOWS - 1);
@@ -655,6 +673,88 @@ static int points_intt_impl(b200zk_ctx* ctx, Slot& sl, int g2, const affine_t<F>
 int points_intt_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_in, unsigned log_n, void* d_out) {
     return g2 ? points_intt_impl<Fq2, INTT_BLOCK_G2>(ctx, sl, 1, (const affine_t<Fq2>*)d_in, log_n, (affine_t<Fq2>*)d_out)
               : points_intt_impl<Fq, INTT_BLOCK_G1>(ctx, sl, 0, (const affine_t<Fq>*)d_in, log_n, (affine_t<Fq>*)d_out);
+}
+
+// ---- each point times its own term of a geometric sequence: out[i] = (first ratio^i) points[i]  (snarkjs `powersoftau
+// contribute`, ffjavascript G.batchApplyKey) -------------------------------------------------------------------------------
+// The whole cost of a phase-1 contribution; orchestration in groth16/phase1.py.  The scalars differ per point, so the
+// point iNTT's product is reused as it stands: a digit kernel makes first ratio^i on the device and recodes it with
+// glv_window_digits into a workspace (64 bytes per point), then every thread runs the same 32 x (4 doublings + 2 mixed
+// additions) over its table P..8P.  The digits are read straight from the workspace: a thread's 64 bytes sit in one cache
+// line, and the reads are two bytes per 4 doublings + 2 additions.
+struct PowersConsts { Fr first, ratio; };        // canonical (reduced mod r), turned into Montgomery form on the device
+
+__global__ void k_powers_digits(const __grid_constant__ PowersConsts c, size_t count, TwiddleDigits* out) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    st16(out + i, glv_window_digits(Fr::from_mont(Fr::pow_u64(Fr::to_mont(c.ratio), i, Fr::to_mont(c.first)))));
+}
+
+template <class F, int B>
+__global__ void __launch_bounds__(B) k_points_mul_powers(const affine_t<F>* points, const TwiddleDigits* __restrict__ dg,
+                                                         size_t n, affine_t<F>* out) {
+    constexpr int C = sizeof(affine_t<F>) / 16;
+    __shared__ uint4 tab[INTT_TAB * C * B];
+    __shared__ F pre[B], suf[B], tot;
+    const size_t i = (size_t)blockIdx.x * B + threadIdx.x;
+    bool mul;
+    {
+        const affine_t<F> P = i < n ? ld16(points + i) : affine_t<F>::infinity();
+        mul = !P.is_inf();
+        build_mul_table<F, B>(tab, P, mul, pre, suf, &tot);
+    }
+    xyzz_t<F> prod = xyzz_t<F>::identity();
+    if (mul) glv_table_mul<F, B, 4>(prod, tab, dg[i].d[0], dg[i].d[1], INTT_WINDOWS - 1);
+    const affine_t<F> r = block_to_affine<F, B>(prod, !prod.is_inf(), pre, suf, &tot);
+    if (i < n) st16(out + i, r);
+}
+
+template <class F, int B>
+static int points_mul_powers_impl(b200zk_ctx* ctx, Slot& sl, const affine_t<F>* d_points, size_t n, const uint64_t first[4],
+                                  const uint64_t ratio[4], affine_t<F>* d_out) {
+    if (n == 0) return B200ZK_OK;
+    if (n >= ((size_t)1 << 31) * B) return set_error(ctx, B200ZK_ERR_ARG, "points_mul_powers: too many points");
+    cudaStream_t st = sl.stream;
+    PowersConsts c;
+    reduce_mod_r(first, c.first.l);
+    reduce_mod_r(ratio, c.ratio.l);
+    TwiddleDigits* dg = nullptr;
+    {
+        const cudaError_t e = cudaMalloc(&dg, n * sizeof(TwiddleDigits));
+        if (e != cudaSuccess) {
+            cudaGetLastError();                                           // nothing was launched: leave no error behind
+            char b[256];
+            snprintf(b, sizeof(b), "points_mul_powers: the scalar digits of %zu points (%zu MB of device memory) do not fit: %s",
+                     n, n * sizeof(TwiddleDigits) >> 20, cudaGetErrorString(e));
+            return set_error(ctx, e == cudaErrorMemoryAllocation ? B200ZK_ERR_OOM : B200ZK_ERR_CUDA, b);
+        }
+    }
+    auto run = [&]() -> int {
+        {
+            LaunchScope ls(ctx, st, "powers_digits");
+            k_powers_digits<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, n, dg);
+        }
+        B2_TRY(check_launch(ctx, "k_powers_digits"));
+        {
+            LaunchScope ls(ctx, st, sizeof(F) > 32 ? "points_mul_powers_g2" : "points_mul_powers_g1");
+            k_points_mul_powers<F, B><<<(unsigned)((n + B - 1) / B), B, 0, st>>>(d_points, dg, n, d_out);
+        }
+        return check_launch(ctx, "k_points_mul_powers");
+    };
+    const int rc = run();
+    const cudaError_t e = cudaStreamSynchronize(st);                     // the digits are freed below
+    cudaFree(dg);
+    if (rc != B200ZK_OK) return rc;
+    B2_CUDA_OK(ctx, e);
+    return B200ZK_OK;
+}
+
+int points_mul_powers_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_points, size_t n, const uint64_t first[4],
+                          const uint64_t ratio[4], void* d_out) {
+    return g2 ? points_mul_powers_impl<Fq2, INTT_BLOCK_G2>(ctx, sl, (const affine_t<Fq2>*)d_points, n, first, ratio,
+                                                           (affine_t<Fq2>*)d_out)
+              : points_mul_powers_impl<Fq, INTT_BLOCK_G1>(ctx, sl, (const affine_t<Fq>*)d_points, n, first, ratio,
+                                                          (affine_t<Fq>*)d_out);
 }
 
 }  // namespace b200zk

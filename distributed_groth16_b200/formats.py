@@ -272,6 +272,9 @@ class PTau:
         """(byte offset, length) of section sid in the file."""
         return self._secs[sid]
 
+    def has_section(self, sid: int) -> bool:
+        return sid in self._secs
+
     def section_chunks(self, sid: int, chunk: int = 1 << 26):
         """The bytes of section sid, in copies of at most `chunk` bytes."""
         off, ln = self._secs[sid]
@@ -327,6 +330,77 @@ def read_ptau(path: str) -> PTau:
     return PTau(path)
 
 
+def ptau_preamble(n_sections: int, power: int) -> bytes:
+    """The first bytes of every ptau file this package writes: magic, version 1, the section count and section 1 =
+    (n8 = 32, q, power, ceremonyPower = power) -- what snarkjs' writePTauHeader(curve, power) writes as far as is known
+    here (not checked against snarkjs)."""
+    s1 = struct.pack("<I", 32) + FQ_MODULUS.to_bytes(32, "little") + struct.pack("<II", power, power)
+    return b"ptau" + struct.pack("<II", 1, n_sections) + struct.pack("<IQ", 1, len(s1)) + s1
+
+
+class PTauWriter:
+    """Streams a phase-1 ceremony file (snarkjs `powersoftau new` / `contribute` / `beacon` output) of `power` (1..27) to
+    `path`: sections 1-7 in that order.  Section 1 is ptau_preamble's; sections 2-6 are appended in chunks through
+    write(sid, data) in file order, each exactly PTau.tau_section_bytes(power) long; section 7 (the contribution records,
+    ptau_contributions_bytes) is written whole by write_contributions() once 2-6 are complete.  Every length is checked:
+    close() raises ValueError for a file left short."""
+
+    def __init__(self, path: str, power: int):
+        if not 1 <= power <= PTau.MAX_UNPREPARED_POWER:
+            raise ValueError("ptau power must be in 1..%d, got %d" % (PTau.MAX_UNPREPARED_POWER, power))
+        self.power = power
+        self._lengths = PTau.tau_section_bytes(power)
+        self._sid, self._left = 1, 0              # section being written and bytes it still needs
+        self.section_offsets = {}                 # section -> file offset of its first byte, once begun
+        self._f = open(path, "wb")
+        try:
+            self._f.write(ptau_preamble(7, power))
+        except BaseException:
+            self._f.close()
+            raise
+
+    def write(self, sid: int, data) -> None:
+        """Append `data` (bytes or a u64 array of points) to section sid (2..6); sections come in order, each complete
+        before the next begins."""
+        data = memoryview(np.ascontiguousarray(data) if isinstance(data, np.ndarray) else data).cast("B")
+        if sid != self._sid:
+            if self._left or sid != self._sid + 1 or not 2 <= sid <= 6:
+                raise ValueError("ptau section %d out of order (section %d has %d bytes to go)" % (sid, self._sid, self._left))
+            self._sid, self._left = sid, self._lengths[sid]
+            self._f.write(struct.pack("<IQ", sid, self._left))
+            self.section_offsets[sid] = self._f.tell()
+        if data.nbytes > self._left:
+            raise ValueError("ptau section %d: %d bytes more than its %d" % (sid, data.nbytes - self._left, self._lengths[sid]))
+        self._f.write(data)
+        self._left -= data.nbytes
+
+    def flush(self) -> None:
+        """Push what was written so far to the file, so that it can be read back while the writer stays open."""
+        self._f.flush()
+
+    def write_contributions(self, sec7: bytes) -> None:
+        if self._sid != 6 or self._left:
+            raise ValueError("ptau section 7 before sections 2-6 are complete")
+        self._f.write(struct.pack("<IQ", 7, len(sec7)) + bytes(sec7))
+        self._sid = 7
+
+    def close(self) -> None:
+        f, self._f = self._f, None
+        if f is None:
+            return
+        f.close()
+        if self._sid != 7:
+            raise ValueError("ptau incomplete: stopped in section %d" % self._sid)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        f, self._f = self._f, None
+        if f is not None:
+            f.close()
+
+
 class PreparedPTauWriter:
     """Streams the output of snarkjs `powersoftau prepare phase2` for an open ceremony `src` (a PTau, prepared or not) to
     `path`: 11 sections in the order 1, 2-7, 12-15.  Section 1 is restated as (n8, q, power, ceremonyPower = power) -- what
@@ -341,8 +415,7 @@ class PreparedPTauWriter:
         self._next = 0
         self._f = open(path, "wb")
         try:
-            s1 = struct.pack("<I", 32) + FQ_MODULUS.to_bytes(32, "little") + struct.pack("<II", self.power, self.power)
-            self._f.write(b"ptau" + struct.pack("<II", 1, 11) + struct.pack("<IQ", 1, len(s1)) + s1)
+            self._f.write(ptau_preamble(11, self.power))
             for sid in (2, 3, 4, 5, 6, 7):
                 self._f.write(struct.pack("<IQ", sid, src.section_span(sid)[1]))
                 for part in src.section_chunks(sid):
@@ -441,34 +514,136 @@ def parse_mpc_params(sec: bytes) -> MPCParams:
         p, end = off, off + plen
         c = Contribution(delta_after=pts[:8], g1_s=pts[8:16], g1_sx=pts[16:24], g2_spx=pts[24:40], transcript=transcript,
                          type=ctype)
-        while p < end:
-            key = sec[p]
-            if key == 1:
-                if p + 2 > end or p + 2 + sec[p + 1] > end:
-                    raise FormatError("contribution %d: name runs past its parameters" % i)
-                ln = sec[p + 1]
-                if ln > _MPC_NAME_MAX:
-                    raise FormatError("contribution %d: name of %d bytes (at most %d)" % (i, ln, _MPC_NAME_MAX))
-                try:
-                    c.name = sec[p + 2:p + 2 + ln].decode("utf-8")
-                except UnicodeDecodeError as e:
-                    raise FormatError("contribution %d: name is not UTF-8 (%s)" % (i, e)) from None
-                p += 2 + ln
-            elif key == 2:
-                if p + 2 > end:
-                    raise FormatError("contribution %d: numIterationsExp runs past its parameters" % i)
-                c.num_iterations_exp = sec[p + 1]
-                p += 2
-            elif key == 3:
-                if p + 2 > end or p + 2 + sec[p + 1] > end:
-                    raise FormatError("contribution %d: beacon hash runs past its parameters" % i)
-                c.beacon_hash = sec[p + 2:p + 2 + sec[p + 1]]
-                p += 2 + sec[p + 1]
-            else:
-                raise FormatError("contribution %d: unknown parameter key %d" % (i, key))
+        _read_params(sec, p, end, i, c)
         off = end
         out.append(c)
     return MPCParams(cs_hash=cs_hash, contributions=out)
+
+
+def _read_params(sec: bytes, p: int, end: int, i: int, c) -> None:
+    """The key / value parameters of contribution i in sec[p:end] into c.name, c.num_iterations_exp and c.beacon_hash
+    (the same stream in a zkey's section 10 and a ptau's section 7)."""
+    while p < end:
+        key = sec[p]
+        if key == 1:
+            if p + 2 > end or p + 2 + sec[p + 1] > end:
+                raise FormatError("contribution %d: name runs past its parameters" % i)
+            ln = sec[p + 1]
+            if ln > _MPC_NAME_MAX:
+                raise FormatError("contribution %d: name of %d bytes (at most %d)" % (i, ln, _MPC_NAME_MAX))
+            try:
+                c.name = sec[p + 2:p + 2 + ln].decode("utf-8")
+            except UnicodeDecodeError as e:
+                raise FormatError("contribution %d: name is not UTF-8 (%s)" % (i, e)) from None
+            p += 2 + ln
+        elif key == 2:
+            if p + 2 > end:
+                raise FormatError("contribution %d: numIterationsExp runs past its parameters" % i)
+            c.num_iterations_exp = sec[p + 1]
+            p += 2
+        elif key == 3:
+            if p + 2 > end or p + 2 + sec[p + 1] > end:
+                raise FormatError("contribution %d: beacon hash runs past its parameters" % i)
+            c.beacon_hash = sec[p + 2:p + 2 + sec[p + 1]]
+            p += 2 + sec[p + 1]
+        else:
+            raise FormatError("contribution %d: unknown parameter key %d" % (i, key))
+
+
+def _params_bytes(c) -> bytes:
+    """The parameter stream of a record (inverse of _read_params): name, then for a beacon (type 1) its parameters."""
+    prm = b""
+    if c.name:
+        name = c.name.encode("utf-8")
+        if len(name) > _MPC_NAME_MAX:
+            raise FormatError("contribution name of %d bytes (at most %d)" % (len(name), _MPC_NAME_MAX))
+        prm += bytes([1, len(name)]) + name
+    if c.type == 1:
+        if c.num_iterations_exp is None or c.beacon_hash is None or len(c.beacon_hash) > 255:
+            raise FormatError("a beacon record needs numIterationsExp and a beacon hash of at most 255 bytes")
+        prm += bytes([2, c.num_iterations_exp, 3, len(c.beacon_hash)]) + bytes(c.beacon_hash)
+    return prm
+
+
+@dataclass
+class PTauContribution:
+    """One phase-1 record of a ptau's section 7 (snarkjs `powersoftau contribute` / `beacon`).  Points are Montgomery
+    little-endian affine limb arrays (G1 8, G2 16 u64 limbs; infinity all-zero).  key[name] for name in "tau", "alpha",
+    "beta" holds the proof of knowledge of that secret x: g1_s, g1_sx = x g1_s (G1) and g2_spx = x g2_sp (G2), where g2_sp
+    is hashed from the previous challenge and is not stored."""
+    tau_g1: np.ndarray             # tau G1 after this contribution (point 1 of section 2)
+    tau_g2: np.ndarray             # point 1 of section 3
+    alpha_g1: np.ndarray           # point 0 of section 4
+    beta_g1: np.ndarray            # point 0 of section 5
+    beta_g2: np.ndarray            # the point of section 6
+    key: dict                      # "tau" / "alpha" / "beta" -> {"g1_s", "g1_sx", "g2_spx"}
+    partial_hash: bytes            # 216 bytes: the response hasher's state after the points (see csrc/blake2b.cuh)
+    next_challenge: bytes          # 64 bytes
+    type: int = 0                  # 0 = contribution, 1 = beacon
+    name: str | None = None
+    num_iterations_exp: int | None = None
+    beacon_hash: bytes | None = None
+
+
+_KEY_NAMES = ("tau", "alpha", "beta")
+_PTAU_POINTS_U64 = (8 + 16 + 8 + 8 + 16) + 6 * 8 + 3 * 16          # record points, then the public key: 152 u64
+_PTAU_REC = _PTAU_POINTS_U64 * 8 + 216 + 64 + 8                    # fixed part of one record: 1504 bytes
+
+
+def parse_ptau_contributions(sec: bytes) -> list:
+    """Section 7 bytes of a ptau -> [PTauContribution], oldest first.  Layout (restated from snarkjs powersoftau_utils
+    writeContribution, NOT checked against a file snarkjs wrote): u32 count, then per record tauG1, tauG2, alphaG1,
+    betaG1, betaG2, the public key tau.g1_s, tau.g1_sx, alpha.g1_s, alpha.g1_sx, beta.g1_s, beta.g1_sx, tau.g2_spx,
+    alpha.g2_spx, beta.g2_spx (all Montgomery LE), partialHash (216 bytes), nextChallenge (64 bytes), u32 type, u32 byte
+    length of the key / value parameters (as in a zkey's section 10: 1 = name, 2 = numIterationsExp, 3 = beacon hash).
+    Raises FormatError for a truncated section, a count that runs past it, an unknown parameter key or an over-long
+    name."""
+    sec = bytes(sec)
+
+    def need(off, n, what):
+        if off + n > len(sec):
+            raise FormatError("ptau section 7 ends inside %s (%d + %d > %d bytes)" % (what, off, n, len(sec)))
+
+    need(0, 4, "the contribution count")
+    count = struct.unpack_from("<I", sec, 0)[0]
+    if 4 + count * _PTAU_REC > len(sec):
+        raise FormatError("ptau section 7 claims %d contributions, more than its %d bytes hold" % (count, len(sec)))
+    off, out = 4, []
+    for i in range(count):
+        need(off, _PTAU_REC, "contribution %d" % i)
+        pts = np.frombuffer(sec, dtype="<u8", count=_PTAU_POINTS_U64, offset=off).copy()
+        off += _PTAU_POINTS_U64 * 8
+        g1s = [pts[56 + 8 * k:64 + 8 * k] for k in range(6)]
+        g2s = [pts[104 + 16 * k:120 + 16 * k] for k in range(3)]
+        key = {nm: {"g1_s": g1s[2 * k], "g1_sx": g1s[2 * k + 1], "g2_spx": g2s[k]} for k, nm in enumerate(_KEY_NAMES)}
+        partial, nxt = sec[off:off + 216], sec[off + 216:off + 280]
+        ctype, plen = struct.unpack_from("<II", sec, off + 280)
+        off += 288
+        need(off, plen, "the parameters of contribution %d" % i)
+        c = PTauContribution(tau_g1=pts[0:8], tau_g2=pts[8:24], alpha_g1=pts[24:32], beta_g1=pts[32:40], beta_g2=pts[40:56],
+                             key=key, partial_hash=partial, next_challenge=nxt, type=ctype)
+        _read_params(sec, off, off + plen, i, c)
+        off += plen
+        out.append(c)
+    return out
+
+
+def ptau_contributions_bytes(contributions) -> bytes:
+    """[PTauContribution] -> section 7 bytes (the inverse of parse_ptau_contributions)."""
+    out = [struct.pack("<I", len(contributions))]
+    for c in contributions:
+        flat = lambda a: np.ascontiguousarray(a, dtype="<u8").reshape(-1)
+        pts = [flat(a) for a in (c.tau_g1, c.tau_g2, c.alpha_g1, c.beta_g1, c.beta_g2)]
+        pts += [flat(c.key[nm][f]) for nm in _KEY_NAMES for f in ("g1_s", "g1_sx")]
+        pts += [flat(c.key[nm]["g2_spx"]) for nm in _KEY_NAMES]
+        if [p.size for p in pts] != [8, 16, 8, 8, 16] + [8] * 6 + [16] * 3:
+            raise FormatError("phase-1 record points must be G1 (8 limbs) and G2 (16 limbs) as the layout says")
+        if len(c.partial_hash) != 216 or len(c.next_challenge) != 64:
+            raise FormatError("partialHash must be 216 bytes and nextChallenge 64")
+        prm = _params_bytes(c)
+        out += [b"".join(p.tobytes() for p in pts), bytes(c.partial_hash), bytes(c.next_challenge),
+                struct.pack("<II", c.type, len(prm)), prm]
+    return b"".join(out)
 
 
 def read_mpc_params(zkey_bytes: bytes) -> MPCParams:
@@ -491,16 +666,7 @@ def mpc_params_bytes(params: MPCParams) -> bytes:
         pts = [np.ascontiguousarray(a, dtype="<u8").reshape(-1) for a in (c.delta_after, c.g1_s, c.g1_sx, c.g2_spx)]
         if [p.size for p in pts] != [8, 8, 8, 16] or len(c.transcript) != 64:
             raise FormatError("contribution points must be 8, 8, 8 and 16 limbs and the transcript 64 bytes")
-        prm = b""
-        if c.name:
-            name = c.name.encode("utf-8")
-            if len(name) > _MPC_NAME_MAX:
-                raise FormatError("contribution name of %d bytes (at most %d)" % (len(name), _MPC_NAME_MAX))
-            prm += bytes([1, len(name)]) + name
-        if c.type == 1:
-            if c.num_iterations_exp is None or c.beacon_hash is None or len(c.beacon_hash) > 255:
-                raise FormatError("a beacon record needs numIterationsExp and a beacon hash of at most 255 bytes")
-            prm += bytes([2, c.num_iterations_exp, 3, len(c.beacon_hash)]) + bytes(c.beacon_hash)
+        prm = _params_bytes(c)
         out += [b"".join(p.tobytes() for p in pts), bytes(c.transcript), struct.pack("<II", c.type, len(prm)), prm]
     return b"".join(out)
 

@@ -32,6 +32,43 @@ def ptau_prepare_phase2(net: Net, src_path: str, dst_path: str) -> None:
     ptau.prepare_phase2(net, src_path, dst_path)
 
 
+def ptau_new(path: str, power: int) -> None:
+    """snarkjs `powersoftau new bn128 <power>` (power 1..27): a phase-1 ceremony file with the generators in every slot
+    and no contributions (phase1.new; file writing only)."""
+    from . import phase1
+    phase1.new(path, power)
+
+
+def ptau_contribute(net: Net, src_path: str, dst_path: str, name: str | None = None, entropy: str = ""):
+    """snarkjs `powersoftau contribute <src> <dst>` on the GPU: the key is drawn, as snarkjs getRandomRng does, from a
+    ChaCha seeded with Blake2b-512(os.urandom(64) || UTF-8 entropy); the secrets are dropped on return.  Returns
+    (responseHash, nextChallenge)."""
+    import hashlib
+    import os
+    from . import phase1, phase2
+    rng = phase2.ChaCha.from_hash(hashlib.blake2b(os.urandom(64) + str(entropy).encode("utf-8"), digest_size=64).digest())
+    return phase1.contribute(net, src_path, dst_path, rng, name=name)
+
+
+def ptau_beacon(net: Net, src_path: str, dst_path: str, beacon_hash: bytes, num_iterations_exp: int,
+                name: str | None = None):
+    """snarkjs `powersoftau beacon <src> <dst> <hash> <e>`: the final, publicly reproducible contribution (2^e SHA-256
+    rounds on the host).  Returns (responseHash, nextChallenge)."""
+    from . import phase1
+    if not 10 <= int(num_iterations_exp) <= 63:
+        raise ValueError("num_iterations_exp must be in 10..63, got %d" % num_iterations_exp)
+    if len(beacon_hash) > 255:
+        raise ValueError("beacon hash longer than 255 bytes")
+    return phase1.beacon(net, src_path, dst_path, bytes(beacon_hash), int(num_iterations_exp), name=name)
+
+
+def ptau_verify(net: Net, ptau_path: str):
+    """snarkjs `powersoftau verify <ptau>` on the GPU: -> phase1.Phase1Report (ok, one failure line per check that does
+    not hold, naming the contribution or section; per record its name, type and nextChallenge)."""
+    from . import phase1
+    return phase1.verify(net, ptau_path)
+
+
 def ptau_check_lagrange(net: Net, ptau_path: str):
     """The Lagrange part of snarkjs `powersoftau verify` on a prepared file: -> ptau.LagrangeReport (ok, one failure line
     per section and level that does not check).  Needs no toxic waste."""

@@ -108,6 +108,14 @@ class ChaCha:
     def next_bool(self) -> bool:
         return (self.next_u32() & 1) == 1
 
+    def snapshot(self):
+        """The position in the stream, for restore(): the block counter, the current block and the index into it."""
+        return list(self._state), self._buf, self._idx
+
+    def restore(self, snap) -> None:
+        state, buf, idx = snap
+        self._state, self._buf, self._idx = list(state), buf, idx
+
 
 def field_from_rng(rng: ChaCha, modulus: int) -> int:
     """F.fromRng: the Montgomery REPRESENTATION v of the drawn element (the element itself is v R^-1 mod modulus)."""
@@ -208,10 +216,13 @@ def _same_ratio(net, p1, p2, q1, q2) -> bool:
 def _from_rng(net, rng: ChaCha, g2: bool) -> np.ndarray:
     """G.fromRng (see the module docstring).  Candidates are drawn from the RNG in order and decompressed on the device
     in batches (b200zk_points_decompress_dev, check_subgroup = 0: an invalid slot means x^3 + b is not a square); the
-    first valid one is the result, so the RNG may be read past it -- callers draw nothing after a fromRng."""
+    first valid one is the result.  The RNG is left right after the accepted candidate's last word, as a one-at-a-time
+    fromRng leaves it (a phase-1 key draws three G1.fromRng from one RNG): the position after each candidate is saved
+    and the winner's restored."""
     import torch
     while True:
         enc = bytearray()
+        after = []
         for _ in range(_CANDIDATES):
             if g2:
                 c0 = field_from_rng(rng, Q) * _RINV_Q % Q
@@ -222,6 +233,7 @@ def _from_rng(net, rng: ChaCha, g2: bool) -> np.ndarray:
             if rng.next_bool():
                 b[-1] |= 0x80
             enc += b
+            after.append(rng.snapshot())
         data = torch.from_numpy(np.frombuffer(bytes(enc), dtype=np.uint8).copy()).to(net._dev())
         out = torch.empty((_CANDIDATES, 16 if g2 else 8), dtype=torch.int64, device=data.device)
         bad = ctypes.c_size_t(0)
@@ -233,6 +245,7 @@ def _from_rng(net, rng: ChaCha, g2: bool) -> np.ndarray:
         for i in range(_CANDIDATES):
             if pts[i].any():
                 p = pts[i].copy()
+                rng.restore(after[i])
                 return _scale_one(net, p, G2_COFACTOR, g2=True) if g2 else p
 
 

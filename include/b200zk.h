@@ -266,6 +266,31 @@ int b200zk_points_scale_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_p
  * Temporary device memory: 2^(log_n - 1) x 64 bytes, allocated before anything is launched (B200ZK_ERR_OOM with a message
  * when it does not fit).  log_n > 28: B200ZK_ERR_DOMAIN; a null pointer: B200ZK_ERR_ARG.  Returns once out is complete. */
 int b200zk_points_intt_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_in, unsigned log_n, void* d_out);
+/* out[i] = (first * ratio^i) * points[i], i < n: the step of a snarkjs `powersoftau contribute` that multiplies every point
+ * of a ceremony section by its own power of the secret (ffjavascript G.batchApplyKey).  first, ratio: 4 u64 limbs, plain
+ * little-endian integers (reduced mod r by the call, like b200zk_points_scale_dev's k), host.  Affine Montgomery points
+ * (G1 8 / G2 16 u64 limbs), infinity all-zero (also as input); a zero scalar gives infinity, ratio = 0 gives first * P_0
+ * at i = 0 (0^0 = 1) and infinity elsewhere.  out may equal points.  On G2 the GLV split is only right for points of the
+ * order-r subgroup, which every ceremony point is.  A section may be processed in chunks: the call on points [a, b) with
+ * first * ratio^a as `first` equals that slice of one call over the whole section.  Temporary device memory: n x 64 bytes,
+ * allocated before anything is launched (B200ZK_ERR_OOM with a message when it does not fit).  A null pointer with n > 0:
+ * B200ZK_ERR_ARG; n = 0 does nothing.  Returns once out is complete. */
+int b200zk_points_mul_powers_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_points, size_t n, const uint64_t first[4],
+                                 const uint64_t ratio[4], void* d_out);
+/* ffjavascript's point encodings, the bytes a phase-1 ceremony hashes.  fmt 0 = toRprUncompressed: canonical big-endian
+ * x || y (G2: x.c1 x.c0 y.c1 y.c0), 64 / 128 bytes; fmt 1 = toRprCompressed: canonical big-endian x (G2: x.c1 x.c0) with
+ * 0x80 in byte 0 when y is the larger of (y, -y) (Fq2: decided by c1 unless c1 = 0, then by c0), 32 / 64 bytes.
+ * Infinity: 0x40 then zeros in both.  d_affine: n affine Montgomery points; d_bytes: n encodings back to back (16-byte
+ * aligned).  Enqueued on the slot's stream. */
+int b200zk_points_encode_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_affine, size_t n, int fmt, void* d_bytes);
+/* Blake2b-512 (RFC 7693) whose state is a caller-owned 216-byte buffer, so that hashing can be suspended and resumed (a
+ * phase-1 contribution record stores the response hasher's state as its partialHash).  Layout: buffer[128] || h[8] (u64
+ * LE) || t[2] (u64 LE) || c (u32 LE) || outlen (u32 LE), with the reference implementation's lazy rule (a full buffer is
+ * compressed only when more input arrives); believed to be blake2b-wasm's context, not checked against snarkjs.  Host
+ * only: no context and no GPU.  B200ZK_ERR_ARG for a null pointer or a state no init / update can produce. */
+int b200zk_blake2b512_init(uint8_t state[216]);
+int b200zk_blake2b512_update(uint8_t state[216], const void* data, size_t len);
+int b200zk_blake2b512_final(const uint8_t state[216], uint8_t out[64]);
 /* out[i] = (a[i] s0 + b[i] s1 + c[i] s2) s3   (s: 16 limbs = 4 Montgomery scalars, host). */
 int b200zk_fr_lincomb_dev(b200zk_ctx* ctx, const void* d_a, const void* d_b, const void* d_c, const uint64_t s[16], size_t n,
                           void* d_out);
