@@ -749,6 +749,16 @@ int b200zk_points_encode_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_
     B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
     return points_encode_dev(ctx, sl, g2, d_affine, n, fmt, d_bytes);
 }
+int b200zk_points_decode_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_bytes, size_t n, int fmt, int check_subgroup,
+                             void* d_affine, size_t* n_invalid, size_t* first_invalid) {
+    if (!ctx) return B200ZK_ERR_ARG;
+    if (!valid_slot(stream) || (n && (!d_bytes || !d_affine)))
+        return set_error(ctx, B200ZK_ERR_ARG, "points_decode: null pointer or bad stream slot");
+    Slot& sl = ctx->slots[stream];
+    std::lock_guard<std::mutex> g(sl.mu);
+    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
+    return points_decode_dev(ctx, sl, g2, d_bytes, n, fmt, check_subgroup, d_affine, n_invalid, first_invalid);
+}
 
 // ---- Blake2b-512 with an exported state (csrc/blake2b.cuh): host only, no context --------------------------------------
 int b200zk_blake2b512_init(uint8_t state[216]) {

@@ -98,6 +98,69 @@ int points_encode_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_affine, s
     return check_launch(ctx, "k_points_encode");
 }
 
+// The inverse (codec.cuh ffjs_decode): one square root per compressed point, one curve-equation check per uncompressed
+// one, and with check_subgroup a 254-bit ladder per G2 point.  bad[0] counts the invalid encodings, bad[1] keeps the
+// lowest invalid index; an invalid slot is left at infinity.
+template <class F, bool COMPRESSED>
+__global__ void __launch_bounds__(128) k_points_decode(const uint8_t* in, size_t n, int check_subgroup, affine_t<F>* out,
+                                                       unsigned long long* bad) {
+    constexpr int LEN = (COMPRESSED ? 1 : 2) * (int)sizeof(F);
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    __align__(16) uint8_t b[LEN];
+    const uint4* s = reinterpret_cast<const uint4*>(in + i * LEN);
+#pragma unroll
+    for (int k = 0; k < LEN / 16; ++k) *reinterpret_cast<uint4*>(b + 16 * k) = s[k];
+    affine_t<F> p;
+    if (!ffjs_decode<F, COMPRESSED>(b, check_subgroup != 0, &p)) {
+        atomicAdd(&bad[0], 1ull);
+        atomicMin(&bad[1], (unsigned long long)i);
+    }
+    st16(out + i, p);
+}
+
+int points_decode_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_bytes, size_t n, int fmt, int check_subgroup,
+                      void* d_affine, size_t* n_invalid, size_t* first_invalid) {
+    if (n_invalid) *n_invalid = 0;
+    if (first_invalid) *first_invalid = n;
+    if (fmt != 0 && fmt != 1) return set_error(ctx, B200ZK_ERR_ARG, "points_decode: fmt must be 0 (uncompressed) or 1 (compressed)");
+    if (n == 0) return B200ZK_OK;
+    if (n >= ((size_t)1 << 31) * 128) return set_error(ctx, B200ZK_ERR_ARG, "points_decode: too many points");
+    if (((uintptr_t)d_bytes | (uintptr_t)d_affine) & 15)
+        return set_error(ctx, B200ZK_ERR_ARG, "points_decode: the encodings and the points must be 16-byte aligned");
+    B2_CUDA_OK(ctx, sl.small.reserve(1024));
+    unsigned long long* bad = reinterpret_cast<unsigned long long*>(sl.small.p);
+    B2_CUDA_OK(ctx, cudaMemsetAsync(bad, 0, 8, sl.stream));
+    B2_CUDA_OK(ctx, cudaMemsetAsync(bad + 1, 0xFF, 8, sl.stream));
+    const unsigned grid = (unsigned)((n + 127) / 128);
+    {
+        LaunchScope ls(ctx, sl.stream, "points_decode");
+        const uint8_t* in = (const uint8_t*)d_bytes;
+        if (g2) {
+            affine_t<Fq2>* out = reinterpret_cast<affine_t<Fq2>*>(d_affine);
+            if (fmt) k_points_decode<Fq2, true><<<grid, 128, 0, sl.stream>>>(in, n, check_subgroup, out, bad);
+            else k_points_decode<Fq2, false><<<grid, 128, 0, sl.stream>>>(in, n, check_subgroup, out, bad);
+        } else {
+            affine_t<Fq>* out = reinterpret_cast<affine_t<Fq>*>(d_affine);
+            if (fmt) k_points_decode<Fq, true><<<grid, 128, 0, sl.stream>>>(in, n, check_subgroup, out, bad);
+            else k_points_decode<Fq, false><<<grid, 128, 0, sl.stream>>>(in, n, check_subgroup, out, bad);
+        }
+    }
+    B2_TRY(check_launch(ctx, "k_points_decode"));
+    unsigned long long h_bad[2] = {0, 0};
+    B2_CUDA_OK(ctx, cudaMemcpyAsync(h_bad, bad, 16, cudaMemcpyDeviceToHost, sl.stream));
+    B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
+    if (n_invalid) *n_invalid = (size_t)h_bad[0];
+    if (h_bad[0]) {
+        if (first_invalid) *first_invalid = (size_t)h_bad[1];
+        char msg[128];
+        snprintf(msg, sizeof(msg), "points_decode: %llu of %zu encodings are not valid points, the first at index %llu", h_bad[0],
+                 n, h_bad[1]);
+        return set_error(ctx, B200ZK_ERR_ARG, msg);
+    }
+    return B200ZK_OK;
+}
+
 int points_decompress_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_bytes, size_t n, int check_subgroup, void* d_affine,
                           size_t* n_invalid) {
     if (n_invalid) *n_invalid = 0;

@@ -109,6 +109,43 @@ B2_HD void fq_to_bytes(const Fq& xm, uint8_t* out) {
     for (int i = 0; i < 32; ++i) out[i] = (uint8_t)(x.l[i >> 2] >> (8 * (i & 3)));
 }
 
+B2_HD bool is_larger(const Fq& y) { return fq_is_larger(y); }
+B2_HD bool is_larger(const Fq2& y) { return fq2_is_larger(y); }
+
+// ---- the curve equation, y from x and a sign, and the order-r subgroup test, for ffjs_decode ----------------------------
+// g1_decode / g2_decode below keep their own inline copies: built on these helpers, k_g1_decompress went from 68 to 56
+// registers and k_g2_decompress from 246 to 252 (sm_90a), and those kernels are left as they were.
+B2_HD Fq curve_rhs(const Fq& x) {                // x^3 + b on G1
+    Fq bb;
+    for (int k = 0; k < 8; ++k) bb.l[k] = CurveConst::g1_b(k);
+    return Fq::add(Fq::mul_ni(Fq::mul_ni(x, x), x), bb);
+}
+B2_HD Fq2 curve_rhs(const Fq2& x) {              // x^3 + b' on the twist
+    Fq2 bb;
+    for (int k = 0; k < 8; ++k) { bb.c0.l[k] = CurveConst::g2_b_c0(k); bb.c1.l[k] = CurveConst::g2_b_c1(k); }
+    return Fq2::add(Fq2::mul(Fq2::sqr(x), x), bb);
+}
+B2_HD Fq field_sqr(const Fq& a) { return Fq::mul_ni(a, a); }
+B2_HD Fq2 field_sqr(const Fq2& a) { return Fq2::sqr(a); }
+B2_HD bool field_sqrt(const Fq& a, Fq* out) { return fq_sqrt(a, out); }
+B2_HD bool field_sqrt(const Fq2& a, Fq2* out) { return fq2_sqrt(a, out); }
+
+// the y of x's curve point that is_larger(y) == larger; false when x^3 + b is not a square (no point has that x)
+template <class F>
+B2_HD bool curve_y(const F& x, bool larger, F* y) {
+    if (!field_sqrt(curve_rhs(x), y)) return false;
+    if (is_larger(*y) != larger) *y = F::neg(*y);
+    return true;
+}
+
+// [r] P == O.  G1 has cofactor 1, so every G1 point passes; the twist has a large cofactor.
+B2_HD bool in_subgroup(const affine_t<Fq>&) { return true; }
+B2_HD bool in_subgroup(const affine_t<Fq2>& p) {
+    uint32_t r[8];
+    for (int k = 0; k < 8; ++k) r[k] = FrParams::mod(k);
+    return xyzz_t<Fq2>::mul_scalar(xyzz_t<Fq2>::from_affine(p), r).is_inf();
+}
+
 // one G1 / G2 encoding -> affine point; false when it is not a valid encoding (the point is then left at infinity)
 B2_HD_NI bool g1_decode(const uint8_t* b, affine_t<Fq>* out) {
     *out = affine_t<Fq>::infinity();
@@ -175,8 +212,17 @@ B2_HD void ffjs_put(const Fq2& a, uint8_t* out) {
     ffjs_put(a.c1, out);
     ffjs_put(a.c0, out + 32);
 }
-B2_HD bool is_larger(const Fq& y) { return fq_is_larger(y); }
-B2_HD bool is_larger(const Fq2& y) { return fq2_is_larger(y); }
+// the inverse: canonical big-endian bytes (byte 0 ANDed with top_mask) -> Montgomery form; false when the value is >= q
+B2_HD bool ffjs_get(const uint8_t* in, Fq* out, uint8_t top_mask = 0xFF) {
+    uint8_t le[32];
+    for (int i = 0; i < 32; ++i) le[i] = in[31 - i];
+    return fq_from_bytes(le, top_mask, out);
+}
+B2_HD bool ffjs_get(const uint8_t* in, Fq2* out, uint8_t top_mask = 0xFF) {
+    const bool ok1 = ffjs_get(in, &out->c1, top_mask);
+    const bool ok0 = ffjs_get(in + 32, &out->c0);
+    return ok1 && ok0;
+}
 
 // COMPRESSED = false: x || y (64 / 128 bytes); true: x with 0x80 in byte 0 when y is the larger of (y, -y) (32 / 64
 // bytes).  Infinity: 0x40 then zeros in both.
@@ -194,6 +240,32 @@ B2_HD void ffjs_encode(const affine_t<F>& p, uint8_t* b) {
     } else {
         ffjs_put(p.y, b + FB);
     }
+}
+
+// The inverse of ffjs_encode: one encoding -> affine point; false when it is not a valid encoding (the point is then
+// left at infinity).  Valid: infinity is 0x40 then zeros; uncompressed is x || y, both < q, byte 0's top bits clear and
+// y^2 = x^3 + b; compressed is x < q (0x80 masked off) with a curve point, y the root whose is_larger matches 0x80.
+// check_subgroup also requires [r] P == O (G2 only: G1 has cofactor 1).
+template <class F, bool COMPRESSED>
+B2_HD bool ffjs_decode(const uint8_t* b, bool check_subgroup, affine_t<F>* out) {
+    constexpr int FB = (int)sizeof(F), LEN = COMPRESSED ? FB : 2 * FB;
+    *out = affine_t<F>::infinity();
+    if (b[0] & 0x40) {
+        for (int k = 1; k < LEN; ++k) if (b[k] != 0) return false;
+        return b[0] == 0x40;
+    }
+    if (!COMPRESSED && (b[0] & 0x80)) return false;
+    affine_t<F> p;
+    if (!ffjs_get(b, &p.x, 0x3F)) return false;
+    if (COMPRESSED) {
+        if (!curve_y(p.x, (b[0] & 0x80) != 0, &p.y)) return false;
+    } else {
+        if (!ffjs_get(b + FB, &p.y)) return false;
+        if (!(field_sqr(p.y) == curve_rhs(p.x))) return false;
+    }
+    if (check_subgroup && !in_subgroup(p)) return false;
+    *out = p;
+    return true;
 }
 
 B2_HD void g2_encode(const affine_t<Fq2>& p, uint8_t* b) {

@@ -239,6 +239,8 @@ int fr_lincomb_dev(b200zk_ctx* ctx, Slot& sl, const void* a, const void* b, cons
 // codec.cu
 int points_compress_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_affine, size_t n, void* d_bytes);
 int points_encode_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_affine, size_t n, int fmt, void* d_bytes);
+int points_decode_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_bytes, size_t n, int fmt, int check_subgroup,
+                      void* d_affine, size_t* n_invalid, size_t* first_invalid);
 int points_decompress_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_bytes, size_t n, int check_subgroup, void* d_affine,
                           size_t* n_invalid);
 // packexp.cu

@@ -324,6 +324,35 @@ class PTau:
         self.close()
 
 
+def ptau_challenge_bytes(power: int) -> int:
+    """Size of a snarkjs phase-1 challenge file of this power (n = 2^power): the 64-byte lastResponseHash, then the
+    uncompressed sections 2 (2n - 1 G1), 3 (n G2), 4 and 5 (n G1 each) and 6 (1 G2): 384 n + 128 bytes."""
+    return 384 * (1 << power) + 128
+
+
+def ptau_response_bytes(power: int) -> int:
+    """Size of a snarkjs phase-1 response file of this power: the 64-byte challenge hash, the compressed sections 2-6 and
+    the 768-byte public key: 192 n + 864 bytes."""
+    return 192 * (1 << power) + 864
+
+
+def _power_of(size: int, per_power, what: str) -> int:
+    for p in range(1, PTau.MAX_UNPREPARED_POWER + 1):
+        if per_power(p) == size:
+            return p
+    raise FormatError("a %s file of %d bytes fits no power from 1 to %d" % (what, size, PTau.MAX_UNPREPARED_POWER))
+
+
+def ptau_challenge_power(size: int) -> int:
+    """The power whose challenge file is `size` bytes; FormatError when there is none in 1..27."""
+    return _power_of(size, ptau_challenge_bytes, "challenge")
+
+
+def ptau_response_power(size: int) -> int:
+    """The power whose response file is `size` bytes; FormatError when there is none in 1..27."""
+    return _power_of(size, ptau_response_bytes, "response")
+
+
 def read_ptau(path: str) -> PTau:
     """Open a prepared .ptau (memory-mapped; see PTau).  Raises FormatError for a file that is not a BN254 ptau, is not
     prepared for phase 2 or whose sections are shorter than its stated power."""

@@ -62,6 +62,31 @@ def ptau_beacon(net: Net, src_path: str, dst_path: str, beacon_hash: bytes, num_
     return phase1.beacon(net, src_path, dst_path, bytes(beacon_hash), int(num_iterations_exp), name=name)
 
 
+def ptau_export_challenge(net: Net, ptau_path: str, challenge_path: str) -> bytes:
+    """snarkjs `powersoftau export challenge <ptau> <challenge>`: the bare challenge a contributor works on, without the
+    .ptau (phase1.export_challenge).  Returns the challenge hash."""
+    from . import phase1
+    return phase1.export_challenge(net, ptau_path, challenge_path)
+
+
+def ptau_challenge_contribute(net: Net, challenge_path: str, response_path: str, entropy: str = ""):
+    """snarkjs `powersoftau challenge contribute bn128 <challenge> <response>` on the GPU, the key drawn as in
+    ptau_contribute; the secrets are dropped on return.  Returns (challengeHash, responseHash)."""
+    import hashlib
+    import os
+    from . import phase1, phase2
+    rng = phase2.ChaCha.from_hash(hashlib.blake2b(os.urandom(64) + str(entropy).encode("utf-8"), digest_size=64).digest())
+    return phase1.challenge_contribute(net, challenge_path, response_path, rng)
+
+
+def ptau_import_response(net: Net, ptau_path: str, response_path: str, dst_path: str, name: str | None = None):
+    """snarkjs `powersoftau import response <ptau> <response> <dst>`: the contributor's response appended to the ceremony
+    as a new record (phase1.import_response; it does not verify, ptau_verify does).  Returns (responseHash,
+    nextChallenge)."""
+    from . import phase1
+    return phase1.import_response(net, ptau_path, response_path, dst_path, name=name)
+
+
 def ptau_verify(net: Net, ptau_path: str):
     """snarkjs `powersoftau verify <ptau>` on the GPU: -> phase1.Phase1Report (ok, one failure line per check that does
     not hold, naming the contribution or section; per record its name, type and nextChallenge)."""

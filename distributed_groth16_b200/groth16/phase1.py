@@ -18,6 +18,18 @@ knowledge of the three secrets and chains the contribution to the previous one t
 
 The encodings of every point are made on the device (b200zk_points_encode_dev); the hashing runs on the host.
 
+A coordinated ceremony moves two bare files instead of the .ptau (n = 2^power; snarkjs `powersoftau export challenge`,
+`challenge contribute` and `import response`):
+
+  * challenge, 384 n + 128 bytes: lastResponseHash (64 bytes; Blake2b-512("") before any contribution), then U of
+    sections 2 (2n - 1 G1), 3 (n G2), 4 (n G1), 5 (n G1) and 6 (1 G2).  Its Blake2b-512 is the file's current
+    challenge: the last record's nextChallenge, or first_challenge_hash(power) before any contribution;
+  * response, 192 n + 864 bytes: the challenge hash (64 bytes), C of the five new sections in the same order, then
+    pub_key_bytes(key) (768 bytes).  Its Blake2b-512 is the responseHash; the hasher's state before the key is the
+    record's partialHash.
+
+Reading them back decodes every point on the device (b200zk_points_decode_dev): one square root per compressed point.
+
 Unpinned: there was no snarkjs and no published ceremony file to check against.  The section-7 layout and the 216-byte
 partialHash layout (formats.parse_ptau_contributions, blake2b.cuh), the compressed encoding's flag rule, the order of the
 key draws, the personalisation bytes and the stream hashed by first_challenge_hash are restated from memory of snarkjs /
@@ -149,6 +161,41 @@ def points_encode(net, points, g2: bool = False, compressed: bool = False):
     return out
 
 
+class InvalidEncodings(formats.FormatError):
+    """points_decode met encodings that are not points: `count` of them, the first at index `first`."""
+
+    def __init__(self, msg: str, count: int, first: int):
+        super().__init__(msg)
+        self.count, self.first = count, first
+
+
+def points_decode(net, data, g2: bool = False, compressed: bool = False, check_subgroup: bool = False):
+    """The inverse of points_encode on the device (b200zk_points_decode_dev): ffjavascript encodings (a CUDA uint8 tensor,
+    or host bytes / uint8 array) -> CUDA int64 (n, 8 | 16) affine Montgomery points.  check_subgroup also requires
+    [r] P == O on G2.  Raises InvalidEncodings (count, first index) when an encoding is not a valid point."""
+    import torch
+    w = (64 if g2 else 32) * (1 if compressed else 2)
+    if not isinstance(data, torch.Tensor):
+        host = np.ascontiguousarray(data).reshape(-1).view(np.uint8) if isinstance(data, np.ndarray) else \
+            np.frombuffer(data, dtype=np.uint8)
+        data = net.to_device(host if host.flags.writeable else host.copy())
+    data = data.contiguous()
+    if data.numel() % w:
+        raise ValueError("points_decode: %d bytes are not a whole number of %d-byte encodings" % (data.numel(), w))
+    n = data.numel() // w
+    out = torch.empty((n, 16 if g2 else 8), dtype=torch.int64, device=data.device)
+    bad, first = ctypes.c_size_t(0), ctypes.c_size_t(0)
+    rc = net._lib.b200zk_points_decode_dev(net._h, 0, int(g2), c_vp(data.data_ptr()), n, int(compressed), int(check_subgroup),
+                                           c_vp(out.data_ptr()), ctypes.byref(bad), ctypes.byref(first))
+    if rc != _native.OK and bad.value:
+        raise InvalidEncodings("%d of %d %s %s encodings are not valid points%s, the first at index %d"
+                               % (bad.value, n, "G2" if g2 else "G1", "compressed" if compressed else "uncompressed",
+                                  " of the order-r subgroup" if check_subgroup and g2 else "", first.value),
+                               bad.value, first.value)
+    net.check(rc)
+    return out
+
+
 def c_g1(p) -> bytes:
     """ffjavascript toRprCompressed of a G1 point on the host (8 Montgomery limbs): big-endian x, 0x80 in byte 0 when y
     is the larger of (y, -y)."""
@@ -229,9 +276,10 @@ def _read_records(pt: formats.PTau) -> list:
     return formats.parse_ptau_contributions(b"".join(pt.section_chunks(7)))
 
 
-def _hash_written(net, fd: int, offsets: dict, power: int, hasher, chunk: int, t: dict, grab=None) -> None:
-    """Feed U of sections 2..6 as written at `offsets` in the open file fd to hasher (encodings on the device).
-    grab[(sid, i)] is filled with point i of section sid when asked for."""
+def _hash_written(net, fd: int, offsets: dict, power: int, hasher, chunk: int, t: dict, grab=None, out=None) -> None:
+    """Feed U of sections 2..6 as written at `offsets` in the open file fd to hasher (encodings on the device), and
+    write them to the open file `out` too when given.  grab[(sid, i)] is filled with point i of section sid when asked
+    for."""
     for sid, (g2, _, count) in _SECTIONS.items():
         w, n = 16 if g2 else 8, count(power)
         for lo in range(0, n, chunk):
@@ -251,24 +299,92 @@ def _hash_written(net, fd: int, offsets: dict, power: int, hasher, chunk: int, t
                 for (s, i) in grab:
                     if s == sid and lo <= i < lo + cnt:
                         grab[(s, i)] = host[i - lo].copy()
-            t["file_s"] += t1 - t0
+            if out is not None:
+                out.write(enc)
+            t4 = time.perf_counter()
+            t["file_s"] += (t1 - t0) + (t4 - t3)
             t["encode_s"] += t2 - t1
             t["hash_s"] += t3 - t2
 
 
-def _contribute(net, src: str, dst: str, rng: phase2.ChaCha, record: dict, chunk: int, timings: dict | None):
+def _timings() -> dict:
+    return {"kernel_s": 0.0, "decode_s": 0.0, "encode_s": 0.0, "hash_s": 0.0, "transfer_s": 0.0, "file_s": 0.0, "key_s": 0.0}
+
+
+def _open_ceremony(src: str, dst: str, command: str) -> formats.PTau:
+    """The input of contribute / beacon / import response: not the output file, not reduced; prepared with a warning."""
     if os.path.exists(dst) and os.path.exists(src) and os.path.samefile(src, dst):
-        raise ValueError("powersoftau contribute: the output %r is the input file" % dst)
-    if chunk < 1:
-        raise ValueError("chunk must be at least 1 point")
-    t = {"kernel_s": 0.0, "encode_s": 0.0, "hash_s": 0.0, "transfer_s": 0.0, "file_s": 0.0, "key_s": 0.0}
-    with formats.PTau(src, prepared=False) as pt:
+        raise ValueError("powersoftau %s: the output %r is the input file" % (command, dst))
+    pt = formats.PTau(src, prepared=False)
+    try:
         if pt.power != pt.ceremony_power:
-            raise ValueError("ptau %r is reduced (power %d of a ceremony of power %d): contribute to the full ceremony file"
-                             % (src, pt.power, pt.ceremony_power))
+            raise ValueError("ptau %r is reduced (power %d of a ceremony of power %d): %s the full ceremony file"
+                             % (src, pt.power, pt.ceremony_power, "contribute to" if command == "contribute" else
+                                "use"))
         if any(pt.has_section(s) for s in (12, 13, 14, 15)):
             warnings.warn("ptau %r is prepared for phase 2: its Lagrange sections are dropped, the output has sections 1-7 "
                           "only (prepare it again afterwards)" % src)
+    except BaseException:
+        pt.close()
+        raise
+    return pt
+
+
+def _public_key(key: dict) -> dict:
+    return {k: {f: key[k][f] for f in ("g1_s", "g1_sx", "g2_spx")} for k in _KEYS}
+
+
+def _mul_chunk(net, d, g2: bool, first: int, tau: int, response, t: dict) -> np.ndarray:
+    """One chunk of a contribution: d <- (first tau^i) d[i] in place on the device, its compressed encodings hashed into
+    the response hasher.  -> the encodings on the host."""
+    t1 = time.perf_counter()
+    points_mul_powers(net, d, first, tau, g2, out=d)
+    net.sync(0)
+    t2 = time.perf_counter()
+    enc = points_encode(net, d, g2, compressed=True)
+    net.sync(0)
+    t3 = time.perf_counter()
+    enc = enc.cpu().numpy()
+    t4 = time.perf_counter()
+    response.update(enc)
+    t5 = time.perf_counter()
+    t["kernel_s"] += t2 - t1
+    t["encode_s"] += t3 - t2
+    t["transfer_s"] += t4 - t3
+    t["hash_s"] += t5 - t4
+    return enc
+
+
+def _finish(net, w: formats.PTauWriter, dst: str, records: list, pub: dict, partial: bytes, response_hash: bytes,
+            record: dict, chunk: int, t: dict) -> bytes:
+    """Close a ceremony file whose sections 2-6 are written: nextChallenge = Blake2b-512(responseHash || U of the written
+    sections) in a second pass over the file, then the new record (the points it names read back from the file) appended
+    to section 7.  -> nextChallenge."""
+    w.flush()
+    nxt = hashlib.blake2b(digest_size=64)
+    nxt.update(response_hash)
+    grab = {(2, 1): None, (3, 1): None, (4, 0): None, (5, 0): None, (6, 0): None}
+    fd = os.open(dst, os.O_RDONLY)
+    try:
+        _hash_written(net, fd, w.section_offsets, w.power, nxt, chunk, t, grab)
+    finally:
+        os.close(fd)
+    next_challenge = nxt.digest()
+    rec = formats.PTauContribution(tau_g1=grab[(2, 1)], tau_g2=grab[(3, 1)], alpha_g1=grab[(4, 0)],
+                                   beta_g1=grab[(5, 0)], beta_g2=grab[(6, 0)], key=pub, partial_hash=partial,
+                                   next_challenge=next_challenge, **record)
+    t0 = time.perf_counter()
+    w.write_contributions(formats.ptau_contributions_bytes(records + [rec]))
+    w.close()
+    t["file_s"] += time.perf_counter() - t0
+    return next_challenge
+
+
+def _contribute(net, src: str, dst: str, rng: phase2.ChaCha, record: dict, chunk: int, timings: dict | None):
+    if chunk < 1:
+        raise ValueError("chunk must be at least 1 point")
+    t = _timings()
+    with _open_ceremony(src, dst, "contribute") as pt:
         power = pt.power
         records = _read_records(pt)
         last = _last_challenge(pt, records)
@@ -289,46 +405,19 @@ def _contribute(net, src: str, dst: str, rng: phase2.ChaCha, record: dict, chunk
                     t0 = time.perf_counter()
                     d = net.to_device(pt.points(sid, lo, cnt, width))
                     net.sync(0)
+                    t["transfer_s"] += time.perf_counter() - t0
+                    _mul_chunk(net, d, g2, first * pow(tau, lo, R) % R, tau, response, t)
+                    t0 = time.perf_counter()
+                    host = d.cpu().numpy()
                     t1 = time.perf_counter()
-                    points_mul_powers(net, d, first * pow(tau, lo, R) % R, tau, g2, out=d)
-                    net.sync(0)
-                    t2 = time.perf_counter()
-                    enc = points_encode(net, d, g2, compressed=True)
-                    net.sync(0)
-                    t3 = time.perf_counter()
-                    host, enc = d.cpu().numpy(), enc.cpu().numpy()
-                    t4 = time.perf_counter()
-                    response.update(enc)
-                    t5 = time.perf_counter()
                     w.write(sid, host)
-                    t6 = time.perf_counter()
-                    t["transfer_s"] += (t1 - t0) + (t4 - t3)
-                    t["kernel_s"] += t2 - t1
-                    t["encode_s"] += t3 - t2
-                    t["hash_s"] += t5 - t4
-                    t["file_s"] += t6 - t5
+                    t["transfer_s"] += t1 - t0
+                    t["file_s"] += time.perf_counter() - t1
             partial = response.state()
-            pub = {k: {f: key[k][f] for f in ("g1_s", "g1_sx", "g2_spx")} for k in _KEYS}
+            pub = _public_key(key)
             response.update(pub_key_bytes(pub))
             response_hash = response.digest()
-            # nextChallenge hashes U of the new points after the response hash: a second pass over the written sections
-            w.flush()
-            nxt = hashlib.blake2b(digest_size=64)
-            nxt.update(response_hash)
-            grab = {(2, 1): None, (3, 1): None, (4, 0): None, (5, 0): None, (6, 0): None}
-            fd = os.open(dst, os.O_RDONLY)
-            try:
-                _hash_written(net, fd, w.section_offsets, power, nxt, chunk, t, grab)
-            finally:
-                os.close(fd)
-            next_challenge = nxt.digest()
-            rec = formats.PTauContribution(tau_g1=grab[(2, 1)], tau_g2=grab[(3, 1)], alpha_g1=grab[(4, 0)],
-                                           beta_g1=grab[(5, 0)], beta_g2=grab[(6, 0)], key=pub, partial_hash=partial,
-                                           next_challenge=next_challenge, **record)
-            t0 = time.perf_counter()
-            w.write_contributions(formats.ptau_contributions_bytes(records + [rec]))
-            w.close()
-            t["file_s"] += time.perf_counter() - t0
+            next_challenge = _finish(net, w, dst, records, pub, partial, response_hash, record, chunk, t)
         except BaseException:
             w.__exit__(None, None, None)
             os.unlink(dst)
@@ -360,6 +449,225 @@ def beacon(net, src: str, dst: str, beacon_hash: bytes, num_iterations_exp: int,
     rng = phase2.rng_from_beacon(bytes(beacon_hash), int(num_iterations_exp))
     return _contribute(net, src, dst, rng, dict(type=1, name=name, num_iterations_exp=int(num_iterations_exp),
                                                 beacon_hash=bytes(beacon_hash)), chunk, timings)
+
+
+# ---- challenge / response ------------------------------------------------------------------------------------------------
+def _last_response_hash(records: list) -> bytes:
+    """The responseHash of the last record, from its partialHash and key (as verify recomputes it); Blake2b-512("")
+    before any contribution."""
+    if not records:
+        return hashlib.blake2b(b"", digest_size=64).digest()
+    h = Blake2b512(bytes(records[-1].partial_hash))
+    h.update(pub_key_bytes(records[-1].key))
+    return h.digest()
+
+
+def _section_layout(power: int, compressed: bool) -> list:
+    """[(sid, g2, points, byte offset in the challenge / response file, bytes per point)] for sections 2-6."""
+    out, off = [], 64
+    for sid, (g2, _, count) in _SECTIONS.items():
+        per = (64 if g2 else 32) * (1 if compressed else 2)
+        out.append((sid, g2, count(power), off, per))
+        off += count(power) * per
+    return out
+
+
+def _pread_exact(fd: int, n: int, off: int) -> bytearray:
+    buf = bytearray(n)
+    got = os.preadv(fd, [buf], off)
+    if got != n:
+        raise formats.FormatError("file ends at byte %d, %d bytes were expected" % (off + got, off + n))
+    return buf
+
+
+def export_challenge(net, ptau: str, challenge: str, chunk: int = DEFAULT_CHUNK, timings: dict | None = None) -> bytes:
+    """snarkjs `powersoftau export challenge <ptau> <challenge>`: the last responseHash (recomputed from the last record's
+    partialHash and key) followed by U of sections 2-6, encoded on the device and hashed on the way out.  Refuses, and
+    deletes the output, when the hash is not the file's current challenge (the last nextChallenge, or the first challenge
+    hash of a fresh file).  Returns the challenge hash."""
+    if chunk < 1:
+        raise ValueError("chunk must be at least 1 point")
+    t = _timings()
+    with formats.PTau(ptau, prepared=False) as pt:
+        records = _read_records(pt)
+        want = _last_challenge(pt, records)
+        h = hashlib.blake2b(digest_size=64)
+        prefix = _last_response_hash(records)
+        h.update(prefix)
+        try:
+            with open(challenge, "wb") as out:
+                out.write(prefix)
+                fd = os.open(ptau, os.O_RDONLY)
+                try:
+                    _hash_written(net, fd, {sid: pt.section_span(sid)[0] for sid in _SECTIONS}, pt.power, h, chunk, t,
+                                  out=out)
+                finally:
+                    os.close(fd)
+            got = h.digest()
+            if got != want:
+                raise ValueError("ptau %r: its challenge hash %s is not the file's current challenge %s (the file's points or "
+                                 "its last record were altered)" % (ptau, got.hex(), want.hex()))
+        except BaseException:
+            if os.path.exists(challenge):
+                os.unlink(challenge)
+            raise
+    if timings is not None:
+        timings.update(t)
+    return got
+
+
+def challenge_contribute(net, challenge: str, response: str, rng: phase2.ChaCha, chunk: int = DEFAULT_CHUNK,
+                         timings: dict | None = None):
+    """snarkjs `powersoftau challenge contribute <challenge> <response>` with the key drawn from `rng`: the key is drawn
+    against Blake2b-512 of the challenge (a first pass over the file); then every point is decoded on the device, multiplied
+    by its power of the new secrets (as contribute does) and written compressed to the response, which ends with the
+    public key.  Returns (challengeHash, responseHash)."""
+    if chunk < 1:
+        raise ValueError("chunk must be at least 1 point")
+    if os.path.exists(response) and os.path.samefile(challenge, response):
+        raise ValueError("challenge contribute: the response %r is the challenge file" % response)
+    t = _timings()
+    fd = os.open(challenge, os.O_RDONLY)
+    try:
+        size = os.fstat(fd).st_size
+        power = formats.ptau_challenge_power(size)
+        t0 = time.perf_counter()
+        h = hashlib.blake2b(digest_size=64)
+        for lo in range(0, size, 1 << 26):
+            h.update(_pread_exact(fd, min(1 << 26, size - lo), lo))
+        challenge_hash = h.digest()
+        t["hash_s"] += time.perf_counter() - t0
+        t0 = time.perf_counter()
+        key = create_key(net, rng, challenge_hash)
+        t["key_s"] += time.perf_counter() - t0
+        tau = key["tau"]["prv"]
+        first_of = {"one": 1, "alpha": key["alpha"]["prv"], "beta": key["beta"]["prv"]}
+        resp = hashlib.blake2b(digest_size=64)
+        resp.update(challenge_hash)
+        try:
+            with open(response, "wb") as out:
+                out.write(challenge_hash)
+                for sid, g2, n, off, per in _section_layout(power, compressed=False):
+                    first = first_of[_SECTIONS[sid][1]]
+                    for lo in range(0, n, chunk):
+                        cnt = min(chunk, n - lo)
+                        t0 = time.perf_counter()
+                        raw = _pread_exact(fd, cnt * per, off + lo * per)
+                        t1 = time.perf_counter()
+                        enc = net.to_device(np.frombuffer(raw, dtype=np.uint8))
+                        net.sync(0)
+                        t2 = time.perf_counter()
+                        try:
+                            d = points_decode(net, enc, g2, compressed=False)
+                        except InvalidEncodings as e:
+                            raise formats.FormatError("challenge %r, section %d: %d points are not valid uncompressed "
+                                                      "encodings, the first is point %d" % (challenge, sid, e.count, lo + e.first))
+                        t3 = time.perf_counter()
+                        c = _mul_chunk(net, d, g2, first * pow(tau, lo, R) % R, tau, resp, t)
+                        t4 = time.perf_counter()
+                        out.write(c)
+                        t["file_s"] += (t1 - t0) + (time.perf_counter() - t4)
+                        t["transfer_s"] += t2 - t1
+                        t["decode_s"] += t3 - t2
+                pub = pub_key_bytes(_public_key(key))
+                out.write(pub)
+                resp.update(pub)
+        except BaseException:
+            if os.path.exists(response):
+                os.unlink(response)
+            raise
+    finally:
+        os.close(fd)
+    for k in _KEYS:
+        key[k]["prv"] = 0                   # the secrets go no further than this frame
+    if timings is not None:
+        timings.update(t)
+    return challenge_hash, resp.digest()
+
+
+def _read_pub_key(net, raw: bytes) -> dict:
+    """The 768-byte public key of a response (pub_key_bytes' layout) -> {"tau" | "alpha" | "beta": {"g1_s", "g1_sx",
+    "g2_spx"}} as Montgomery limbs, decoded on the device (G2 with the subgroup check)."""
+    try:
+        g1 = points_decode(net, raw[:384], g2=False).cpu().numpy().view(np.uint64)
+        g2 = points_decode(net, raw[384:], g2=True, check_subgroup=True).cpu().numpy().view(np.uint64)
+    except InvalidEncodings as e:
+        raise formats.FormatError("the response's public key holds %d invalid points (%s)" % (e.count, e))
+    return {k: {"g1_s": g1[2 * j].copy(), "g1_sx": g1[2 * j + 1].copy(), "g2_spx": g2[j].copy()} for j, k in enumerate(_KEYS)}
+
+
+def import_response(net, ptau: str, response: str, dst: str, name: str | None = None, chunk: int = DEFAULT_CHUNK,
+                    timings: dict | None = None):
+    """snarkjs `powersoftau import response <ptau> <response> <dst>`: the response's points decoded on the device (the G2
+    sections 3 and 6 and the key's G2 points with the subgroup check: the file comes from outside) and written to dst with
+    a type-0 record whose partialHash is the response hasher's state before the key.  The response must answer the
+    file's current challenge.  Refuses a reduced ptau and dst == ptau, warns on a prepared one, as contribute does; like
+    snarkjs it does not verify the contribution (verify does).  Returns (responseHash, nextChallenge)."""
+    if name is not None and len(name.encode("utf-8")) > 64:
+        raise ValueError("contribution name longer than 64 bytes")
+    if chunk < 1:
+        raise ValueError("chunk must be at least 1 point")
+    t = _timings()
+    with _open_ceremony(ptau, dst, "import response") as pt:
+        power = pt.power
+        records = _read_records(pt)
+        last = _last_challenge(pt, records)
+        fd = os.open(response, os.O_RDONLY)
+        try:
+            size = os.fstat(fd).st_size
+            if size != formats.ptau_response_bytes(power):
+                raise formats.FormatError("response %r is %d bytes, a power-%d response is %d" % (
+                    response, size, power, formats.ptau_response_bytes(power)))
+            prefix = bytes(_pread_exact(fd, 64, 0))
+            if prefix != last:
+                raise ValueError("response %r answers challenge %s, the file's current challenge is %s" % (
+                    response, prefix.hex(), last.hex()))
+            resp = Blake2b512()
+            resp.update(prefix)
+            w = formats.PTauWriter(dst, power)
+            try:
+                for sid, g2, n, off, per in _section_layout(power, compressed=True):
+                    for lo in range(0, n, chunk):
+                        cnt = min(chunk, n - lo)
+                        t0 = time.perf_counter()
+                        raw = _pread_exact(fd, cnt * per, off + lo * per)
+                        t1 = time.perf_counter()
+                        resp.update(raw)
+                        t2 = time.perf_counter()
+                        enc = net.to_device(np.frombuffer(raw, dtype=np.uint8))
+                        net.sync(0)
+                        t3 = time.perf_counter()
+                        try:
+                            d = points_decode(net, enc, g2, compressed=True, check_subgroup=g2)
+                        except InvalidEncodings as e:
+                            raise formats.FormatError("response %r, section %d: %d points are not valid compressed encodings%s, "
+                                                      "the first is point %d" % (response, sid, e.count,
+                                                                                 " of the order-r subgroup" if g2 else "",
+                                                                                 lo + e.first))
+                        t4 = time.perf_counter()
+                        host = d.cpu().numpy()
+                        t5 = time.perf_counter()
+                        w.write(sid, host)
+                        t6 = time.perf_counter()
+                        t["file_s"] += (t1 - t0) + (t6 - t5)
+                        t["hash_s"] += t2 - t1
+                        t["transfer_s"] += (t3 - t2) + (t5 - t4)
+                        t["decode_s"] += t4 - t3
+                partial = resp.state()
+                key_raw = bytes(_pread_exact(fd, 768, size - 768))
+                pub = _read_pub_key(net, key_raw)
+                resp.update(key_raw)
+                response_hash = resp.digest()
+                next_challenge = _finish(net, w, dst, records, pub, partial, response_hash, dict(type=0, name=name), chunk, t)
+            except BaseException:
+                w.__exit__(None, None, None)
+                os.unlink(dst)
+                raise
+        finally:
+            os.close(fd)
+    if timings is not None:
+        timings.update(t)
+    return response_hash, next_challenge
 
 
 # ---- verify --------------------------------------------------------------------------------------------------------------

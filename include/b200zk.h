@@ -283,6 +283,17 @@ int b200zk_points_mul_powers_dev(b200zk_ctx* ctx, int stream, int g2, const void
  * Infinity: 0x40 then zeros in both.  d_affine: n affine Montgomery points; d_bytes: n encodings back to back (16-byte
  * aligned).  Enqueued on the slot's stream. */
 int b200zk_points_encode_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_affine, size_t n, int fmt, void* d_bytes);
+/* The inverse of b200zk_points_encode_dev: the step of a snarkjs `challenge contribute` (fmt 0) and `import response`
+ * (fmt 1) that reads ffjavascript's encodings back into points, one thread per point.  Valid: infinity is 0x40 then zeros
+ * (both formats); fmt 0 is x || y with both < q, byte 0's top two bits clear and y^2 = x^3 + b; fmt 1 is x < q (after
+ * masking 0x80) with a curve point, y the square root whose "larger" rule (as in encode) agrees with the 0x80 flag.
+ * check_subgroup != 0 also requires [r] P == O on G2 (G1 has cofactor 1).  d_bytes: n encodings back to back; d_affine:
+ * n affine Montgomery points (G1 8 / G2 16 u64 limbs, infinity all-zero); both 16-byte aligned.  *n_invalid = the number
+ * of invalid encodings, *first_invalid = the lowest invalid index (n when there is none); either may be null.  Any invalid
+ * encoding: B200ZK_ERR_ARG with a message giving the count and the first index, and those slots hold infinity.  A null
+ * pointer with n > 0: B200ZK_ERR_ARG; n = 0 does nothing.  Returns once the counters are on the host. */
+int b200zk_points_decode_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_bytes, size_t n, int fmt, int check_subgroup,
+                             void* d_affine, size_t* n_invalid, size_t* first_invalid);
 /* Blake2b-512 (RFC 7693) whose state is a caller-owned 216-byte buffer, so that hashing can be suspended and resumed (a
  * phase-1 contribution record stores the response hasher's state as its partialHash).  Layout: buffer[128] || h[8] (u64
  * LE) || t[2] (u64 LE) || c (u32 LE) || outlen (u32 LE), with the reference implementation's lazy rule (a full buffer is
