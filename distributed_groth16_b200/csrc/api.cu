@@ -740,6 +740,15 @@ int b200zk_points_mul_powers_dev(b200zk_ctx* ctx, int stream, int g2, const void
     B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
     return points_mul_powers_dev(ctx, sl, g2, d_points, n, first, ratio, d_out);
 }
+int b200zk_points_sub_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_a, const void* d_b, size_t n, void* d_out) {
+    if (!ctx) return B200ZK_ERR_ARG;
+    if (!valid_slot(stream) || (n && (!d_a || !d_b || !d_out)))
+        return set_error(ctx, B200ZK_ERR_ARG, "points_sub: null pointer or bad stream slot");
+    Slot& sl = ctx->slots[stream];
+    std::lock_guard<std::mutex> g(sl.mu);
+    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
+    return points_sub_dev(ctx, sl, g2, d_a, d_b, n, d_out);
+}
 int b200zk_points_encode_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_affine, size_t n, int fmt, void* d_bytes) {
     if (!ctx) return B200ZK_ERR_ARG;
     if (!valid_slot(stream) || (n && (!d_affine || !d_bytes)))

@@ -235,6 +235,7 @@ int points_scale_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_points, si
 int points_intt_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_in, unsigned log_n, void* d_out);
 int points_mul_powers_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_points, size_t n, const uint64_t first[4],
                           const uint64_t ratio[4], void* d_out);
+int points_sub_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_a, const void* d_b, size_t n, void* d_out);
 int fr_lincomb_dev(b200zk_ctx* ctx, Slot& sl, const void* a, const void* b, const void* c, const uint64_t s[16], size_t n, void* out);
 // codec.cu
 int points_compress_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_affine, size_t n, void* d_bytes);

@@ -757,4 +757,37 @@ int points_mul_powers_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_point
                                                           (affine_t<Fq>*)d_out);
 }
 
+// ---- pointwise difference: out[i] = a[i] - b[i]  (snarkjs `zkey new`: the circuit hash's H points tau^(n+i) G1 - tau^i G1)
+// One mixed addition per point (madd handles a = +-b and either side at infinity), normalised with one block-batched
+// inversion per block.  Each thread reads its a[i] and b[i] before the block's first barrier and writes only out[i], so
+// out may equal a or b.
+constexpr int SUB_BLOCK = 128;
+
+template <class F>
+__global__ void __launch_bounds__(SUB_BLOCK) k_points_sub(const affine_t<F>* a, const affine_t<F>* b, size_t n, affine_t<F>* out) {
+    __shared__ F pre[SUB_BLOCK], suf[SUB_BLOCK], tot;
+    const size_t i = (size_t)blockIdx.x * SUB_BLOCK + threadIdx.x;
+    xyzz_t<F> d = xyzz_t<F>::identity();
+    if (i < n) {
+        d = xyzz_t<F>::from_affine(ld16(a + i));
+        xyzz_t<F>::madd(d, ld16(b + i), true);
+    }
+    const affine_t<F> r = block_to_affine<F, SUB_BLOCK>(d, !d.is_inf(), pre, suf, &tot);
+    if (i < n) st16(out + i, r);
+}
+
+int points_sub_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_a, const void* d_b, size_t n, void* d_out) {
+    if (n == 0) return B200ZK_OK;
+    if (n >= ((size_t)1 << 31) * SUB_BLOCK) return set_error(ctx, B200ZK_ERR_ARG, "points_sub: too many points");
+    const unsigned grid = (unsigned)((n + SUB_BLOCK - 1) / SUB_BLOCK);
+    {
+        LaunchScope ls(ctx, sl.stream, g2 ? "points_sub_g2" : "points_sub_g1");
+        if (g2) k_points_sub<Fq2><<<grid, SUB_BLOCK, 0, sl.stream>>>((const affine_t<Fq2>*)d_a, (const affine_t<Fq2>*)d_b, n,
+                                                                     (affine_t<Fq2>*)d_out);
+        else k_points_sub<Fq><<<grid, SUB_BLOCK, 0, sl.stream>>>((const affine_t<Fq>*)d_a, (const affine_t<Fq>*)d_b, n,
+                                                                 (affine_t<Fq>*)d_out);
+    }
+    return check_launch(ctx, "k_points_sub");
+}
+
 }  // namespace b200zk

@@ -101,12 +101,23 @@ def ptau_check_lagrange(net: Net, ptau_path: str):
     return ptau.check_lagrange(net, ptau_path)
 
 
-def zkey_new(net: Net, r1cs_bytes: bytes, ptau_path: str) -> bytes:
+def zkey_new(net: Net, r1cs_bytes: bytes, ptau_path: str, cs_hash: bool = False) -> bytes:
     """snarkjs `zkey new <r1cs> <ptau>` on the GPU (scripts/phase2_proving_key.sh, ark-circom/test-vectors/complex-circuit/
-    build.sh:11): the .zkey bytes of the circuit's proving key from a prepared Powers-of-Tau file.  The key has delta = 1
-    and a zero csHash (formats.write_zkey): it needs a phase-2 contribution before production use."""
+    build.sh:11): the .zkey bytes of the circuit's proving key from a prepared Powers-of-Tau file.  The key has delta = 1:
+    it needs a phase-2 contribution before production use.  Section 10 starts with a zero csHash (formats.write_zkey)
+    unless cs_hash is True; then it holds the circuit hash snarkjs writes (cshash.cs_hash), and every other byte is the
+    same."""
     with formats.read_ptau(ptau_path) as pt:
-        return zkey_from_r1cs(net, formats.read_r1cs(r1cs_bytes), pt)
+        return zkey_from_r1cs(net, formats.read_r1cs(r1cs_bytes), pt, cs_hash=cs_hash)
+
+
+def zkey_cs_hash(net: Net, r1cs_bytes: bytes, ptau_path: str) -> bytes:
+    """The circuit hash (csHash) of the circuit's `zkey new` key from a prepared Powers-of-Tau file: the 64 bytes snarkjs
+    prints as "Circuit hash" and stores at the start of zkey section 10 (cshash.cs_hash)."""
+    from .cshash import cs_hash
+    from .setup import ptau_key_points
+    with formats.read_ptau(ptau_path) as pt:
+        return cs_hash(net, ptau_key_points(net, formats.read_r1cs(r1cs_bytes), pt), pt)
 
 
 def _random_scalar(entropy: bytes) -> int:
@@ -145,17 +156,23 @@ def zkey_beacon(net: Net, zkey_bytes: bytes, beacon_hash: bytes, num_iterations_
     return phase2.beacon(net, zkey_bytes, bytes(beacon_hash), int(num_iterations_exp), name=name)
 
 
-def zkey_verify(net: Net, r1cs_bytes: bytes, ptau_path: str, zkey_bytes: bytes):
+def zkey_verify(net: Net, r1cs_bytes: bytes, ptau_path: str, zkey_bytes: bytes, check_cs_hash: bool = False):
     """snarkjs `zkey verify <r1cs> <ptau> <zkey>`: -> phase2.Phase2Report (ok, failure reasons, per contribution its name,
-    type and hash, and the csHash found in the file, which is not recomputed)."""
+    type and hash, and the csHash found in the file).  check_cs_hash also recomputes the circuit hash from the circuit and
+    the ceremony and fails when the file's differs, as snarkjs does; without it the csHash is carried, not checked."""
     from . import phase2
-    return phase2.verify(net, r1cs_bytes, ptau_path, zkey_bytes)
+    return phase2.verify(net, r1cs_bytes, ptau_path, zkey_bytes, check_cs_hash=check_cs_hash)
 
 
-def zkey_from_r1cs(net: Net, r1: formats.R1CS, pt: formats.PTau) -> bytes:
+def zkey_from_r1cs(net: Net, r1: formats.R1CS, pt: formats.PTau, cs_hash: bool = False) -> bytes:
     """zkey_new on a parsed r1cs and an open ceremony file."""
+    import struct
     from .setup import ptau_key_points
     q = ptau_key_points(net, r1, pt)
+    sec10 = None
+    if cs_hash:
+        from .cshash import cs_hash as circuit_hash
+        sec10 = circuit_hash(net, q, pt) + struct.pack("<I", 0)
     r2 = lambda i: net.fr_convert(net.to_device(np.ascontiguousarray(r1.vals[i], dtype=np.uint64).reshape(-1, 4)),
                                   to_mont=True, times=2).cpu().numpy().view(np.uint64)     # value * R^2, on the device
     mi, ci, si, vi = formats.zkey_coefficients(q["n_public"], r1.n_constraints, (r1.rows[0], r1.cols[0], r2(0)),
@@ -166,7 +183,7 @@ def zkey_from_r1cs(net: Net, r1: formats.R1CS, pt: formats.PTau) -> bytes:
                       delta_g2=q["delta_g2"], ic=host(q["ic"]), a_query=host(q["a_query"]), b_g1_query=host(q["b_g1_query"]),
                       b_g2_query=host(q["b_g2_query"]), l_query=host(q["l_query"]), h_query=host(q["h_query"]),
                       coef_matrix=mi, coef_row=ci, coef_col=si, coef_val_r2=vi)
-    return formats.write_zkey(zk)
+    return formats.write_zkey(zk, section10=sec10)
 
 
 def load_witness(net: Net, wtns_bytes: bytes):

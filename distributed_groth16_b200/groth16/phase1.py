@@ -148,6 +148,19 @@ def points_mul_powers(net, points, first: int, ratio: int, g2: bool = False, out
     return out
 
 
+def points_sub(net, a, b, g2: bool = False, out=None):
+    """out[i] = a[i] - b[i] on the device (b200zk_points_sub_dev); a, b: CUDA int64 (n, 8 | 16).  out may be a or b."""
+    import torch
+    a, b = a.contiguous(), b.contiguous()
+    if a.shape != b.shape:
+        raise ValueError("points_sub: a and b have shapes %s and %s" % (tuple(a.shape), tuple(b.shape)))
+    if out is None:
+        out = torch.empty_like(a)
+    net.check(net._lib.b200zk_points_sub_dev(net._h, 0, int(g2), c_vp(a.data_ptr()), c_vp(b.data_ptr()), int(a.shape[0]),
+                                             c_vp(out.data_ptr())))
+    return out
+
+
 def points_encode(net, points, g2: bool = False, compressed: bool = False):
     """ffjavascript toRprUncompressed (compressed=False) / toRprCompressed encodings of CUDA int64 (n, 8 | 16) points on
     the device (b200zk_points_encode_dev) -> CUDA uint8 tensor (n, bytes per point)."""

@@ -386,7 +386,8 @@ class Phase2Report:
     ok: bool
     failures: list = field(default_factory=list)          # one line per failed check
     contributions: list = field(default_factory=list)     # (name, type, contribution hash) per record, oldest first
-    cs_hash: bytes = b""                                   # as found in the file: not recomputed
+    cs_hash: bytes = b""                                   # as found in the file
+    cs_hash_expected: bytes = b""                          # recomputed from the circuit and ceremony (check_cs_hash only)
 
 
 def _g1_gen():
@@ -409,9 +410,11 @@ def _random_scalars(net, n: int):
     return net.fr_convert(net.to_device(raw), to_mont=True)
 
 
-def verify(net, r1cs_bytes: bytes, ptau_path: str, zkey_bytes: bytes) -> Phase2Report:
+def verify(net, r1cs_bytes: bytes, ptau_path: str, zkey_bytes: bytes, check_cs_hash: bool = False) -> Phase2Report:
     """snarkjs `zkey verify <r1cs> <ptau> <zkey>` on the GPU: the key is the `zkey new` key of this circuit and ceremony
-    followed by a valid chain of phase-2 contributions.  The csHash is carried, not recomputed (the report holds it)."""
+    followed by a valid chain of phase-2 contributions.  The report holds the csHash found in the file.  check_cs_hash
+    also recomputes it from the rebuilt initial key and the ceremony (cshash.cs_hash) into cs_hash_expected and fails on
+    a mismatch; without it the csHash is carried, not checked."""
     from .circom import zkey_new
     from .setup import _fixed_base, _mont_limbs
     rep = Phase2Report(ok=False)
@@ -425,7 +428,12 @@ def verify(net, r1cs_bytes: bytes, ptau_path: str, zkey_bytes: bytes) -> Phase2R
         fail("not a zkey with phase-2 parameters: %s" % e)
         return rep
     rep.cs_hash = mpc.cs_hash
-    init = zkey_new(net, r1cs_bytes, ptau_path)
+    init = zkey_new(net, r1cs_bytes, ptau_path, cs_hash=check_cs_hash)
+    if check_cs_hash:
+        rep.cs_hash_expected = _section(init, 10)[:64]
+        if bytes(mpc.cs_hash) != rep.cs_hash_expected:
+            fail("circuit hash (csHash) %s... differs from %s..., the one of this circuit and ceremony"
+                 % (bytes(mpc.cs_hash)[:8].hex(), rep.cs_hash_expected[:8].hex()))
     ihdr = _section(init, 2)
     if len(ihdr) != len(hdr) or ihdr[:_HDR_DELTA] != hdr[:_HDR_DELTA] or ihdr[_HDR_DELTA + 192:] != hdr[_HDR_DELTA + 192:]:
         fail("header (apart from delta) differs from the initial key of this circuit and ceremony")

@@ -277,6 +277,11 @@ int b200zk_points_intt_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_in
  * B200ZK_ERR_ARG; n = 0 does nothing.  Returns once out is complete. */
 int b200zk_points_mul_powers_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_points, size_t n, const uint64_t first[4],
                                  const uint64_t ratio[4], void* d_out);
+/* out[i] = a[i] - b[i], i < n: the step of snarkjs `zkey new` that makes the circuit hash's H points tau^(n+i) G1 - tau^i G1
+ * from a ceremony's tau powers.  Affine Montgomery points (g2 = 0: G1, 8 u64 limbs; 1: G2, 16), infinity all-zero (also
+ * as input); a[i] = b[i] gives infinity, a[i] = -b[i] gives 2 a[i].  out may equal a or b; no other overlap is allowed.
+ * A null pointer with n > 0: B200ZK_ERR_ARG; n = 0 does nothing.  Enqueued on the slot's stream. */
+int b200zk_points_sub_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_a, const void* d_b, size_t n, void* d_out);
 /* ffjavascript's point encodings, the bytes a phase-1 ceremony hashes.  fmt 0 = toRprUncompressed: canonical big-endian
  * x || y (G2: x.c1 x.c0 y.c1 y.c0), 64 / 128 bytes; fmt 1 = toRprCompressed: canonical big-endian x (G2: x.c1 x.c0) with
  * 0x80 in byte 0 when y is the larger of (y, -y) (Fq2: decided by c1 unless c1 = 0, then by c0), 32 / 64 bytes.
