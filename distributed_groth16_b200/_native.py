@@ -8,7 +8,7 @@ import ctypes
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("B200ZK_LIB") or os.path.join(_HERE, "libb200zk.so")   # B200ZK_LIB: experiment variants
+LIB_PATH = os.path.join(_HERE, "libb200zk.so")
 
 OK, ERR_LENGTH, ERR_DOMAIN, ERR_CUDA, ERR_ARG, ERR_OOM = range(6)
 _ERR_NAMES = {1: "BAD_LENGTH", 2: "BAD_DOMAIN", 3: "CUDA", 4: "BAD_ARG", 5: "OOM"}

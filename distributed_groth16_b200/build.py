@@ -35,23 +35,19 @@ def _deps_mtime() -> float:
     return t
 
 
-def build(force: bool = False, verbose: bool = False, defines=(), out: str | None = None) -> str:
-    """defines/out: build an experiment variant (tools/variants.py) next to the product library."""
-    global OBJ
-    lib = out or LIB
-    if not force and not defines and os.path.exists(lib) and os.path.getmtime(lib) >= _deps_mtime():
+def build(force: bool = False, verbose: bool = False) -> str:
+    if not force and os.path.exists(LIB) and os.path.getmtime(LIB) >= _deps_mtime():
         sys.stderr.write("distributed_groth16_b200.build: %s is newer than every source under csrc/ and include/: reused "
-                         "(build(force=True) recompiles)\n" % os.path.relpath(lib))
-        return lib
+                         "(build(force=True) recompiles)\n" % os.path.relpath(LIB))
+        return LIB
     sys.stderr.write("distributed_groth16_b200.build: compiling %d translation units for %s with %s\n" % (len(SOURCES), ARCH, _nvcc()))
-    obj_dir = OBJ if not out else OBJ + "_" + os.path.basename(out).replace(".so", "")
-    os.makedirs(obj_dir, exist_ok=True)
+    os.makedirs(OBJ, exist_ok=True)
     nvcc = _nvcc()
     extra = ["-Xptxas", "-v"] if verbose else []
 
     def compile_one(src):
-        obj = os.path.join(obj_dir, src.replace(".cu", ".o"))
-        cmd = [nvcc] + NVCC_FLAGS + extra + ["-D" + d for d in defines] + ["-c", os.path.join(CSRC, src), "-o", obj]
+        obj = os.path.join(OBJ, src.replace(".cu", ".o"))
+        cmd = [nvcc] + NVCC_FLAGS + extra + ["-c", os.path.join(CSRC, src), "-o", obj]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("nvcc failed for %s:\n%s\n%s" % (src, r.stdout, r.stderr))
@@ -61,11 +57,11 @@ def build(force: bool = False, verbose: bool = False, defines=(), out: str | Non
 
     with ThreadPoolExecutor(max_workers=len(SOURCES)) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    r = subprocess.run([nvcc, "-shared", "-o", lib] + objs + GENCODE,
+    r = subprocess.run([nvcc, "-shared", "-o", LIB] + objs + GENCODE,
                        capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))
-    return lib
+    return LIB
 
 
 if __name__ == "__main__":

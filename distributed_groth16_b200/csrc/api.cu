@@ -24,19 +24,7 @@ int b200zk_ctx_create(int device, b200zk_ctx** out) {
     b200zk_ctx* ctx = new b200zk_ctx();
     ctx->device = device;
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) {
-        ctx->sm_count = prop.multiProcessorCount;
-        // opt-in (B200ZK_L2_PERSIST=1): pin the MSM base array in L2 while the bucket kernel gathers from it.
-        // Measured on an earlier GPU: no gain for the (FMA-bound) bucket kernel, and the carve-out slows the scatter
-        // kernel, so it is off by default.  Not re-measured on H100, whose 50 MB L2 cannot hold a 2^20-point base array.
-        const char* env = getenv("B200ZK_L2_PERSIST");
-        if ((env && env[0] == '1') && prop.persistingL2CacheMaxSize > 0 &&
-            cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, (size_t)prop.persistingL2CacheMaxSize) == cudaSuccess) {
-            ctx->l2_persist_max = (size_t)prop.persistingL2CacheMaxSize;
-            ctx->l2_window_max = (size_t)prop.accessPolicyMaxWindowSize;
-        }
-        cudaGetLastError();
-    }
+    if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) ctx->sm_count = prop.multiProcessorCount;
     for (int i = 0; i < 3; ++i) {
         if (cudaStreamCreateWithFlags(&ctx->slots[i].stream, cudaStreamNonBlocking) != cudaSuccess) {
             delete ctx;
@@ -56,16 +44,7 @@ int b200zk_ctx_create(int device, b200zk_ctx** out) {
     {
         int lo = 0, hi = 0;
         cudaDeviceGetStreamPriorityRange(&lo, &hi);
-        // lane 0 (the G2 MSM, issued first and by far the longest) sorts at the highest priority so that its bucket kernel
-        // starts filling the SMs early; the h pipeline comes next, the other lanes' sort phases are not urgent
-        // (their bucket kernels queue behind lane 0's anyway)
-        const int p_h = hi < lo ? hi + 1 : hi, p_mid = (lo + hi) / 2;
-        bool ok = cudaStreamCreateWithPriority(&ctx->hi_stream, cudaStreamNonBlocking, p_h) == cudaSuccess;
-        for (int k = 0; ok && k < 5; ++k) {
-            ok = cudaStreamCreateWithPriority(&ctx->lane_main[k], cudaStreamNonBlocking, k == 0 ? hi : p_mid) == cudaSuccess &&
-                 cudaStreamCreateWithPriority(&ctx->lane_acc[k], cudaStreamNonBlocking, lo) == cudaSuccess;
-            for (int j = 0; ok && j < 3; ++j) ok = cudaEventCreateWithFlags(&ctx->lane_ev[k][j], cudaEventDisableTiming) == cudaSuccess;
-        }
+        bool ok = true;
         for (int k = 0; ok && k < 6; ++k) ok = cudaStreamCreateWithPriority(&ctx->msm_side[k], cudaStreamNonBlocking, hi) == cudaSuccess;
         if (!ok) { b200zk_ctx_destroy(ctx); return B200ZK_ERR_CUDA; }
     }
@@ -91,14 +70,8 @@ void b200zk_ctx_destroy(b200zk_ctx* ctx) {
         if (s.aux_done) cudaEventDestroy(s.aux_done);
         for (int k = 0; k < 32; ++k) if (s.stage_ev[k]) cudaEventDestroy(s.stage_ev[k]);
     }
-    if (ctx->hi_stream) cudaStreamDestroy(ctx->hi_stream);
     for (int k = 0; k < 6; ++k) if (ctx->msm_side[k]) cudaStreamDestroy(ctx->msm_side[k]);
     for (auto& v : ctx->msm_events) for (cudaEvent_t e : v) cudaEventDestroy(e);
-    for (int k = 0; k < 5; ++k) {
-        if (ctx->lane_main[k]) cudaStreamDestroy(ctx->lane_main[k]);
-        if (ctx->lane_acc[k]) cudaStreamDestroy(ctx->lane_acc[k]);
-        for (int j = 0; j < 3; ++j) if (ctx->lane_ev[k][j]) cudaEventDestroy(ctx->lane_ev[k][j]);
-    }
     for (auto& e : ctx->prof_pending) { cudaEventDestroy(e.start); cudaEventDestroy(e.stop); }
     delete ctx;
 }
@@ -209,34 +182,18 @@ int msm_staged_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* bases, const v
     char* d_bases = reinterpret_cast<char*>(sl.io_a.p);
     char* d_scalars = d_bases + n * PB;
     // Part sizes: a smaller first part shortens the time the GPU waits for its first bases, a smaller last part the bucket work
-    // left when the last byte has arrived.  tools/e2ebench.py compares weightings; 2,3,4,4,3 beat four equal parts, other weightings
-    // and seven parts at 2^20 / 2^22 -- every part costs a sort, a bucket kernel with its drain and a merge.  B200ZK_MSM_PART_WEIGHTS = "w1,w2,..." or B200ZK_MSM_PARTS = k (equal parts) override.
-    static const int parts_env = getenv("B200ZK_MSM_PARTS") ? atoi(getenv("B200ZK_MSM_PARTS")) : 0;
-    static unsigned weights_env[16], nweights_env = 0;
-    static const bool weights_parsed = [] {
-        if (const char* w = getenv("B200ZK_MSM_PART_WEIGHTS")) {
-            while (*w && nweights_env < 16) {
-                unsigned v = (unsigned)strtoul(w, const_cast<char**>(&w), 10);
-                if (v) weights_env[nweights_env++] = v;
-                while (*w == ',' || *w == ' ') ++w;
-            }
-        }
-        return true;
-    }();
-    (void)weights_parsed;
-    static const unsigned default_weights[5] = {2, 3, 4, 4, 3};
-    unsigned weights[16], nparts;
-    if (nweights_env) { nparts = nweights_env; for (unsigned p = 0; p < nparts; ++p) weights[p] = weights_env[p]; }
-    else if (parts_env > 0) { nparts = parts_env > 16 ? 16u : (unsigned)parts_env; for (unsigned p = 0; p < nparts; ++p) weights[p] = 1; }
-    else if (n >= ((size_t)1 << 18)) { nparts = 5; for (unsigned p = 0; p < 5; ++p) weights[p] = default_weights[p]; }
-    else { nparts = 1; weights[0] = 1; }
+    // left when the last byte has arrived.  Weights 2,3,4,4,3 beat four equal parts, other weightings and seven parts at
+    // 2^20 / 2^22 -- every part costs a sort, a bucket kernel with its drain and a merge.  Below 2^18 one part.
+    static const unsigned staged_weights[5] = {2, 3, 4, 4, 3}, one_weight[1] = {1};
+    const unsigned nparts = n >= ((size_t)1 << 18) ? 5 : 1;
+    const unsigned* weights = nparts > 1 ? staged_weights : one_weight;
     unsigned wsum = 0;
     for (unsigned p = 0; p < nparts; ++p) wsum += weights[p];
     const char* hb = reinterpret_cast<const char*>(bases);
     const char* hs = reinterpret_cast<const char*>(scalars);
     cudaStream_t cs = sl.copy_stream;
-    size_t cnt[16];
-    cudaEvent_t ev_s[16], ev_b[16];
+    size_t cnt[5];
+    cudaEvent_t ev_s[5], ev_b[5];
     size_t lo = 0;
     unsigned wcum = 0;
     for (unsigned p = 0; p < nparts; ++p) {

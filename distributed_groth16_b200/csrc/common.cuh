@@ -61,16 +61,7 @@ struct Slot {                 // one per MultiplexedStreamID
 struct b200zk_ctx {
     int device = 0;
     int sm_count = 132;
-    size_t l2_persist_max = 0;      // cudaLimitPersistingL2CacheSize granted at creation
-    size_t l2_window_max = 0;       // accessPolicyMaxWindowSize
     b200zk::Slot slots[3];
-    // prove_dev's streams.  hi_stream (highest priority): the h pipeline; lane_main[k] (middle priority): digit / sort /
-    // reduction kernels of MSM k; lane_acc[k] (lowest = default priority): its bucket kernel.  The block dispatcher
-    // serves the highest-priority pending kernel first, so the short kernels slip between the bucket kernels' blocks.
-    cudaStream_t hi_stream = nullptr;
-    cudaStream_t lane_main[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-    cudaStream_t lane_acc[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-    cudaEvent_t lane_ev[5][3] = {};
     unsigned msm_seg_hint = 0;      // set by prove_dev around its MSM launches (it holds every slot lock): reduction segment length
     std::string last_error;
     std::mutex err_mu;
@@ -87,12 +78,12 @@ struct b200zk_ctx {
     std::mutex plan_mu;
     std::map<uint32_t, b200zk::NttPlan*> plans;
     void *fb_table_g1 = nullptr, *fb_table_g2 = nullptr;     // fixed-base window tables of the generators (setup.cu)
-    // MSM channels (msm.cu, window-group pipeline): 0..5 = slot i's main / aux workspace (2 i + aux), 6..10 = prove lanes.
+    // MSM channels (msm.cu, window-group pipeline): 0..5 = slot i's main / aux workspace (2 i + aux).
     // msm_side[ch]: high-priority helper stream that runs the sort phases and the reduction / Horner tail of one window
     // group while the bucket kernel of the next group occupies the SMs; msm_events[ch]: its event pool (grown on demand,
     // only ever touched under the owning slot's mutex).
     cudaStream_t msm_side[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    std::vector<cudaEvent_t> msm_events[11];
+    std::vector<cudaEvent_t> msm_events[6];
 };
 
 struct b200zk_pk {
@@ -174,13 +165,6 @@ static inline unsigned ceil_log2(size_t n) {
     return l;
 }
 
-struct MsmLane {
-    cudaStream_t st;          // digits, sort, merge, reduction, combine (the result is ordered on this stream)
-    DevBuf* ws;
-    cudaStream_t acc_st;      // bucket accumulation
-    int channel;              // event pool (b200zk_ctx::msm_events)
-};
-
 // ---- entry points implemented across translation units -------------------------------------
 // ntt.cu
 int ntt_dev(b200zk_ctx* ctx, Slot& sl, const Fr* d_in, Fr* d_out, unsigned log_n, bool inverse, bool coset,
@@ -210,8 +194,6 @@ unsigned msm_table_auto_window(size_t n);
 int msm_table_build_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_bases, size_t n, unsigned c, void* d_table);
 int msm_table_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_table, const void* d_scalars, size_t n, unsigned c,
                   void* d_out_xyzz, int aux = 0);
-int msm_lane_dev(b200zk_ctx* ctx, const MsmLane& lane, int g2, unsigned tab_c, const void* d_bases, const void* d_scalars,
-                 size_t n, void* d_out_xyzz);
 int g1_sum_dev(b200zk_ctx* ctx, Slot& sl, const void* d_xyzz, size_t count, void* d_out_affine);
 int g2_sum_dev(b200zk_ctx* ctx, Slot& sl, const void* d_xyzz, size_t count, void* d_out_affine);
 int xyzz_sum_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_in, size_t count, size_t stride, void* d_out);

@@ -71,17 +71,8 @@ struct xyzz_t {
         return r;
     }
 
-#ifndef B2_MADD_INLINE
-#define B2_MADD_INLINE 0       // 1: the Fq2 products of the bucket loop are inlined too (no call / argument traffic, ~3x the code)
-#endif
-#if B2_MADD_INLINE
-#define B2_MADD_MUL(...) F::mul_inl(__VA_ARGS__)
-#define B2_MADD_SQR(...) F::sqr_inl(__VA_ARGS__)
-#else
-#define B2_MADD_MUL(...) F::mul(__VA_ARGS__)
-#define B2_MADD_SQR(...) F::sqr(__VA_ARGS__)
-#endif
-    // acc += (negate ? -p : p), p affine (madd-2008-s); handles p = inf, acc = inf, acc = +-p
+    // acc += (negate ? -p : p), p affine (madd-2008-s); handles p = inf, acc = inf, acc = +-p.  The G2 bucket loop keeps
+    // its Fq2 products out of line (DESIGN §7): inlined they save the call / argument traffic at ~3x the code.
     B2_HD static void madd(xyzz_t& acc, const affine_t<F>& p, bool negate) {
         if (p.is_inf()) return;
         F py = negate ? F::neg(p.y) : p.y;
@@ -89,8 +80,8 @@ struct xyzz_t {
             acc.x = p.x; acc.y = py; acc.zz = F::one(); acc.zzz = F::one();
             return;
         }
-        F U2 = B2_MADD_MUL(p.x, acc.zz);
-        F S2 = B2_MADD_MUL(py, acc.zzz);
+        F U2 = F::mul(p.x, acc.zz);
+        F S2 = F::mul(py, acc.zzz);
         F Pp = F::sub(U2, acc.x);
         F R = F::sub(S2, acc.y);
         if (Pp.is_zero()) {
@@ -98,15 +89,15 @@ struct xyzz_t {
             else acc = identity();
             return;
         }
-        F PP = B2_MADD_SQR(Pp);
-        F PPP = B2_MADD_MUL(Pp, PP);
-        F Q = B2_MADD_MUL(acc.x, PP);
-        F X3 = F::sub(F::sub(B2_MADD_SQR(R), PPP), F::dbl(Q));
-        F Y3 = F::sub(B2_MADD_MUL(R, F::sub(Q, X3)), B2_MADD_MUL(acc.y, PPP));
+        F PP = F::sqr(Pp);
+        F PPP = F::mul(Pp, PP);
+        F Q = F::mul(acc.x, PP);
+        F X3 = F::sub(F::sub(F::sqr(R), PPP), F::dbl(Q));
+        F Y3 = F::sub(F::mul(R, F::sub(Q, X3)), F::mul(acc.y, PPP));
         acc.x = X3;
         acc.y = Y3;
-        acc.zz = B2_MADD_MUL(acc.zz, PP);
-        acc.zzz = B2_MADD_MUL(acc.zzz, PPP);
+        acc.zz = F::mul(acc.zz, PP);
+        acc.zzz = F::mul(acc.zzz, PPP);
     }
 
     // add-2008-s

@@ -27,14 +27,6 @@
 #define B2_HD_NI inline
 #endif
 
-// build-time experiment switches (tools/variants.sh): multiplier schedule and inlining
-#ifndef B2_MUL_VARIANT
-#define B2_MUL_VARIANT 0      // 0: mad.lo.cc/madc.hi.cc rows everywhere; 1: IMAD.WIDE + IADD3 chains for the a*b rows
-#endif
-#ifndef B2_MUL_NOINLINE
-#define B2_MUL_NOINLINE 0     // 1: Fp::mul is an out-of-line call (small I-cache footprint)
-#endif
-
 namespace b200zk {
 
 // ---------------------------------------------------------------------------------------------
@@ -179,21 +171,8 @@ struct Fp {
         acc[6] = cc::madc_lo_cc(a[6], bi, 0);
         acc[7] = cc::madc_hi(a[6], bi, 0);
     }
-    // 64-bit products of the even-indexed limbs of a with bi: t[j], t[j+1] = a[j]*bi (plain IMAD.WIDE,
-    // full rate; the carry-in/out form of IMAD.WIDE issues at half rate, measured with
-    // tools/microbench.cu, so the a*b rows add their products with IADD3 chains on the ALU pipe while
-    // the m*p rows keep the fused carry form on the FMA pipe -- the two pipes then overlap).
-    B2_HD static void prod_n(uint32_t* t, const uint32_t* a, uint32_t bi) {
-#pragma unroll
-        for (int j = 0; j < 8; j += 2) {
-            uint64_t w = (uint64_t)a[j] * bi;
-            t[j] = (uint32_t)w;
-            t[j + 1] = (uint32_t)(w >> 32);
-        }
-    }
     // one row: (ev + 2^32 od) <- (ev + 2^32 od + a*bi + m*p) / 2^32, roles of ev/od swap for the next row
     B2_HD static void mad_row(uint32_t* ev, uint32_t* od, const uint32_t* a, uint32_t bi, bool first) {
-#if B2_MUL_VARIANT == 0
         if (first) {
             mul_n(od, a + 1, bi);
             mul_n(ev, a, bi);
@@ -203,37 +182,12 @@ struct Fp {
             cmad_n(ev, a, bi);
             od[7] = cc::addc(od[7], 0);
         }
-#else
-        if (first) {
-            prod_n(od, a + 1, bi);
-            prod_n(ev, a, bi);
-        } else {
-            uint32_t te[8], to[8];
-            prod_n(to, a + 1, bi);
-            prod_n(te, a, bi);
-            ev[0] = cc::add_cc(ev[0], od[1]);
-#pragma unroll
-            for (int j = 0; j < 6; ++j) od[j] = cc::addc_cc(od[j + 2], to[j]);      // od = (od >> 64) + to + carry
-            od[6] = cc::addc_cc(to[6], 0);
-            od[7] = cc::addc(to[7], 0);                                           // a[7]*bi < 2^62: no carry out
-            ev[0] = cc::add_cc(ev[0], te[0]);
-#pragma unroll
-            for (int j = 1; j < 8; ++j) ev[j] = cc::addc_cc(ev[j], te[j]);
-            od[7] = cc::addc(od[7], 0);
-        }
-#endif
         uint32_t mi = ev[0] * P::INV;
         cmad_mod<1>(od, mi);
         cmad_mod<0>(ev, mi);
         od[7] = cc::addc(od[7], 0);
     }
-#if B2_MUL_NOINLINE && defined(__CUDA_ARCH__)
-    B2_HD static Fp mul(const Fp& a, const Fp& b) { return mul_ni(a, b); }
-    B2_HD static Fp mul_inl(const Fp& a, const Fp& b) {
-#else
-    B2_HD static Fp mul_inl(const Fp& a, const Fp& b) { return mul(a, b); }
     B2_HD static Fp mul(const Fp& a, const Fp& b) {
-#endif
         uint32_t ev[8], od[8];
 #pragma unroll
         for (int i = 0; i < 8; i += 2) {
@@ -246,25 +200,15 @@ struct Fp {
         ev[7] = cc::addc(ev[7], 0);
         Fp r; final_sub(r, ev); return r;
     }
-#ifndef B2_SQR_VARIANT
-#define B2_SQR_VARIANT 0      // 1: dedicated squaring (36 + 72 wide multiply-adds instead of 136) -- measured 3% SLOWER in the G1 bucket kernel (126 vs 120 registers, doubling shifts); 0: mul(a, a)
-#endif
-    B2_HD static Fp sqr_inl(const Fp& a) { return sqr(a); }
-    B2_HD static Fp sqr(const Fp& a) {
-#if B2_SQR_VARIANT == 1
-        uint32_t t[16];
-        sqr_wide(t, a.l);
-        Fp r; redc<1>(r, t); return r;
-#else
-        return mul(a, a);
-#endif
-    }
+    // a dedicated squaring (36 + 72 wide multiply-adds instead of 136) was measured 3% SLOWER in the G1 bucket kernel
+    // (126 vs 120 registers, doubling shifts)
+    B2_HD static Fp sqr(const Fp& a) { return mul(a, a); }
 
     // ---- unreduced 512-bit products and a separate Montgomery reduction ----------------------------------------------------
     // Column-wise (product scanning) with a three-word column accumulator (c0, c1, c2): every partial product is one fused
     // (mad.lo.cc, madc.hi.cc) pair = one wide multiply-add, plus an addc for the third word on the ALU pipe.  They exist for
-    // what the row-interleaved product above cannot do: squarings that compute each cross product once, and Fq2 products that
-    // reduce two sums of products instead of three products (Fq2::mul).
+    // what the row-interleaved product above cannot do: Fq2 products that reduce two sums of products instead of three
+    // products (Fq2::mul).
     B2_HD static void col_mad(uint32_t& c0, uint32_t& c1, uint32_t& c2, uint32_t x, uint32_t y) {
         c0 = cc::mad_lo_cc(x, y, c0);
         c1 = cc::madc_hi_cc(x, y, c1);
@@ -283,36 +227,6 @@ struct Fp {
             t[k] = c0; c0 = c1; c1 = c2; c2 = 0;
         }
         t[15] = c0;
-    }
-    // t[0..16) = a^2: the 28 cross products once, doubled, plus the 8 squares
-    B2_HD static void sqr_wide(uint32_t* t, const uint32_t* a) {
-        uint32_t c0 = 0, c1 = 0, c2 = 0;
-        t[0] = 0;
-#pragma unroll
-        for (int k = 1; k < 14; ++k) {                     // cross terms a_i a_j, i < j, i + j = k (k = 1 .. 13)
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const int j = k - i;
-                if (j > i && j < 8) col_mad(c0, c1, c2, a[i], a[j]);
-            }
-            t[k] = c0; c0 = c1; c1 = c2; c2 = 0;
-        }
-        t[14] = c0; t[15] = c1;                            // c1 = 0: the cross sum is < 2^(32 * 15)
-        // double (the sum of cross terms is < 2^511) and add the squares
-#pragma unroll
-        for (int k = 15; k > 0; --k) t[k] = (t[k] << 1) | (t[k - 1] >> 31);
-        t[0] = 0;
-        uint32_t carry = 0;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-            const uint32_t lo = cc::mul_lo(a[i], a[i]), hi = cc::mul_hi(a[i], a[i]);
-            t[2 * i] = cc::add_cc(t[2 * i], carry);
-            t[2 * i + 1] = cc::addc_cc(t[2 * i + 1], 0);
-            carry = cc::addc(0, 0);
-            t[2 * i] = cc::add_cc(t[2 * i], lo);
-            t[2 * i + 1] = cc::addc_cc(t[2 * i + 1], hi);
-            carry = cc::addc(carry, 0);
-        }
     }
     // r = t / 2^256 mod p for t < SUBS * p * 2^256 (SUBS = 1: products of canonical values; 2: a lazy sum of two of them):
     // column-wise Montgomery reduction, then SUBS conditional subtractions.  Clobbers nothing outside r.
@@ -402,7 +316,7 @@ struct Fp {
     B2_HD static void mul_group(Fp* r, const Fp* a, const Fp* b) { mul_k<K>(r, a, b); }
     // out-of-line copy for the cold / very large kernels (G2, reductions): keeps code size and
     // compile time bounded; the G1 bucket loop uses the inlined `mul`.
-    B2_HD_NI static Fp mul_ni(const Fp& a, const Fp& b) { return mul_inl(a, b); }
+    B2_HD_NI static Fp mul_ni(const Fp& a, const Fp& b) { return mul(a, b); }
 
     B2_HD static Fp to_mont(const Fp& a) { return mul(a, r2()); }
     B2_HD static Fp from_mont(const Fp& a) {
@@ -519,14 +433,9 @@ struct Fq2 {
     B2_HD static Fq2 sub(const Fq2& a, const Fq2& b) { Fq2 r; r.c0 = Fq::sub(a.c0, b.c0); r.c1 = Fq::sub(a.c1, b.c1); return r; }
     B2_HD static Fq2 neg(const Fq2& a) { Fq2 r; r.c0 = Fq::neg(a.c0); r.c1 = Fq::neg(a.c1); return r; }
     B2_HD static Fq2 dbl(const Fq2& a) { return add(a, a); }
-    // one out-of-line unit per Fq2 product (3 inlined Fq products): 10 calls per mixed add instead of 28
-#ifndef B2_FQ2_LAZY
-#define B2_FQ2_LAZY 1         // 1: three unreduced products, two reductions (336 wide multiply-adds); 0: three full products (384)
-#endif
-    B2_HD_NI static Fq2 mul(const Fq2 a, const Fq2 b) { return mul_inl(a, b); }
-    B2_HD_NI static Fq2 sqr(const Fq2 a) { return sqr_inl(a); }
-    B2_HD static Fq2 mul_inl(const Fq2& a, const Fq2& b) {
-#if B2_FQ2_LAZY == 1
+    // one out-of-line unit per Fq2 product (3 inlined Fq products): 10 calls per mixed add instead of 28.  Three
+    // unreduced products and two reductions (336 wide multiply-adds) beat three full products (384).
+    B2_HD_NI static Fq2 mul(const Fq2 a, const Fq2 b) {
         // c0 = a0 b0 - a1 b1, c1 = (a0 + a1)(b0 + b1) - a0 b0 - a1 b1, reduced once each.  Bounds: the products of canonical
         // values are < p^2; sa, sb = a0 + a1, b0 + b1 < 2p (no reduction: < 2^255), so sa sb < 4 p^2 < 2^512 and
         // c1's integer = a0 b1 + a1 b0 < 2 p^2 < 2 p 2^256; c0's = a0 b0 - a1 b1 + p 2^256 in (0, 2 p 2^256).
@@ -550,16 +459,8 @@ struct Fq2 {
         Fq::template redc<2>(r.c0, t0);
         Fq::template redc<2>(r.c1, t2);
         return r;
-#else
-        Fq v0 = Fq::mul(a.c0, b.c0), v1 = Fq::mul(a.c1, b.c1);
-        Fq s = Fq::mul(Fq::add(a.c0, a.c1), Fq::add(b.c0, b.c1));
-        Fq2 r;
-        r.c0 = Fq::sub(v0, v1);
-        r.c1 = Fq::sub(Fq::sub(s, v0), v1);
-        return r;
-#endif
     }
-    B2_HD static Fq2 sqr_inl(const Fq2& a) {
+    B2_HD_NI static Fq2 sqr(const Fq2 a) {
         Fq t = Fq::mul(Fq::add(a.c0, a.c1), Fq::sub(a.c0, a.c1));
         Fq u = Fq::mul(a.c0, a.c1);
         Fq2 r; r.c0 = t; r.c1 = Fq::dbl(u); return r;

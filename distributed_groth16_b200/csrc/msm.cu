@@ -25,13 +25,10 @@ static const uint32_t KEY_NONE = 0xFFFFFFFFu;
 // ---------------------------------------------------------------------------------------------
 // 1. digits + histogram
 // ---------------------------------------------------------------------------------------------
-// fold != 0 (fixed-base tables, section 7): every window shares ONE bucket set, the window is carried by the
-// entry index (w * n + i selects 2^{cw} P_i in the table) instead of by the bucket index.
-// Otherwise window w fills bucket set s = W - 1 - w: sets are numbered in the order the Horner chain consumes them (top
-// window first), so that a *group* of consecutive sets can be reduced and folded into the chain while the bucket
-// kernel of the next group is still running (host side, "window-group pipeline").
-__global__ void k_msm_digits(const Fr* scalars, uint32_t n, uint32_t c, uint32_t W, uint32_t fold, uint32_t* keys,
-                             uint32_t* ranks, uint32_t* counts) {
+// Fixed-base tables (section 7): every window shares ONE bucket set, the window is carried by the entry index
+// (w * n + i selects 2^{cw} P_i in the table) instead of by the bucket index.
+__global__ void k_msm_digits(const Fr* scalars, uint32_t n, uint32_t c, uint32_t W, uint32_t* keys, uint32_t* ranks,
+                             uint32_t* counts) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     Fr s = Fr::from_mont(ld16(scalars + i));
@@ -51,19 +48,21 @@ __global__ void k_msm_digits(const Fr* scalars, uint32_t n, uint32_t c, uint32_t
         uint32_t neg = 0;
         if (d > B) { d = (1u << c) - d; neg = 1; carry = 1; }
         if (d != 0) {
-            uint32_t g = (fold ? 0u : (W - 1 - w) * B) + (d - 1);
+            uint32_t g = d - 1;
             rank = atomicAdd(counts + g, 1u);
             key = g | (neg << 31);
         }
-        const size_t slot = (size_t)(fold ? w : W - 1 - w) * n + i;
+        const size_t slot = (size_t)w * n + i;
         keys[slot] = key;
         ranks[slot] = rank;
     }
 }
 
-// k = k1 + k2 lambda (glv.cuh; G1 and, with beta^2, G2); window w of |k1| fills bucket set 2 (Wh - 1 - w), window w of |k2| set
-// 2 (Wh - 1 - w) + 1 over the same points (top windows first, the two halves interleaved: see k_msm_digits) -- phi is
-// applied once to the second chain's result in k_msm_horner_glv.
+// Every other MSM: k = k1 + k2 lambda (glv.cuh; G1 and, with beta^2, G2); window w of |k1| fills bucket set 2 (Wh - 1 - w),
+// window w of |k2| set 2 (Wh - 1 - w) + 1 over the same points.  Sets are numbered in the order the Horner chain consumes
+// them (top window first, the two halves interleaved), so that a *group* of consecutive sets can be reduced and folded
+// into the chain while the bucket kernel of the next group is still running (host side, "window-group pipeline").  phi
+// is applied once to the second chain's result in k_msm_horner_glv.
 __global__ void k_msm_digits_glv(const Fr* scalars, uint32_t n, uint32_t c, uint32_t Wh, uint32_t* keys, uint32_t* ranks,
                                  uint32_t* counts) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -189,12 +188,7 @@ __global__ void k_msm_scatter(const uint32_t* keys, const uint32_t* ranks, const
 //    multi-task buckets go through task_sums[] and a block-level merge.
 // ---------------------------------------------------------------------------------------------
 static const uint32_t TASK_LEN = 128, MAX_TASK_LEN = 1024;    // default / largest task length (runtime: task_len)
-#ifndef B2_ACC_MINBLOCKS
-#define B2_ACC_MINBLOCKS 4
-#endif
-#ifndef B2_ACC_MINBLOCKS_G2
-#define B2_ACC_MINBLOCKS_G2 4
-#endif
+static const uint32_t ACC_MINBLOCKS = 4, ACC_MINBLOCKS_G2 = 4;  // bucket kernel blocks per SM (k_msm_accumulate)
 
 __global__ void k_msm_task_counts(const uint32_t* offsets, uint32_t nbuckets, uint32_t task_len, uint32_t* ntasks) {
     uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
@@ -257,7 +251,7 @@ __global__ void k_msm_task_order(const uint32_t* offsets, const uint32_t* task_o
 // G2 (Fq2 coordinates): 250 registers uncapped = 8 warps/SM with `wait` the top stall; capped at 128 (4 blocks/SM, some
 // spills) it was faster at 2^20; 5+ blocks lose again
 template <class F, bool RMW>
-__global__ void __launch_bounds__(128, sizeof(F) > 32 ? B2_ACC_MINBLOCKS_G2 : B2_ACC_MINBLOCKS) k_msm_accumulate(const affine_t<F>* bases, const uint32_t* entries, const uint32_t* offsets,
+__global__ void __launch_bounds__(128, sizeof(F) > 32 ? ACC_MINBLOCKS_G2 : ACC_MINBLOCKS) k_msm_accumulate(const affine_t<F>* bases, const uint32_t* entries, const uint32_t* offsets,
                                  const uint32_t* task_off, const uint32_t* task_bucket, const uint32_t* order,
                                  uint32_t nbuckets, uint32_t task_len, uint32_t wave, xyzz_t<F>* buckets, xyzz_t<F>* task_sums) {
     // Block order over the length-sorted task list: the first `wave` blocks (one per resident slot) take an evenly
@@ -429,12 +423,10 @@ __global__ void __launch_bounds__(THREADS) k_msm_window_sum(const xyzz_t<F>* par
     if (threadIdx.x == 0) st16(wsum + blockIdx.x, sh[0]);
 }
 
-// 6. Horner over the bucket sets, in the order the digit kernels number them (top window first).  One launch folds the
-// `nset` window sums of ONE window group into the running chain kept in `state` (first: the chain starts here; last: the
-// result goes to `out`), so the c doublings per window of group g run while the bucket kernel of group g + 1 occupies
-// the SMs.  One quad: the (up to 4) independent field products of each level of a point operation are computed by the
-// 4 lanes in the same instruction stream and exchanged through shared memory (quad_ops).  c = 0 (fixed-base tables):
-// a plain sum of the nset partial sums.
+// 6. Combine.  Fixed-base tables (one bucket set): k_msm_horner with c = 0 adds up the `nset` partial sums of the
+// window-sum blocks.  (Without the constant c and its doubling loop ptxas gives the kernel more registers and stack.)
+// One quad: the (up to 4) independent field products of each level of a point operation are computed by the 4 lanes
+// in the same instruction stream and exchanged through shared memory (quad_ops).
 template <class F>
 __global__ void __launch_bounds__(32) k_msm_horner(const xyzz_t<F>* wsum, uint32_t nset, uint32_t c, uint32_t first, uint32_t last,
                                                    xyzz_t<F>* state, xyzz_t<F>* out) {
@@ -452,9 +444,12 @@ __global__ void __launch_bounds__(32) k_msm_horner(const xyzz_t<F>* wsum, uint32
     if (threadIdx.x == 0) st16(last ? out : state, total);
 }
 
-// GLV variant: quad 0 runs the chain of the |k1| windows (sets 2k), quad 1 that of the |k2| windows (sets 2k + 1) in
-// the same warp (half as many sequential doublings); result = H0 + phi(H1), phi(X, Y, ZZ, ZZZ) = (beta X, Y, ZZ, ZZZ) on G1 and
-// (beta^2 X, Y, ZZ, ZZZ) on the twist (glv_phi_x).
+// Horner over the bucket sets of the GLV digits, in the order k_msm_digits_glv numbers them (top window first).  One
+// launch folds the window sums of ONE window group into the running chains kept in `state` (first: the chains start
+// here; last: the result goes to `out`), so the c doublings per window of group g run while the bucket kernel of group
+// g + 1 occupies the SMs.  Quad 0 runs the chain of the |k1| windows (sets 2k), quad 1 that of the |k2| windows (sets
+// 2k + 1) in the same warp (half as many sequential doublings); result = H0 + phi(H1), phi(X, Y, ZZ, ZZZ) =
+// (beta X, Y, ZZ, ZZZ) on G1 and (beta^2 X, Y, ZZ, ZZZ) on the twist (glv_phi_x).
 template <class F>
 __global__ void __launch_bounds__(32) k_msm_horner_glv(const xyzz_t<F>* wsum, uint32_t nwin, uint32_t c, uint32_t first, uint32_t last,
                                                        xyzz_t<F>* state, xyzz_t<F>* out) {
@@ -543,23 +538,13 @@ static cudaEvent_t msm_event(b200zk_ctx* ctx, int ch, size_t idx) {
 }
 
 // Streams of one MSM.  `seq`: digit / sort phases and, per window group, merge + bucket reduction + Horner step;
-// `acc`: the bucket kernels; `result`: the stream the caller orders the result on.  A plain call runs the bucket
-// kernels on the caller's stream and everything else on the channel's high-priority side stream; a prove lane brings
-// its own pair (lane.st is `seq` and `result`).
+// `acc`: the bucket kernels, on the caller's stream, which the result is ordered on.  `seq` is the channel's
+// high-priority side stream.
 struct MsmStreams {
     cudaStream_t seq, acc;
-    bool result_on_seq;
     int channel;
 };
 
-// The window-group pipeline (one MSM, no host round trips):
-//   seq : digits, scan | prep(0) | prep(1) .. prep(G-1) | wait A0: tail(0) | wait A1: tail(1) | ...
-//   acc :                 wait P0: accumulate(0) -> A0 | wait P1: accumulate(1) -> A1 | ...
-// prep(g) = task tables + scatter of group g's bucket sets, tail(g) = merge + bucket reduction + window sums + Horner
-// step.  Groups hold consecutive bucket sets in Horner order (top windows first), so tail(g) -- a chain of dependent
-// point operations that used to follow the bucket kernel (a quarter of a 2^20 MSM) -- overlaps accumulate(g + 1); only
-// the last group's tail is exposed.  `seq` has the higher stream priority: its short kernels get the SM slots that
-// the running bucket kernel frees, instead of queueing behind it.
 // One input part of an MSM: `n` pairs, and (host-staged callers) the events that signal the arrival of its scalars / bases.
 struct MsmPart {
     const void* bases;
@@ -584,7 +569,7 @@ struct MsmPart {
 // on two streams instead -- two bucket sets, two tails -- were slower.)
 template <class F>
 static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, const MsmPart* parts, unsigned nparts,
-                        void* d_out, const char* acc_name, unsigned tab_c = 0, unsigned c_force = 0) {
+                        void* d_out, const char* acc_name, unsigned tab_c = 0) {
     const int ch = ms.channel;
     size_t nev = 0;
     auto next_event = [&]() { return msm_event(ctx, ch, nev++); };
@@ -592,10 +577,9 @@ static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, c
     for (unsigned p = 0; p < nparts; ++p) { n += parts[p].n; n_max = parts[p].n > n_max ? parts[p].n : n_max; }
     xyzz_t<F>* out = reinterpret_cast<xyzz_t<F>*>(d_out);
     if (n == 0) {
-        cudaStream_t rs = ms.result_on_seq ? ms.seq : ms.acc;
         {
-            LaunchScope ls(ctx, rs, "msm_small");
-            k_set_identity<F><<<1, 32, 0, rs>>>(out);
+            LaunchScope ls(ctx, ms.acc, "msm_small");
+            k_set_identity<F><<<1, 32, 0, ms.acc>>>(out);
         }
         return check_launch(ctx, "k_set_identity");
     }
@@ -604,12 +588,10 @@ static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, c
     // then share one bucket set and the Horner chain disappears
     const bool fold = tab_c != 0;
     if (fold && nparts != 1) return set_error(ctx, B200ZK_ERR_ARG, "fixed-base tables take one input part");
-    const unsigned c = fold ? tab_c : (c_force ? c_force : choose_window(n));
-    static const bool glv_env = !(getenv("B200ZK_MSM_GLV") && getenv("B200ZK_MSM_GLV")[0] == '0');
-    static const bool glv2_env = !(getenv("B200ZK_MSM_GLV_G2") && getenv("B200ZK_MSM_GLV_G2")[0] == '0');
-    const bool glv = !fold && glv_env && (sizeof(F) == 32 || glv2_env);   // glv.cuh; G2: the same split, phi = (beta^2 x, y)
+    const unsigned c = fold ? tab_c : choose_window(n);
+    // every other MSM splits its scalars (glv.cuh; G2: the same split, phi = (beta^2 x, y))
     const unsigned Wh = (128 + c - 1) / c;                   // |k1|, |k2| < 2^127: Wh * c >= 128 leaves the carry room
-    const unsigned W = glv ? 2 * Wh : (255 + c - 1) / c;     // digit windows
+    const unsigned W = fold ? msm_table_windows(c) : 2 * Wh; // digit windows
     const unsigned WB = fold ? 1 : W;                        // bucket sets
     if ((uint64_t)W * n >= (fold ? (1ull << 31) : (1ull << 32)))
         return set_error(ctx, B200ZK_ERR_ARG, "MSM too large for 32-bit bucket offsets / entry indices (W * n)");
@@ -619,70 +601,39 @@ static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, c
     // Small bucket sets (<= 8192 16-bucket segments in all: a 30 k-point MSM, the small windows of a 2^16 one) are reduced by one
     // QUAD per segment (k_msm_reduce_segments_quad) and, being pure latency chains, in 8-bucket segments whatever the caller's
     // hint: 16 + ~16 dependent point operations per segment instead of 64 + ~15 with the 32-bucket segments a 2^20 proof prefers.
-    static const bool quad_env = !(getenv("B200ZK_MSM_QUAD_REDUCE") && getenv("B200ZK_MSM_QUAD_REDUCE")[0] == '0');
-    const bool quad_reduce = quad_env && (uint64_t)WB * (B / seg_len) <= 8192;
-    {
-        static const int seg_env = getenv("B200ZK_MSM_SEG") ? atoi(getenv("B200ZK_MSM_SEG")) : 0;
-        if (seg_env >= 2 && (seg_env & (seg_env - 1)) == 0 && (uint32_t)seg_env <= B) seg_len = (uint32_t)seg_env;
-        else if (quad_reduce) seg_len = B < 8 ? B : 8;
-        else if (ctx->msm_seg_hint && ctx->msm_seg_hint <= B) seg_len = ctx->msm_seg_hint;
-    }
+    const bool quad_reduce = (uint64_t)WB * (B / seg_len) <= 8192;
+    if (quad_reduce) seg_len = B < 8 ? B : 8;
+    else if (ctx->msm_seg_hint && ctx->msm_seg_hint <= B) seg_len = ctx->msm_seg_hint;
     const uint32_t nseg = B / seg_len;
     // fold (one bucket set): the segment partials are summed by `wsplit` blocks whose results the Horner kernel adds up
     const uint32_t wsplit = fold ? (nseg >= 16 * 256 ? 16 : (nseg >= 1024 ? 4 : 1)) : 1;
 
-    // window groups: consecutive bucket sets (GLV: whole windows, i.e. both halves).  Measured on an earlier GPU:
+    // window groups: consecutive bucket sets (whole windows, i.e. both GLV halves).  Measured on an earlier GPU:
     // at 2^20 the extra launches, the drain bubble at the end of every bucket kernel and the slowdown of the latency-bound
     // tail kernels when they share SMs with a bucket kernel cost more than the hidden tail saves (1 group beats 2 and 4);
-    // from 2^22 up four groups win.  Fixed-base tables have one bucket set;
+    // from 2^22 up four groups win; uneven groups lose.  Fixed-base tables have one bucket set;
     // several input parts already cut the bucket work into pieces.
+    const unsigned unit_sets = fold ? 1 : 2;
+    const unsigned units = fold ? 1 : Wh;                    // windows
     unsigned ngroups = 1;
-    if (!fold && nparts == 1) {
-        static const int g_env = getenv("B200ZK_MSM_GROUPS") ? atoi(getenv("B200ZK_MSM_GROUPS")) : 0;
-        const unsigned nunits = glv ? Wh : W;                // windows
-        unsigned want = g_env > 0 ? (unsigned)g_env : (n >= (1u << 22) ? 4u : 1u);
-        if (want > nunits) want = nunits;
-        ngroups = want;
-    }
-    const unsigned unit_sets = glv ? 2 : 1;
-    const unsigned units = (fold ? 1 : (glv ? Wh : W));
-    // B200ZK_MSM_GROUP_UNITS = "u1,u2,...": explicit group sizes in windows (top windows first), e.g. "7,1": the tail of the seven
-    // top windows runs under the bucket kernel of the last one.  Ignored unless the sizes add up to the number of windows.
-    unsigned bounds[17] = {0};
-    bool custom_units = false;
-    if (!fold && nparts == 1) {
-        static const char* gu_env = getenv("B200ZK_MSM_GROUP_UNITS");
-        if (gu_env) {
-            unsigned k = 0, sum = 0;
-            const char* w = gu_env;
-            while (*w && k < 16) {
-                unsigned v = (unsigned)strtoul(w, const_cast<char**>(&w), 10);
-                if (v) { sum += v; bounds[++k] = sum; }
-                while (*w == ',' || *w == ' ') ++w;
-            }
-            if (k >= 1 && sum == units) { custom_units = true; ngroups = k; }
-        }
-    }
-    auto group_first_unit = [&](unsigned g) {
-        return custom_units ? bounds[g] : (unsigned)(((uint64_t)units * g) / ngroups);                  // default: balanced split
-    };
+    if (!fold && nparts == 1 && n >= (1u << 22)) ngroups = units < 4 ? units : 4;
+    auto group_first_unit = [&](unsigned g) { return (unsigned)(((uint64_t)units * g) / ngroups); };   // balanced split
     const uint32_t rmw = nparts > 1 ? 1u : 0u;               // bucket kernels add into the shared buckets
 
     // Streams.  One group and one part (every MSM of a proof, the 2^20 benchmark point): nothing to overlap inside the MSM, so
     // everything runs in order on the caller's stream -- a high-priority side stream would only let this MSM's
     // reductions take SM time from the bucket kernels of the proof's other MSMs (measured: a slower 2^20 proof).
-    // Otherwise `seq` (side stream / lane stream) runs sort + tail and `acc` the bucket kernels.
-    const bool split_streams = ms.result_on_seq || ngroups > 1 || nparts > 1;
+    // Otherwise `seq` (the side stream) runs sort + tail and `acc` the bucket kernels.
+    const bool split_streams = ngroups > 1 || nparts > 1;
     const cudaStream_t st = split_streams ? ms.seq : ms.acc, ast = ms.acc;
-    const bool handshake = split_streams && !ms.result_on_seq;
-    if (handshake) {                      // inputs were produced in `result`-stream order
+    if (split_streams) {                  // inputs were produced in `acc`-stream order
         cudaEvent_t e = next_event();
         if (!e) return set_error(ctx, B200ZK_ERR_CUDA, "cudaEventCreate failed");
         B2_CUDA_OK(ctx, cudaEventRecord(e, ast));
         B2_CUDA_OK(ctx, cudaStreamWaitEvent(st, e, 0));
     }
-    auto finish = [&]() -> int {          // the result (written on seq) becomes visible in result-stream order
-        if (handshake) {
+    auto finish = [&]() -> int {          // the result (written on seq) becomes visible in `acc`-stream order
+        if (split_streams) {
             cudaEvent_t e = next_event();
             if (!e) return set_error(ctx, B200ZK_ERR_CUDA, "cudaEventCreate failed");
             B2_CUDA_OK(ctx, cudaEventRecord(e, st));
@@ -705,8 +656,7 @@ static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, c
     // reference's sha256 witness are 0 or 1, groth16/examples/sha256.rs:182-185) puts thousands of entries into ONE bucket:
     // 118 serial chains of 128 additions for a 30 k-point MSM.  Shorter tasks turn that bucket into ~900 parallel
     // chains of 16 plus a block-level tree (k_msm_merge_tasks); buckets that stay below 16 entries are unaffected.
-    static const bool short_env = !(getenv("B200ZK_MSM_SHORT_TASKS") && getenv("B200ZK_MSM_SHORT_TASKS")[0] == '0');
-    if (short_env && n_max <= (1u << 16))
+    if (n_max <= (1u << 16))
         while (task_len > 16 && total_max / task_len < (1u << 17)) task_len /= 2;
     const size_t max_tasks = total_max / task_len + nb + ngroups;             // per part, all groups together
     size_t o = 0;
@@ -770,22 +720,6 @@ static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, c
     for (auto& e : prepped) if (!(e = next_event())) return set_error(ctx, B200ZK_ERR_CUDA, "cudaEventCreate failed");
     for (auto& e : accumulated) if (!(e = next_event())) return set_error(ctx, B200ZK_ERR_CUDA, "cudaEventCreate failed");
 
-    bool l2_window = false;
-    if (nparts == 1 && ctx->l2_persist_max && ctx->l2_window_max) {
-        // every base point is gathered once per window (W times per launch): pin the array in L2
-        size_t bytes = n * sizeof(affine_t<F>);
-        cudaStreamAttrValue attr;
-        memset(&attr, 0, sizeof(attr));
-        attr.accessPolicyWindow.base_ptr = const_cast<void*>(parts[0].bases);
-        attr.accessPolicyWindow.num_bytes = bytes < ctx->l2_window_max ? bytes : ctx->l2_window_max;
-        double ratio = (double)ctx->l2_persist_max / (double)attr.accessPolicyWindow.num_bytes;
-        attr.accessPolicyWindow.hitRatio = ratio > 1.0 ? 1.0f : (float)ratio;
-        attr.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-        attr.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-        l2_window = cudaStreamSetAttribute(ast, cudaStreamAttributeAccessPolicyWindow, &attr) == cudaSuccess;
-        cudaGetLastError();
-    }
-
     for (unsigned p = 0; p < nparts; ++p) {
         const MsmPart& P = parts[p];
         const size_t np = P.n, total = (size_t)W * np;
@@ -814,10 +748,10 @@ static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, c
         B2_CUDA_OK(ctx, cudaMemsetAsync(counts, 0, ((size_t)nb + 1) * 4, st));
         {
             LaunchScope ls(ctx, st, "msm_digits");
-            if (glv) k_msm_digits_glv<<<(unsigned)((np + 255) / 256), 256, 0, st>>>(reinterpret_cast<const Fr*>(P.scalars), (uint32_t)np, c,
-                                                                                   Wh, keys, ranks, counts);
-            else k_msm_digits<<<(unsigned)((np + 255) / 256), 256, 0, st>>>(reinterpret_cast<const Fr*>(P.scalars), (uint32_t)np, c, W,
-                                                                              fold ? 1u : 0u, keys, ranks, counts);
+            if (fold) k_msm_digits<<<(unsigned)((np + 255) / 256), 256, 0, st>>>(reinterpret_cast<const Fr*>(P.scalars), (uint32_t)np, c, W,
+                                                                               keys, ranks, counts);
+            else k_msm_digits_glv<<<(unsigned)((np + 255) / 256), 256, 0, st>>>(reinterpret_cast<const Fr*>(P.scalars), (uint32_t)np, c,
+                                                                                Wh, keys, ranks, counts);
         }
         B2_TRY(check_launch(ctx, "k_msm_digits"));
         B2_TRY(exclusive_scan(ctx, st, counts, offsets, sums, nb + 1));
@@ -876,7 +810,7 @@ static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, c
             {
                 LaunchScope ls(ctx, ast, acc_name);
                 const unsigned grid = (unsigned)((G.task_cap + 127) / 128);
-                const uint32_t wave = (uint32_t)ctx->sm_count * (sizeof(F) > 32 ? B2_ACC_MINBLOCKS_G2 : B2_ACC_MINBLOCKS);
+                const uint32_t wave = (uint32_t)ctx->sm_count * (sizeof(F) > 32 ? ACC_MINBLOCKS_G2 : ACC_MINBLOCKS);
                 const affine_t<F>* bp = reinterpret_cast<const affine_t<F>*>(P.bases);
                 if (rmw) k_msm_accumulate<F, true><<<grid, 128, 0, ast>>>(bp, entries, offsets + G.b0, task_off_all + G.b0 + g, task_bucket_all + G.task_base,
                                                                        order_all + G.task_base, G.nbk, task_len, wave, buckets + G.b0, task_sums_all + G.task_base);
@@ -901,14 +835,6 @@ static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, c
             B2_CUDA_OK(ctx, cudaEventRecord(accumulated[(size_t)p * ngroups + g], ast));
         }
     }
-    if (l2_window) {
-        cudaStreamAttrValue attr;
-        memset(&attr, 0, sizeof(attr));
-        attr.accessPolicyWindow.num_bytes = 0;
-        cudaStreamSetAttribute(ast, cudaStreamAttributeAccessPolicyWindow, &attr);
-        cudaGetLastError();
-    }
-
     // ---- tail(g) on seq: merge, bucket reduction, window sums, Horner step ----------------------------------------------
     for (unsigned g = 0; g < ngroups; ++g) {
         const Group& G = groups[g];
@@ -949,8 +875,8 @@ static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, c
         {
             LaunchScope ls(ctx, st, "msm_combine");
             const uint32_t first = g == 0, last = g + 1 == ngroups;
-            if (glv) k_msm_horner_glv<F><<<1, 32, 0, st>>>(wsum + G.set0, G.nsets / 2, c, first, last, hstate, out);
-            else k_msm_horner<F><<<1, 32, 0, st>>>(wsum + (size_t)G.set0 * wsplit, G.nsets * wsplit, fold ? 0u : c, first, last, hstate, out);
+            if (fold) k_msm_horner<F><<<1, 32, 0, st>>>(wsum, wsplit, 0u, first, last, hstate, out);
+            else k_msm_horner_glv<F><<<1, 32, 0, st>>>(wsum + G.set0, G.nsets / 2, c, first, last, hstate, out);
         }
         B2_TRY(check_launch(ctx, "k_msm_horner"));
     }
@@ -961,14 +887,14 @@ static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, c
 template <class F>
 static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, const void* d_bases, const void* d_scalars, size_t n,
                         void* d_out, const char* acc_name, cudaEvent_t bases_ready, cudaEvent_t scalars_ready = nullptr,
-                        unsigned tab_c = 0, unsigned c_force = 0) {
+                        unsigned tab_c = 0) {
     const MsmPart part{d_bases, d_scalars, n, bases_ready, scalars_ready};
-    return msm_dev_impl<F>(ctx, ms, ws_buf, &part, 1, d_out, acc_name, tab_c, c_force);
+    return msm_dev_impl<F>(ctx, ms, ws_buf, &part, 1, d_out, acc_name, tab_c);
 }
 
 static MsmStreams slot_streams(b200zk_ctx* ctx, Slot& sl, int aux) {
     const int ch = 2 * (int)(&sl - ctx->slots) + (aux ? 1 : 0);
-    return MsmStreams{ctx->msm_side[ch], aux ? sl.aux_stream : sl.stream, false, ch};
+    return MsmStreams{ctx->msm_side[ch], aux ? sl.aux_stream : sl.stream, ch};
 }
 
 int msm_g1_dev(b200zk_ctx* ctx, Slot& sl, const void* d_bases, const void* d_scalars, size_t n, void* d_out,
@@ -1045,13 +971,6 @@ int msm_table_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_table, const 
     DevBuf& ws = aux ? sl.ws_msm_aux : sl.ws_msm;
     return g2 ? msm_dev_impl<Fq2>(ctx, st, ws, d_table, d_scalars, n, d_out, "msm_accumulate_g2", nullptr, nullptr, c)
               : msm_dev_impl<Fq>(ctx, st, ws, d_table, d_scalars, n, d_out, "msm_accumulate_g1", nullptr, nullptr, c);
-}
-
-int msm_lane_dev(b200zk_ctx* ctx, const MsmLane& lane, int g2, unsigned tab_c, const void* d_bases, const void* d_scalars,
-                 size_t n, void* d_out) {
-    const MsmStreams st{lane.st, lane.acc_st, true, lane.channel};
-    return g2 ? msm_dev_impl<Fq2>(ctx, st, *lane.ws, d_bases, d_scalars, n, d_out, "msm_accumulate_g2", nullptr, nullptr, tab_c)
-              : msm_dev_impl<Fq>(ctx, st, *lane.ws, d_bases, d_scalars, n, d_out, "msm_accumulate_g1", nullptr, nullptr, tab_c);
 }
 
 // Host-staged MSM in `nparts` pieces (api.cu): d_bases / d_scalars are the device staging buffers the caller is filling on its copy

@@ -100,10 +100,8 @@ struct PassParams {
     uint32_t batch_tile;
 };
 
-#ifndef B2_NTT_MINBLOCKS
-#define B2_NTT_MINBLOCKS 2      // 64 registers: four 256-thread tiles per SM (76 registers uncapped = three)
-#endif
-__global__ void __launch_bounds__(512, B2_NTT_MINBLOCKS) k_ntt_pass(PassParams p) {
+static const unsigned NTT_MINBLOCKS = 2;   // 64 registers: four 256-thread tiles per SM (76 registers uncapped = three)
+__global__ void __launch_bounds__(512, NTT_MINBLOCKS) k_ntt_pass(PassParams p) {
     extern __shared__ uint4 smem[];
     const uint32_t R = 1u << p.logR, G = 1u << p.logG;
     const uint32_t RG = R << p.logG;
@@ -264,13 +262,7 @@ static int get_plan(b200zk_ctx* ctx, cudaStream_t st, unsigned log_n, bool inver
     NttPlan* pl = new NttPlan();
     pl->log_n = log_n; pl->inverse = inverse;
     pl->coset.lo = nullptr; pl->shift.lo = nullptr;
-    // B200ZK_NTT_MAX_LOG_R (8..11, experiment): larger tiles = fewer passes (2^22 as 11 + 11), at one or two blocks per SM
-    static const unsigned max_log_r = [] {
-        const char* e = getenv("B200ZK_NTT_MAX_LOG_R");
-        unsigned v = e ? (unsigned)atoi(e) : MAX_LOG_R;
-        return v < MAX_LOG_R ? MAX_LOG_R : (v > 11 ? 11u : v);
-    }();
-    pl->npass = log_n == 0 ? 0 : (log_n + max_log_r - 1) / max_log_r;
+    pl->npass = log_n == 0 ? 0 : (log_n + MAX_LOG_R - 1) / MAX_LOG_R;
     for (unsigned i = 0; i < pl->npass; ++i) {
         pl->logR[i] = log_n / pl->npass + (i < log_n % pl->npass ? 1 : 0);
     }
@@ -415,22 +407,9 @@ static int ntt_run(b200zk_ctx* ctx, Slot& sl, NttPlan* pl, const Fr* d_in, Fr* d
         uint32_t RG = 1u << (p.logR + p.logG);
         // threads = tile / tdiv: tdiv / 4 radix-4 units per thread per stage pair.  Measured on an earlier GPU: 4 wins at
         // 2^20, the two tie at 2^22, 8 wins at 2^24 -> 8 from 2^23 up
-        static const unsigned tdiv_env = getenv("B200ZK_NTT_TDIV") ? (unsigned)atoi(getenv("B200ZK_NTT_TDIV")) : 0;
-        unsigned tdiv = tdiv_env ? tdiv_env : (pl->log_n >= 23 ? 8u : 4u);
-        if (p.logR > MAX_LOG_R) {                              // big-tile experiment: fewer columns per tile, at most 512 threads
-            static const unsigned big_log_g = getenv("B200ZK_NTT_BIG_LOG_G") ? (unsigned)atoi(getenv("B200ZK_NTT_BIG_LOG_G")) : 1u;
-            if (p.logG > big_log_g) p.logG = big_log_g;
-            RG = 1u << (p.logR + p.logG);
-            while (RG / tdiv > 512) tdiv *= 2;
-            static const bool optin = [] {
-                cudaFuncSetAttribute(k_ntt_pass, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-                return true;
-            }();
-            (void)optin;
-        }
+        const unsigned tdiv = pl->log_n >= 23 ? 8u : 4u;
         uint32_t threads = RG / tdiv < 32 ? 32 : RG / tdiv;
         size_t smem = (size_t)(2 * RG + (1u << p.logR)) * sizeof(uint4);
-        if (smem > 227 * 1024) return set_error(ctx, B200ZK_ERR_ARG, "NTT tile does not fit shared memory (B200ZK_NTT_MAX_LOG_R / B200ZK_NTT_BIG_LOG_G)");
         dim3 grid((unsigned)(((size_t)1 << log_cols) >> p.logG), batch);
         if (last && p2p && p.logM == 0 && batch >= (1u << LOG_G) && batch % (1u << LOG_G) == 0) {
             p.batch_tile = 1;

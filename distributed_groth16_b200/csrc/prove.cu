@@ -192,59 +192,25 @@ int prove_dev(b200zk_ctx* ctx, const b200zk_pk* pk, const Fr* d_z, const Fr* d_a
     // three d_msm on mux streams 0/1/2 (prove.rs:119-125): slot 1 = the G2 MSM (issued first: longest bucket kernel and
     // longest latency-bound tail), slot 2 = MSM(a_query), MSM(l_query), (MSM(b_g1_query)), slot 0 = h pipeline then
     // MSM(h_query, h).  The tails of one MSM then overlap the bucket kernels of another.
-    // B200ZK_PROVE_SCHED=lanes is the alternative that was measured and lost at 2^20: one stream pair
-    // per MSM (common.cuh: lane_main / lane_acc), bucket kernels at the lowest priority, h pipeline at the highest.
-    // It removes the idle stretches of the default schedule, but the proof is bound by total multiplier work and the
-    // reductions then compete with the bucket kernels (tools/prove_timeline.py).
-    static const char* sched_env = getenv("B200ZK_PROVE_SCHED");
-    static const bool use_lanes = sched_env && !strcmp(sched_env, "lanes");
-    int rc = B200ZK_OK;
+    // One stream pair per MSM with bucket kernels at the lowest priority and the h pipeline at the highest was measured
+    // and lost at 2^20: it removes the idle stretches of this schedule, but the proof is bound by total multiplier work
+    // and the reductions then compete with the bucket kernels (tools/prove_timeline.py).
     ctx->msm_seg_hint = 32;            // bucket reduction in 32-bucket segments: 21% fewer group operations than 16, and
                                        // its longer dependency chains are hidden by the concurrent MSMs
-    if (use_lanes) {
-        auto msm = [&](int lane_id, DevBuf& ws, int k, int g2, const void* query, const Fr* scalars, size_t n, void* out) -> int {
-            MsmLane lane{ctx->lane_main[lane_id], &ws, ctx->lane_acc[lane_id], 6 + lane_id};
-            return msm_lane_dev(ctx, lane, g2, pk->tab_c[k], pk->tab_c[k] ? pk->tab[k] : query, scalars, n, out);
-        };
-        cudaStreamWaitEvent(ctx->hi_stream, ev_in, 0);
-        cudaStream_t normal = s0.stream;
-        s0.stream = ctx->hi_stream;                          // h_circom_dev launches on the slot's stream
-        rc = h_circom_dev(ctx, s0, d_a, d_b, d_c, log_m, d_h);
-        s0.stream = normal;
-        cudaEventRecord(ctx->lane_ev[4][2], ctx->hi_stream);
-        cudaStreamWaitEvent(ctx->lane_main[4], ctx->lane_ev[4][2], 0);
-        // the lanes borrow the MSM workspaces of slots 1 and 2: order them after whatever those slots still have in flight
-        cudaEventRecord(ev1, s1.stream);
-        cudaEventRecord(ev2, s2.stream);
-        for (int k = 0; k < 4; ++k) {
-            cudaStreamWaitEvent(ctx->lane_main[k], ev_in, 0);
-            cudaStreamWaitEvent(ctx->lane_main[k], (k == 0 || k == 3) ? ev1 : ev2, 0);
-        }
-        if (!rc) rc = msm(0, s1.ws_msm, 2, 1, b2q + 128, d_z + 1, n1, sm + o_b2);
-        if (!rc) rc = msm(1, s2.ws_msm, 0, 0, aq + 64, d_z + 1, n1, sm + o_a);
-        if (!rc) rc = msm(2, s2.ws_msm_aux, 3, 0, pk->l_query, d_z + pk->n_inputs, n_aux, sm + o_l);
-        if (!rc && need_b1) rc = msm(3, s1.ws_msm_aux, 1, 0, b1q + 64, d_z + 1, n1, sm + o_b1);
-        if (!rc) rc = msm(4, s0.ws_msm, 4, 0, pk->h_query, d_h, m, sm + o_h);
-        for (int k = 0; k < 5; ++k) {
-            cudaEventRecord(ctx->lane_ev[k][2], ctx->lane_main[k]);
-            cudaStreamWaitEvent(st, ctx->lane_ev[k][2], 0);
-        }
-    } else {
-        auto msm = [&](Slot& sl, int k, int g2, const void* query, const Fr* scalars, size_t n, void* out) -> int {
-            if (pk->tab_c[k]) return msm_table_dev(ctx, sl, g2, pk->tab[k], scalars, n, pk->tab_c[k], out);
-            return g2 ? msm_g2_dev(ctx, sl, query, scalars, n, out) : msm_g1_dev(ctx, sl, query, scalars, n, out);
-        };
-        rc = msm(s1, 2, 1, b2q + 128, d_z + 1, n1, sm + o_b2);
-        if (!rc) rc = msm(s2, 0, 0, aq + 64, d_z + 1, n1, sm + o_a);
-        if (!rc) rc = msm(s2, 3, 0, pk->l_query, d_z + pk->n_inputs, n_aux, sm + o_l);
-        if (!rc && need_b1) rc = msm(s2, 1, 0, b1q + 64, d_z + 1, n1, sm + o_b1);
-        if (!rc) rc = h_circom_dev(ctx, s0, d_a, d_b, d_c, log_m, d_h);
-        if (!rc) rc = msm(s0, 4, 0, pk->h_query, d_h, m, sm + o_h);
-        cudaEventRecord(ev1, s1.stream);
-        cudaEventRecord(ev2, s2.stream);
-        cudaStreamWaitEvent(st, ev1, 0);
-        cudaStreamWaitEvent(st, ev2, 0);
-    }
+    auto msm = [&](Slot& sl, int k, int g2, const void* query, const Fr* scalars, size_t n, void* out) -> int {
+        if (pk->tab_c[k]) return msm_table_dev(ctx, sl, g2, pk->tab[k], scalars, n, pk->tab_c[k], out);
+        return g2 ? msm_g2_dev(ctx, sl, query, scalars, n, out) : msm_g1_dev(ctx, sl, query, scalars, n, out);
+    };
+    int rc = msm(s1, 2, 1, b2q + 128, d_z + 1, n1, sm + o_b2);
+    if (!rc) rc = msm(s2, 0, 0, aq + 64, d_z + 1, n1, sm + o_a);
+    if (!rc) rc = msm(s2, 3, 0, pk->l_query, d_z + pk->n_inputs, n_aux, sm + o_l);
+    if (!rc && need_b1) rc = msm(s2, 1, 0, b1q + 64, d_z + 1, n1, sm + o_b1);
+    if (!rc) rc = h_circom_dev(ctx, s0, d_a, d_b, d_c, log_m, d_h);
+    if (!rc) rc = msm(s0, 4, 0, pk->h_query, d_h, m, sm + o_h);
+    cudaEventRecord(ev1, s1.stream);
+    cudaEventRecord(ev2, s2.stream);
+    cudaStreamWaitEvent(st, ev1, 0);
+    cudaStreamWaitEvent(st, ev2, 0);
     ctx->msm_seg_hint = 0;
     if (rc) {
         cudaStreamSynchronize(st);

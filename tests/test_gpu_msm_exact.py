@@ -1,15 +1,13 @@
-"""The MSM (csrc/msm.cu) against exact answers at every window width, pipeline switch and size up to 2^26.
+"""The MSM (csrc/msm.cu) against exact answers at every window width and size up to 2^26.
 
 The bases are generated with known discrete logs, P_i = k_i G (tests/dlog_oracle.py), so MSM(P, s) = (sum_i k_i s_i) G
 is known exactly at any size without running another MSM.  Covered here:
-  - the default configuration at 2^20 .. 2^26 (device-resident, host-staged in parts, fixed-base table), with the
-    generated points themselves spot-checked against k_i G;
+  - the default configuration at 2^20 .. 2^26 (device-resident with its window groups, host-staged in parts, fixed-base
+    table), with the generated points themselves spot-checked against k_i G, and host-staged MSMs of 1, 5 and 15 pairs;
   - every window width B200ZK_MSM_WINDOW = 2..23 on G1 and 2..20 on G2 (read on every call), each with digit-pattern
-    scalar families that put B, B + 1 or 2^c - 1 into every window of k (plain path) or of both GLV halves; at 2^20 the
-    small widths (c <= 8) also run task lengths above 128 and block-level merges of the giant buckets.  Width 24 needs
-    about 33 GB of G1 bucket workspace (10^8 buckets with their task sums) and is left out;
-  - the same sweep without GLV, and every MSM switch (segment length, window groups and their explicit sizes, input
-    parts with empty ones, part weights, thread reduction, long tasks, G2 without GLV), one fresh process each;
+    scalar families that put B, B + 1 or 2^c - 1 into every window of both GLV halves; at 2^20 the small widths
+    (c <= 8) also run task lengths above 128 and block-level merges of the giant buckets.  Width 24 needs about 33 GB of
+    G1 bucket workspace (10^8 buckets with their task sums) and is left out;
   - adversarial bucket contents: one point n times, P and -P, s and r - s, and +-G bases whose bucket counts make a
     running sum of the segment reduction hit the identity and equal the bucket it adds (quad and thread reduction);
   - the W * n >= 2^32 guard, which must refuse before any allocation;
@@ -17,12 +15,8 @@ is known exactly at any size without running another MSM.  Covered here:
     `wsplit` branches, a G2 table at 2^20, and the fold path's W * n >= 2^31 guard.
 A failure names the configuration, the family and the size.
 
-Measured on one H100 80GB HBM3 at a 700 W power limit: 279 s for the file, host oracle and subprocess start-up included.
-The table section added later takes about 10 s (H100 80GB HBM3, 400 W power limit)."""
-import json
+Measured on one H100 80GB HBM3 at a 700 W power limit: 180 s for the file, host oracle included."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -76,10 +70,9 @@ def _check_generated(net, seed, n, g2, what, staged=False):
     return bases
 
 
-def _family_scalars(c, glv):
-    fams = dl.digit_families(c, glv)
-    if glv:
-        fams["glv_halves"] = [dl.glv_compose(a, b) for a, b in dl.glv_designed_halves()] + list(_extremes())
+def _family_scalars(c):
+    fams = dl.digit_families(c, True)
+    fams["glv_halves"] = [dl.glv_compose(a, b) for a, b in dl.glv_designed_halves()] + list(_extremes())
     return fams
 
 
@@ -92,13 +85,12 @@ def _extremes():
     return _EXT
 
 
-def _check_families(net, c, g2, glv, what):
-    """one MSM per scalar family on the first generated bases; for GLV the designed halves are confirmed first"""
+def _check_families(net, c, g2, what):
+    """one MSM per scalar family on the first generated bases; the designed GLV halves are confirmed first"""
     import torch
-    fams = _family_scalars(c, glv)
-    if glv:
-        for a, b in dl.glv_designed_halves():
-            assert dl.glv_decompose(dl.glv_compose(a, b)) == (a, b)
+    fams = _family_scalars(c)
+    for a, b in dl.glv_designed_halves():
+        assert dl.glv_decompose(dl.glv_compose(a, b)) == (a, b)
     seed = 0xFA000000 + c
     m = max(len(v) for v in fams.values())
     bases = net.generate_g2(seed, m) if g2 else net.generate_g1(seed, m)
@@ -109,13 +101,13 @@ def _check_families(net, c, g2, glv, what):
         _check_point(got, want, "%s family %s" % (what, name))
 
 
-def _sweep_one(net, c, g2, glv, big=True):
+def _sweep_one(net, c, g2, big=True):
     os.environ["B200ZK_MSM_WINDOW"] = str(c)
     try:
-        what = "%s c=%d glv=%s" % ("G2" if g2 else "G1", c, glv)
+        what = "%s c=%d" % ("G2" if g2 else "G1", c)
         for n in (3001, 40000) + (((1 << 20),) if big and c <= 8 else ()):
             _check_generated(net, 0xC0000000 + 1000 * c + n % 997, n, g2, "%s n=%d" % (what, n))
-        _check_families(net, c, g2, glv, what)
+        _check_families(net, c, g2, what)
     finally:
         del os.environ["B200ZK_MSM_WINDOW"]
 
@@ -196,9 +188,15 @@ def _spot_check_points(bases, seed, g2):
 @pytest.mark.parametrize("g2,n", [(False, 1 << 20), (False, (1 << 22) + 1), (False, (1 << 23) - 1), (False, 1 << 24),
                                   (False, 1 << 26), (True, 1 << 20), (True, 1 << 22)])
 def test_size_ladder_device_resident(net, g2, n):
+    """also the window groups: one Horner step per group, 1 group below 2^22 and 4 from there up"""
     import torch
     seed = 0xA1000000 + n
+    net.profile(True)
+    net.profile_reset()
     bases = _check_generated(net, seed, n, g2, "default %s n=%d" % ("G2" if g2 else "G1", n))
+    rep = net.profile_report()
+    net.profile(False)
+    assert rep["msm_combine"]["launches"] == (4 if n >= 1 << 22 else 1), rep["msm_combine"]
     _spot_check_points(bases, seed, g2)
     del bases
     torch.cuda.empty_cache()
@@ -214,6 +212,13 @@ def test_size_ladder_host_staged(net, g2, log_n):
     rep = net.profile_report()
     net.profile(False)
     assert rep["msm_digits"]["launches"] == 5                 # one sort per part
+
+
+@pytest.mark.parametrize("g2", [False, True], ids=["g1", "g2"])
+def test_host_staged_tiny(net, g2):
+    """host-staged MSMs of 1, 5 and 15 pairs: one part each"""
+    for n in (1, 5, 15):
+        _check_generated(net, 0xB2000000 + n, n, g2, "tiny %s n=%d host-staged" % ("G2" if g2 else "G1", n), staged=True)
 
 
 def test_fixed_base_table_2_22_c20(net):
@@ -234,12 +239,12 @@ def test_fixed_base_table_2_22_c20(net):
 # ---- 2. window sweep ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("c", G1_WINDOWS)
 def test_window_sweep_g1(net, c):
-    _sweep_one(net, c, False, True)
+    _sweep_one(net, c, False)
 
 
 @pytest.mark.parametrize("c", G2_WINDOWS)
 def test_window_sweep_g2(net, c):
-    _sweep_one(net, c, True, True, big=False)
+    _sweep_one(net, c, True, big=False)
 
 
 # ---- 3. adversarial bucket contents ---------------------------------------------------------------------------------
@@ -276,6 +281,15 @@ def test_bucket_running_sum_collisions_quad_reduce(net, g2):
     check_collisions(net, g2, seg_len=8)                  # small bucket sets: one quad per 8-bucket segment
 
 
+@pytest.mark.parametrize("g2", [False, True], ids=["g1", "g2"])
+def test_bucket_running_sum_collisions_thread_reduce(net, g2):
+    """c = 16: 2 x 8 GLV bucket sets of 2048 16-bucket segments, more than the 8192 the quad reduction takes, so one thread
+    reduces each 16-bucket segment"""
+    c, seg_len = 16, 16
+    assert 2 * (-(-128 // c)) * ((1 << (c - 1)) // seg_len) > 8192
+    check_collisions(net, g2, seg_len, c=c)
+
+
 def test_size_guard_refuses_before_launch(net, monkeypatch):
     """c = 2 gives W = 128 digit windows: 2^25 points make W * n = 2^32 entries, past the 32-bit offsets"""
     import torch
@@ -290,104 +304,14 @@ def test_size_guard_refuses_before_launch(net, monkeypatch):
     torch.cuda.empty_cache()
 
 
-# ---- 4. switches: one fresh process each ------------------------------------------------------------------------------
-def run_switch_checks(spec):
-    """Body of one switch subprocess: G1 and G2 at two sizes, device-resident and host-staged, the +-G collision case, and
-    the effect the switch must have (window groups, input parts) read from the profile."""
-    import torch
-    from distributed_groth16_b200 import Net
-    net = Net(0)
-    net.use_torch_stream(0)
-    if spec.get("sweep_glv0"):
-        for c in G1_WINDOWS:
-            _sweep_one(net, c, False, False)
-        torch.cuda.synchronize()
-        net.close()
-        return
-    if "window" in spec:
-        os.environ["B200ZK_MSM_WINDOW"] = str(spec["window"])
-    for g2 in (False, True):
-        for n in spec.get("sizes", (3001, (1 << 17) + 3)):
-            what = "%s %s n=%d" % (spec["name"], "G2" if g2 else "G1", n)
-            net.profile(True)
-            net.profile_reset()
-            _check_generated(net, 0xB0000000 + n, n, g2, what + " device")
-            rep = net.profile_report()
-            if "groups" in spec and not g2:
-                assert rep["msm_combine"]["launches"] == spec["groups"], (what, rep["msm_combine"])
-            net.profile_reset()
-            _check_generated(net, 0xB1000000 + n, n, g2, what + " host-staged", staged=True)
-            rep = net.profile_report()
-            if "parts" in spec:
-                assert rep["msm_digits"]["launches"] == min(spec["parts"], n), (what, rep["msm_digits"])
-            net.profile(False)
-    for n in spec.get("tiny", ()):
-        for g2 in (False, True):
-            _check_generated(net, 0xB2000000 + n, n, g2, "%s tiny n=%d host-staged" % (spec["name"], n), staged=True)
-    os.environ.pop("B200ZK_MSM_WINDOW", None)
-    for g2 in (False, True):
-        check_collisions(net, g2, spec.get("seg_len", 8))
-    torch.cuda.synchronize()
-    net.close()
-
-
-# seg_len: the segment length the +-G collision case (c = 5, B = 16) runs with under the switch; a forced length above B is
-# ignored there, and the small bucket set keeps its 8-bucket quads
-SWITCHES = [
-    ({"B200ZK_MSM_SEG": "2"}, {"seg_len": 2}),
-    ({"B200ZK_MSM_SEG": "4"}, {"seg_len": 4}),
-    ({"B200ZK_MSM_SEG": "32"}, {"seg_len": 8}),
-    ({"B200ZK_MSM_SEG": "64"}, {"seg_len": 8}),
-    ({"B200ZK_MSM_GROUPS": "2"}, {"groups": 2}),
-    ({"B200ZK_MSM_GROUPS": "3"}, {"groups": 3}),
-    ({"B200ZK_MSM_GROUPS": "7"}, {"groups": 7}),
-    ({"B200ZK_MSM_GROUP_UNITS": "7,1"}, {"window": 16, "groups": 2}),
-    ({"B200ZK_MSM_GROUP_UNITS": ",".join(["1"] * 10)}, {"window": 13, "groups": 10}),
-    ({"B200ZK_MSM_PARTS": "2"}, {"parts": 2}),
-    ({"B200ZK_MSM_PARTS": "7"}, {"parts": 7}),
-    ({"B200ZK_MSM_PARTS": "16"}, {"parts": 16, "tiny": (1, 5, 15)}),
-    ({"B200ZK_MSM_PART_WEIGHTS": "1,3"}, {"parts": 2}),
-    ({"B200ZK_MSM_PART_WEIGHTS": "5,1,1"}, {"parts": 3}),
-    ({"B200ZK_MSM_QUAD_REDUCE": "0"}, {"seg_len": 16}),
-    ({"B200ZK_MSM_SHORT_TASKS": "0"}, {}),
-    ({"B200ZK_MSM_GLV_G2": "0"}, {}),
-    ({"B200ZK_MSM_GLV": "0"}, {"sweep_glv0": True}),
-]
-
-
-def _switch_id(env):
-    return "-".join("%s=%s" % (k.replace("B200ZK_MSM_", "").lower(), v if len(v) < 8 else "1x10") for k, v in env.items())
-
-
-SCRIPT = r"""
-import json, sys
-sys.path.insert(0, %r)
-sys.path.insert(0, %r)
-import test_gpu_msm_exact as t
-t.run_switch_checks(json.loads(%r))
-print("switch checks ok")
-"""
-
-
-@pytest.mark.parametrize("env,spec", SWITCHES, ids=[_switch_id(e) for e, _ in SWITCHES])
-def test_switch_matrix(env, spec):
-    spec = dict(spec, name=_switch_id(env))
-    e = dict(os.environ)
-    e.pop("B200ZK_MSM_WINDOW", None)
-    e.update(env)
-    r = subprocess.run([sys.executable, "-c", SCRIPT % (ROOT, HERE, json.dumps(spec))], env=e, capture_output=True, text=True,
-                       timeout=900, cwd=ROOT)
-    assert r.returncode == 0 and "switch checks ok" in r.stdout, r.stdout[-2000:] + r.stderr[-4000:]
-
-
-# ---- 5. fixed-base tables: window sweep, G2 at 2^20, the fold guard -----------------------------------------------------
+# ---- 4. fixed-base tables: window sweep, G2 at 2^20, the fold guard -----------------------------------------------------
 TABLE_G1_WINDOWS = list(range(2, 25))
 TABLE_G2_WINDOWS = list(range(2, 21))
 PROVER_TABLE_WINDOWS = (7, 16, 22)           # B200ZK_PK_TABLE_WINDOW in test_gpu_prove_exact.py (32-bucket segment hint)
 
 
 def table_seg_len(c, hint=0):
-    """segment length of a fixed-base table MSM (one bucket set), as msm_dev_impl picks it without B200ZK_MSM_SEG"""
+    """segment length of a fixed-base table MSM (one bucket set), as msm_dev_impl picks it"""
     B = 1 << (c - 1)
     seg = min(B, 16)
     if B // seg <= 8192:                     # quad reduction: 8-bucket segments whatever the hint

@@ -10,14 +10,14 @@ twin in tests/test_prove_dlog_oracle.py).  No curve MSM is needed for the expect
     the host-staged entry point;
   - key shapes: n_vars in {1, 40, m, 3m + 7}, n_inputs in {1, 2, 17, n_vars}, query rows at infinity (index 0, half the
     b-queries, all of l_query), and the exact table bytes of the mixed case where short queries get no table;
+    n_inputs = n_vars also at 2^20 and 2^22, over the tables and the generic MSM;
   - the table budget and window variables, and the W * n >= 2^31 guard of the table build;
-  - the switches read once per process (lanes schedule, window groups, two-level NTT twiddles, no GLV), one fresh
-    process each;
+  - the two-level NTT twiddle tables (B200ZK_NTT_BIGTAB=0, read once per process) in a fresh process;
   - one Net reused across sizes and live keys, and a proof running while other host threads use slots 1 and 2.
 A failure names the size, the configuration, the witness family and the (r, s) case.
 
-Measured on one H100 80GB HBM3 at a 400 W power limit: about 500 s for the file, most of it in the 2^24 leg (CPU h and
-the exact dot products) and the subprocess start-ups."""
+Measured on one H100 80GB HBM3 at a 700 W power limit: 433 s for the file, most of it in the 2^24 leg (CPU h and the
+exact dot products)."""
 import json
 import os
 import subprocess
@@ -135,7 +135,7 @@ def rs_cases(e, full):
 def net():
     """This module's own GPU party, closed when the module ends.  The 2^22 and 2^24 legs grow the slot workspaces to tens
     of GB; on the session's Net they would stay allocated for the rest of the run, and the key tables of later tests and
-    other processes are sized by the HBM left free.  The switch subprocesses run first, before this Net exists."""
+    other processes are sized by the HBM left free.  The switch subprocess runs first, before this Net exists."""
     import torch
     from distributed_groth16_b200 import Net
     n = Net(0)
@@ -147,41 +147,41 @@ def net():
     torch.cuda.empty_cache()
 
 
-# ---- 1. switches read once per process ------------------------------------------------------------------------------------
+# ---- 1. the two-level NTT twiddle tables (read once per process) ------------------------------------------------------------
+def prove_legs(net, cref, legs, name, all_inputs=False):
+    """per (log_m, path) a key with n_inputs = 2, or n_inputs = n_vars when `all_inputs`, proved at (0, 0) and random (r, s)"""
+    import torch
+    for log_m, path in legs:
+        m = 1 << log_m
+        abc = qap_inputs(net, cref, m)
+        z, zh = witness(net, m, "random", 0x66000000 + log_m)
+        ni = m if all_inputs else 2
+        key = po.KeySpec(m, m, ni, 0x67000000 + 64 * log_m + (ni == m))
+        e = po.exponents(key, zh, abc[3])
+        pk = make_key(net, key, tables=path == "tables")
+        if path == "tables":
+            require_tables(pk, "%s m=2^%d" % (name, log_m))
+        for cname, (r, s) in rs_cases(e, full=False).items():
+            check_proof(pk, e, z, abc, r, s, "%s m=2^%d %s n_inputs=%d rs=%s" % (name, log_m, path, ni, cname))
+        pk.free()
+        torch.cuda.empty_cache()
+
+
 def run_prove_switch(spec):
-    """Body of one switch subprocess: per (log_m, path) a key with n_inputs = 2 and, where asked, one with
-    n_inputs = n_vars, proved at (0, 0) and random (r, s)."""
+    """Body of one switch subprocess"""
     import torch
     from distributed_groth16_b200 import Net
     from oracle import cref
     cref.build()
     net = Net(0)
     net.use_torch_stream(0)
-    for log_m, path in spec["legs"]:
-        m = 1 << log_m
-        abc = qap_inputs(net, cref, m)
-        z, zh = witness(net, m, "random", 0x66000000 + log_m)
-        for ni in (2, m) if spec.get("all_inputs") else (2,):
-            key = po.KeySpec(m, m, ni, 0x67000000 + 64 * log_m + (ni == m))
-            e = po.exponents(key, zh, abc[3])
-            pk = make_key(net, key, tables=path == "tables")
-            if path == "tables":
-                require_tables(pk, "%s m=2^%d" % (spec["name"], log_m))
-            for cname, (r, s) in rs_cases(e, full=False).items():
-                check_proof(pk, e, z, abc, r, s, "%s m=2^%d %s n_inputs=%d rs=%s" % (spec["name"], log_m, path, ni, cname))
-            pk.free()
-        torch.cuda.empty_cache()
+    prove_legs(net, cref, spec["legs"], spec["name"])
     torch.cuda.synchronize()
     net.close()
 
 
 PROVE_SWITCHES = [
-    ({"B200ZK_PROVE_SCHED": "lanes"}, {"legs": [(16, "tables"), (20, "tables"), (22, "tables"), (22, "generic")],
-                                       "all_inputs": True}),
-    ({"B200ZK_MSM_GROUPS": "2"}, {"legs": [(20, "generic")]}),
-    ({"B200ZK_MSM_GROUPS": "7"}, {"legs": [(20, "generic")]}),
     ({"B200ZK_NTT_BIGTAB": "0"}, {"legs": [(20, "tables")]}),
-    ({"B200ZK_MSM_GLV": "0"}, {"legs": [(16, "generic"), (16, "tables")]}),
 ]
 
 SCRIPT = r"""
@@ -362,7 +362,15 @@ def test_prove_while_other_threads_use_slots_1_and_2(net, cref):
     pk.free()
 
 
-# ---- 7. size ladder -----------------------------------------------------------------------------------------------------
+# ---- 7. every variable public -----------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("log_m,path", [(20, "tables"), (22, "tables"), (22, "generic")])
+def test_all_inputs_public(net, cref, log_m, path):
+    """n_inputs = n_vars: the l_query MSM is empty (n = 0).  Runs before the size ladder: its 2^24 leg grows this module's slot
+    workspaces until 60% of the free HBM no longer holds the 2^22 tables."""
+    prove_legs(net, cref, [(log_m, path)], "n_inputs=n_vars", all_inputs=True)
+
+
+# ---- 8. size ladder -----------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("log_m", LADDER)
 def test_size_ladder(net, cref, log_m, monkeypatch):
     import torch
@@ -406,3 +414,4 @@ def test_size_ladder(net, cref, log_m, monkeypatch):
     pk.free()
     del wits
     torch.cuda.empty_cache()
+
