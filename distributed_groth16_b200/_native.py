@@ -127,6 +127,7 @@ SIGNATURES = {
     "b200zk_group_groth16_prove": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b200zk_fr_op": (ctypes.c_int, [c_vp, ctypes.c_int, c_vp, c_vp, c_vp, ctypes.c_size_t]),
     "b200zk_test_field_op": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, c_vp, c_vp, ctypes.c_size_t]),
+    "b200zk_test_arith": (ctypes.c_int, [c_vp, ctypes.c_int, c_vp, ctypes.c_size_t, c_vp]),
 }
 
 

@@ -13,7 +13,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libb200zk.so")
-SOURCES = ["api.cu", "ntt.cu", "msm.cu", "prove.cu", "qap.cu", "setup.cu", "codec.cu", "verify.cu", "packexp.cu", "group.cu"]
+SOURCES = ["api.cu", "ntt.cu", "msm.cu", "prove.cu", "qap.cu", "setup.cu", "codec.cu", "verify.cu", "packexp.cu", "group.cu",
+           "selftest.cu"]
 ARCH = "sm_90a"
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = GENCODE + ["-O3", "-lineinfo", "-std=c++17",

@@ -21,7 +21,9 @@
 
 #if defined(__CUDACC__)
 #define B2_HD __host__ __device__ __forceinline__
-#define B2_HD_NI __host__ __device__ __noinline__
+// inline: only the linkage (the free functions of codec.cuh / pairing.cuh are defined in every translation unit that
+// includes them); __noinline__ still keeps each one a single out-of-line copy per unit
+#define B2_HD_NI __host__ __device__ __noinline__ inline
 #else
 #define B2_HD inline __attribute__((always_inline))
 #define B2_HD_NI inline

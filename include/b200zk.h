@@ -360,6 +360,29 @@ int b200zk_fr_op(b200zk_ctx* ctx, int op, const uint64_t* a, const uint64_t* b, 
 /* op: 0 mul, 1 add, 2 sub; field: 0 Fq, 1 Fr.  a, b, out: n x 4 limbs host buffers. */
 int b200zk_test_field_op(b200zk_ctx* ctx, int field, int op, const uint64_t* a, const uint64_t* b, uint64_t* out,
                          size_t n);
+/* One device primitive of csrc/fp.cuh, codec.cuh, pairing.cuh, glv.cuh or ec.cuh per element (csrc/selftest.cu), for the
+ * exact tests against big integers.  in: n records of IN u64 words, out: n records of OUT words (host buffers).  Field
+ * elements are raw Montgomery limbs (Fq / Fr 4 words, Fq2 c0 c1 8, Fq6 a b c 24, Fq12 c0 c1 48); points affine_t (x y:
+ * G1 8 words, G2 16) or xyzz_t (x y zz zzz: G1 16, G2 32).  F = Fq at op s, Fr at op 32 + s:
+ *   s  0 add (a, b)   1 sub   2 neg (a)   3 dbl   4 mul (a, b)   5 mul_ni   6 sqr (a)   7 mul, b any value < 2^256
+ *   s  8/9/10 mul_k<2/3/4> (K (a, b) pairs -> K products)   11 mul_wide + redc<1> (a, b -> 512-bit a b (8 words), result)
+ *   s 12 redc<2> (512-bit t < 2 p 2^256)   13 inv   14 inv_fermat   15 to_mont   16 from_mont   17 from_u32 (1 word)
+ *   s 18 pow_u64 (a, u64 e)
+ *   64 fr_root_of_unity (1 word: log_n | inverse << 8, log_n <= 28)                                       [device only]
+ *   70 Fq2 mul (a, b)  71 sqr  72 inv  73..76 mul_group<1..4> (K pairs -> K)  77 fq2_mul_xi  78 fq2_conj
+ *   79 glv_phi_x on Fq (G1)  80 glv_phi_x on Fq2 (G2)
+ *   84 fq_pow_p1_4  85 fq_sqrt -> (flag, root)  86 fq2_sqrt -> (flag, root, zero when false)  87 fq_half
+ *   88 fq_is_larger -> flag  89 fq2_is_larger -> flag  90 fq_from_bytes (32 bytes, top_mask) -> (flag, value)
+ *   96 Fq6 mul  97 Fq6 inv  98 Fq6 mul_v  99 Fq12 mul  100 Fq12 inv  101 Fq12 conj  102 Fq12 frob2
+ *   103 final_exponentiation  104 final_exponentiation(miller_loop(P, Q)) (G1 affine, G2 affine)  105 g2_frobenius_twist
+ *   108 glv_decompose (canonical k < r) -> (|k1| 2 words, neg1, |k2| 2 words, neg2)
+ * Group law, G1 at 112 + s, G2 at 128 + s, xyzz_t in and out unless noted:
+ *   s  0 dbl  1 add (a, b)  2 dbl_ilp  3 add_ilp  4 madd (acc, affine p, u64 negate)  5 dbl_affine (affine)
+ *   s  6 to_affine -> affine  7 mul_scalar (p, 4 canonical words k < 2^256)
+ *   s  8 quad_ops<F, false>::add  9 ::dbl (one element per quad)  10 quad_ops<F, true>::add  11 ::dbl (one element per
+ *      warp)                                                                                               [device only]
+ * BAD_ARG for an unknown op. */
+int b200zk_test_arith(b200zk_ctx* ctx, int op, const uint64_t* in, size_t n, uint64_t* out);
 
 #ifdef __cplusplus
 }
