@@ -75,6 +75,8 @@ SIGNATURES = {
     "b200zk_qap_dev": (ctypes.c_int, [c_vp, ctypes.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, ctypes.c_size_t, ctypes.c_size_t,
                                       c_vp, ctypes.c_uint, c_vp, c_vp, c_vp]),
     "b200zk_fr_convert_dev": (ctypes.c_int, [c_vp, ctypes.c_int, c_vp, c_vp, ctypes.c_size_t, ctypes.c_int, ctypes.c_int]),
+    "b200zk_r1cs_check_dev": (ctypes.c_int, [c_vp, ctypes.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                             ctypes.c_size_t, c_vp, c_u64p, c_u64p]),
     "b200zk_pk_upload": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, ctypes.c_size_t, ctypes.c_size_t,
                                         ctypes.c_size_t, c_vp, ctypes.POINTER(c_vp)]),
     "b200zk_pk_upload_dev": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, ctypes.c_size_t, ctypes.c_size_t,
@@ -88,6 +90,7 @@ SIGNATURES = {
                                                 ctypes.c_size_t, c_vp]),
     "b200zk_groth16_verify": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, ctypes.c_size_t, c_vp, c_vp, c_vp, c_vp,
                                              ctypes.POINTER(ctypes.c_int)]),
+    "b200zk_vk_alphabeta_12": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp]),
     "b200zk_points_compress_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, ctypes.c_size_t, c_vp]),
     "b200zk_points_decompress_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, ctypes.c_size_t, ctypes.c_int, c_vp,
                                                     ctypes.POINTER(ctypes.c_size_t)]),

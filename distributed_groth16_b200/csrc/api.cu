@@ -486,6 +486,25 @@ int b200zk_fr_convert_dev(b200zk_ctx* ctx, int stream, const void* d_in, void* d
     B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
     return fr_convert_dev(ctx, sl, d_in, d_out, n, to_mont, times);
 }
+int b200zk_r1cs_check_dev(b200zk_ctx* ctx, int stream, const void* a_ptr, const void* a_col, const void* a_val, const void* b_ptr,
+                          const void* b_col, const void* b_val, const void* c_ptr, const void* c_col, const void* c_val, size_t nc,
+                          const void* d_w, uint64_t* n_failed, uint64_t* first_failed) {
+    if (!ctx) return B200ZK_ERR_ARG;
+    if (nc == 0) {
+        if (n_failed) *n_failed = 0;
+        if (first_failed) *first_failed = 0;
+        return B200ZK_OK;
+    }
+    if (!valid_slot(stream) || !a_ptr || !b_ptr || !c_ptr || !d_w || !n_failed || !first_failed)
+        return set_error(ctx, B200ZK_ERR_ARG, "r1cs_check: null pointer or bad stream slot");
+    Slot& sl = ctx->slots[stream];
+    std::lock_guard<std::mutex> g(sl.mu);
+    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
+    const void* ptr[3] = {a_ptr, b_ptr, c_ptr};
+    const void* col[3] = {a_col, b_col, c_col};
+    const void* val[3] = {a_val, b_val, c_val};
+    return r1cs_check_dev(ctx, sl, ptr, col, val, nc, d_w, n_failed, first_failed);
+}
 
 // ---- proving key + prove -----------------------------------------------------------------------
 static int upload(b200zk_ctx* ctx, void** dst, const void* src, size_t bytes, cudaMemcpyKind kind = cudaMemcpyHostToDevice) {
@@ -620,6 +639,13 @@ int b200zk_groth16_verify(b200zk_ctx* ctx, const uint64_t* alpha_g1, const uint6
     B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     return groth16_verify_dev(ctx, sl, alpha_g1, beta_g2, gamma_g2, delta_g2, gamma_abc_g1, n_public, public_inputs, proof_a, proof_b,
                               proof_c, is_valid);
+}
+int b200zk_vk_alphabeta_12(b200zk_ctx* ctx, const uint64_t alpha_g1[8], const uint64_t beta_g2[16], uint64_t out[48]) {
+    if (!ctx || !alpha_g1 || !beta_g2 || !out) return B200ZK_ERR_ARG;
+    Slot& sl = ctx->slots[0];
+    std::lock_guard<std::mutex> g(sl.mu);
+    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    return vk_alphabeta_12_dev(ctx, sl, alpha_g1, beta_g2, out);
 }
 
 int b200zk_xyzz_sum_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_in, size_t count, size_t stride, void* d_out) {

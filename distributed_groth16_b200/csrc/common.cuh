@@ -207,6 +207,8 @@ int fr_convert_dev(b200zk_ctx* ctx, Slot& sl, const void* d_in, void* d_out, siz
 int qap_dev(b200zk_ctx* ctx, Slot& sl, const void* a_ptr, const void* a_col, const void* a_val, const void* b_ptr,
             const void* b_col, const void* b_val, size_t nc, size_t n_inputs, const void* d_z, unsigned log_m, void* d_a,
             void* d_b, void* d_c);
+int r1cs_check_dev(b200zk_ctx* ctx, Slot& sl, const void* const ptr[3], const void* const col[3], const void* const val[3], size_t nc,
+                   const void* d_w, uint64_t* n_failed, uint64_t* first_failed);
 // setup.cu
 int fixed_base_mul_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_scalars, size_t n, void* d_out);
 int fr_powers_dev(b200zk_ctx* ctx, Slot& sl, const uint64_t base[4], const uint64_t scale[4], size_t n, void* d_out);
@@ -233,6 +235,7 @@ int points_matmul_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_points, s
 int groth16_verify_dev(b200zk_ctx* ctx, Slot& sl, const uint64_t* alpha_g1, const uint64_t* beta_g2, const uint64_t* gamma_g2,
                        const uint64_t* delta_g2, const uint64_t* gamma_abc_g1, size_t n_public, const uint64_t* public_inputs,
                        const uint64_t* proof_a, const uint64_t* proof_b, const uint64_t* proof_c, int* is_valid);
+int vk_alphabeta_12_dev(b200zk_ctx* ctx, Slot& sl, const uint64_t* alpha_g1, const uint64_t* beta_g2, uint64_t* out);
 // prove.cu
 int assemble_dev(b200zk_ctx* ctx, Slot& sl, const b200zk_pk* pk, const void* msm_a, const void* msm_b2, const void* msm_l,
                  const void* msm_h, const void* msm_b1, const uint64_t r[4], const uint64_t s[4], int include_zero_terms,

@@ -95,4 +95,44 @@ int groth16_verify_dev(b200zk_ctx* ctx, Slot& sl, const uint64_t* alpha_g1, cons
     return B200ZK_OK;
 }
 
+// snarkjs's vk_alphabeta_12.  ffjavascript's final exponentiation computes the hard part with the Fuentes-Castaneda chain,
+// which raises to m (p^4 - p^2 + 1)/r with m = 2u(6u^2 + 3u + 1), so snarkjs's e(alpha, beta) is the plain pairing of
+// pairing.cuh raised to m.  m is 190 bits; SNARKJS_M holds it little-endian.
+__constant__ uint64_t SNARKJS_M[3] = {0x2e5d4e223ddedaf4ull, 0x1ea96b02d9d9e38dull, 0x3bec47df15e307c8ull};
+constexpr int SNARKJS_M_BITS = 190;
+
+// One scalar computation: one thread.  out: the 12 Fq coefficients in snarkjs's nesting (c0.a, c0.b, c0.c, c1.a, c1.b,
+// c1.c, each Fq2 as c0, c1), canonical.
+__global__ void k_vk_alphabeta_12(const affine_t<Fq>* alpha, const affine_t<Fq2>* beta, Fq* out) {
+    const Fq12 e = final_exponentiation(miller_loop(*alpha, *beta));
+    Fq12 r = Fq12::one();
+    for (int bit = SNARKJS_M_BITS - 1; bit >= 0; --bit) {
+        r = Fq12::mul(r, r);
+        if ((SNARKJS_M[bit >> 6] >> (bit & 63)) & 1) r = Fq12::mul(r, e);
+    }
+    const Fq2* c[6] = {&r.c0.a, &r.c0.b, &r.c0.c, &r.c1.a, &r.c1.b, &r.c1.c};
+    for (int k = 0; k < 6; ++k) {
+        out[2 * k] = Fq::from_mont(c[k]->c0);
+        out[2 * k + 1] = Fq::from_mont(c[k]->c1);
+    }
+}
+
+int vk_alphabeta_12_dev(b200zk_ctx* ctx, Slot& sl, const uint64_t* alpha_g1, const uint64_t* beta_g2, uint64_t* out) {
+    cudaStream_t st = sl.stream;
+    // staging block: alpha 64 | beta 128 | out 384
+    B2_CUDA_OK(ctx, sl.io_b.reserve(576));
+    char* d = reinterpret_cast<char*>(sl.io_b.p);
+    B2_CUDA_OK(ctx, cudaMemcpyAsync(d, alpha_g1, 64, cudaMemcpyHostToDevice, st));
+    B2_CUDA_OK(ctx, cudaMemcpyAsync(d + 64, beta_g2, 128, cudaMemcpyHostToDevice, st));
+    {
+        LaunchScope ls(ctx, st, "vk_alphabeta_12");
+        k_vk_alphabeta_12<<<1, 1, 0, st>>>(reinterpret_cast<const affine_t<Fq>*>(d), reinterpret_cast<const affine_t<Fq2>*>(d + 64),
+                                            reinterpret_cast<Fq*>(d + 192));
+    }
+    B2_TRY(check_launch(ctx, "k_vk_alphabeta_12"));
+    B2_CUDA_OK(ctx, cudaMemcpyAsync(out, d + 192, 384, cudaMemcpyDeviceToHost, st));
+    B2_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    return B200ZK_OK;
+}
+
 }  // namespace b200zk

@@ -775,3 +775,148 @@ def coo_to_csr(rows: np.ndarray, cols: np.ndarray, vals: np.ndarray, n_rows: int
     row_ptr = np.zeros(n_rows + 1, dtype=np.uint32)
     row_ptr[1:] = np.cumsum(counts).astype(np.uint32)
     return row_ptr, np.ascontiguousarray(cols[order], dtype=np.uint32), np.ascontiguousarray(vals[order], dtype=np.uint64)
+
+
+# ---- snarkjs's Groth16 JSON files: proof.json, public.json, verification_key.json ------------------------------------------
+# Text only: points are coordinates as Python ints (G1 (x, y), G2 ((x.c0, x.c1), (y.c0, y.c1)), None = infinity); turning them
+# into device points is groth16/snarkjs.py's job.  The writer reproduces snarkjs's JSON.stringify(obj, null, 1) byte for byte
+# (one-space indent, one array item per line, no trailing newline); the reader takes decimal and 0x-hex strings, as
+# ffjavascript's unstringifyBigInts does.
+
+@dataclass
+class SnarkjsProof:
+    pi_a: tuple | None
+    pi_b: tuple | None
+    pi_c: tuple | None
+
+
+@dataclass
+class SnarkjsVerificationKey:
+    n_public: int
+    alpha_1: tuple | None
+    beta_2: tuple | None
+    gamma_2: tuple | None
+    delta_2: tuple | None
+    alphabeta_12: list          # 2 x 3 x 2 canonical Fq ints: [Fq6 c0, Fq6 c1], each [Fq2 a, b, c], each [c0, c1]
+    ic: list                    # n_public + 1 G1 points
+
+
+def _dumps(obj) -> str:
+    import json
+    return json.dumps(obj, indent=1)            # == JSON.stringify(obj, null, 1) for strings, ints, lists and dicts
+
+
+def _g1_json(p) -> list:
+    return ["0", "1", "0"] if p is None else [str(int(p[0])), str(int(p[1])), "1"]
+
+
+def _g2_json(p) -> list:
+    if p is None:
+        return [["0", "0"], ["1", "0"], ["0", "0"]]
+    return [[str(int(p[0][0])), str(int(p[0][1]))], [str(int(p[1][0])), str(int(p[1][1]))], ["1", "0"]]
+
+
+def write_proof_json(proof: SnarkjsProof) -> str:
+    return _dumps({"pi_a": _g1_json(proof.pi_a), "pi_b": _g2_json(proof.pi_b), "pi_c": _g1_json(proof.pi_c),
+                   "protocol": "groth16", "curve": "bn128"})
+
+
+def write_public_json(values) -> str:
+    return _dumps([str(int(v)) for v in values])
+
+
+def write_vk_json(vk: SnarkjsVerificationKey) -> str:
+    ab = [[[str(int(vk.alphabeta_12[h][k][j])) for j in range(2)] for k in range(3)] for h in range(2)]
+    return _dumps({"protocol": "groth16", "curve": "bn128", "nPublic": int(vk.n_public), "vk_alpha_1": _g1_json(vk.alpha_1),
+                   "vk_beta_2": _g2_json(vk.beta_2), "vk_gamma_2": _g2_json(vk.gamma_2), "vk_delta_2": _g2_json(vk.delta_2),
+                   "vk_alphabeta_12": ab, "IC": [_g1_json(p) for p in vk.ic]})
+
+
+def _json_load(text, what: str):
+    import json
+    try:
+        return json.loads(text)
+    except (ValueError, TypeError) as e:
+        raise FormatError("%s is not JSON: %s" % (what, e)) from None
+
+
+def _json_object(text, what: str, keys) -> dict:
+    obj = _json_load(text, what)
+    if not isinstance(obj, dict):
+        raise FormatError("%s: expected a JSON object" % what)
+    for k in keys:
+        if k not in obj:
+            raise FormatError("%s: missing key %r" % (what, k))
+    for k, want in (("protocol", "groth16"), ("curve", "bn128")):
+        if k in obj and obj[k] != want:
+            raise FormatError("%s: %s is %r, only %r is supported" % (what, k, obj[k], want))
+    return obj
+
+
+def _json_int(v, field: str, bound: int | None = None) -> int:
+    """A decimal or 0x-hex string -> int; bound: the value must be below it (FQ_MODULUS for coordinates)."""
+    import re
+    if not isinstance(v, str) or not (re.fullmatch(r"[0-9]+", v) or re.fullmatch(r"0x[0-9a-fA-F]+", v)):
+        raise FormatError("%s: %r is not a decimal or 0x-hex number string" % (field, v))
+    x = int(v, 0) if v.startswith("0x") else int(v)
+    if bound is not None and x >= bound:
+        raise FormatError("%s: %d is not below the base-field modulus q" % (field, x))
+    return x
+
+
+def _json_list(v, n: int, field: str) -> list:
+    if not isinstance(v, list) or len(v) != n:
+        raise FormatError("%s: expected a list of %d items" % (field, n))
+    return v
+
+
+def _json_g1(v, field: str):
+    x, y, z = (_json_int(c, "%s[%d]" % (field, i), FQ_MODULUS) for i, c in enumerate(_json_list(v, 3, field)))
+    if z == 0:
+        return None
+    if z != 1:
+        raise FormatError("%s: z = %d; only affine points (z = 1) and infinity (z = 0) are read" % (field, z))
+    return (x, y)
+
+
+def _json_fq2(v, field: str) -> tuple:
+    return tuple(_json_int(c, "%s[%d]" % (field, i), FQ_MODULUS) for i, c in enumerate(_json_list(v, 2, field)))
+
+
+def _json_g2(v, field: str):
+    x, y, z = (_json_fq2(c, "%s[%d]" % (field, i)) for i, c in enumerate(_json_list(v, 3, field)))
+    if z == (0, 0):
+        return None
+    if z != (1, 0):
+        raise FormatError("%s: z = %s; only affine points (z = [1, 0]) and infinity (z = [0, 0]) are read" % (field, z))
+    return (x, y)
+
+
+def read_proof_json(text) -> SnarkjsProof:
+    obj = _json_object(text, "proof.json", ("pi_a", "pi_b", "pi_c", "protocol", "curve"))
+    return SnarkjsProof(_json_g1(obj["pi_a"], "pi_a"), _json_g2(obj["pi_b"], "pi_b"), _json_g1(obj["pi_c"], "pi_c"))
+
+
+def read_public_json(text) -> list:
+    """-> the public signals as ints (not reduced: a value >= r is the verifier's to reject)."""
+    arr = _json_load(text, "public.json")
+    if not isinstance(arr, list):
+        raise FormatError("public.json: expected a JSON array")
+    return [_json_int(v, "public[%d]" % i) for i, v in enumerate(arr)]
+
+
+def read_vk_json(text) -> SnarkjsVerificationKey:
+    obj = _json_object(text, "verification_key.json", ("protocol", "curve", "nPublic", "vk_alpha_1", "vk_beta_2", "vk_gamma_2",
+                                                       "vk_delta_2", "vk_alphabeta_12", "IC"))
+    n = obj["nPublic"]
+    if isinstance(n, bool) or not isinstance(n, int) or n < 0:
+        raise FormatError("nPublic: %r is not a non-negative integer" % (n,))
+    ic = obj["IC"]
+    if not isinstance(ic, list) or len(ic) != n + 1:
+        raise FormatError("IC: %s points for nPublic = %d (expected %d)" % (len(ic) if isinstance(ic, list) else "no list of",
+                                                                           n, n + 1))
+    ab = [[_json_fq2(c, "vk_alphabeta_12[%d][%d]" % (h, k)) for k, c in enumerate(_json_list(half, 3, "vk_alphabeta_12[%d]" % h))]
+          for h, half in enumerate(_json_list(obj["vk_alphabeta_12"], 2, "vk_alphabeta_12"))]
+    return SnarkjsVerificationKey(n, _json_g1(obj["vk_alpha_1"], "vk_alpha_1"), _json_g2(obj["vk_beta_2"], "vk_beta_2"),
+                                  _json_g2(obj["vk_gamma_2"], "vk_gamma_2"), _json_g2(obj["vk_delta_2"], "vk_delta_2"), ab,
+                                  [_json_g1(p, "IC[%d]" % i) for i, p in enumerate(ic)])

@@ -216,3 +216,37 @@ def prove_zkey_wtns(net: Net, zkey_bytes: bytes, wtns_bytes: bytes, r=None, s=No
     proof = prove_from_matrices(pk, mats, z, r, s)
     pk.free()
     return proof, w[1:1 + zk.n_public].copy()
+
+
+def wtns_check(net: Net, r1cs_bytes: bytes, wtns_bytes: bytes):
+    """snarkjs `wtns check <r1cs> <wtns>`: does the witness satisfy the circuit?  -> snarkjs.WtnsCheckReport (ok, n_failed,
+    first_failed, one line per failure).  A witness whose length is not the circuit's wire count, whose w[0] is not 1 or
+    with an entry >= r fails with one line naming the index; otherwise every constraint <A_i,w> <B_i,w> = <C_i,w> is
+    evaluated on the device, and the line for the first failing one gives its three products."""
+    from . import snarkjs
+    return snarkjs.check_witness(net, formats.read_r1cs(r1cs_bytes), formats.read_wtns(wtns_bytes))
+
+
+def zkey_export_verificationkey(net: Net, zkey_bytes: bytes) -> str:
+    """snarkjs `zkey export verificationkey <zkey> <json>`: the text of verification_key.json, vk_alphabeta_12 computed on
+    the device."""
+    from . import snarkjs
+    return formats.write_vk_json(snarkjs.vk_from_zkey(net, formats.read_zkey(zkey_bytes)))
+
+
+def groth16_prove(net: Net, zkey_bytes: bytes, wtns_bytes: bytes, r=None, s=None):
+    """snarkjs `groth16 prove <zkey> <wtns> <proof.json> <public.json>`: prove_zkey_wtns (r, s as it takes them: 4 Montgomery
+    limbs each, None = 0), written as snarkjs writes it.  -> (text of proof.json, text of public.json)."""
+    from . import snarkjs
+    proof, public = prove_zkey_wtns(net, zkey_bytes, wtns_bytes, r, s)
+    return snarkjs.proof_to_json(net, proof), snarkjs.public_to_json(public)
+
+
+def groth16_verify(net: Net, vk_json, public_json, proof_json) -> bool:
+    """snarkjs `groth16 verify <verification_key.json> <public.json> <proof.json>` on the texts of the three files.
+    Raises formats.FormatError for a malformed file (not JSON, a missing key, protocol other than groth16 or curve other than
+    bn128, a non-numeric string, a coordinate >= q, a verification-key point that does not decode, len(IC) != nPublic + 1).
+    Returns False where snarkjs does: a public count other than nPublic, a signal >= r, a proof point off the curve or
+    outside the G2 subgroup, or a failing pairing check."""
+    from . import snarkjs
+    return snarkjs.verify_json(net, vk_json, public_json, proof_json)

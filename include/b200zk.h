@@ -164,6 +164,16 @@ int b200zk_qap_dev(b200zk_ctx* ctx, int stream, const void* d_a_row_ptr, const v
 /* Montgomery <-> canonical conversion applied `times` times (zkey coefficients are stored times R^2:
  * ark-circom/src/zkey.rs:333-338 -> to_mont = 0, times = 1; .wtns / .r1cs values: to_mont = 1, times = 1). */
 int b200zk_fr_convert_dev(b200zk_ctx* ctx, int stream, const void* d_in, void* d_out, size_t n, int to_mont, int times);
+/* R1CS satisfaction, the check of snarkjs `wtns check <r1cs> <wtns>`: constraint i fails when
+ * <A_i, w> <B_i, w> != <C_i, w> over Fr.  A, B and C in CSR form with the conventions of b200zk_qap_dev (row_ptr:
+ * n_constraints + 1 x u32, col: nnz x u32 wire index, val: nnz x 4 limbs Montgomery; col / val may be null for a matrix
+ * without terms); w: the full assignment (Montgomery), long enough for every column.  *n_failed = the number of failing
+ * constraints, *first_failed = the lowest failing index (n_constraints when none fails).  n_constraints = 0: OK with no
+ * failure; a null row_ptr, w or output with n_constraints > 0: B200ZK_ERR_ARG.  Returns once the counters are on the host. */
+int b200zk_r1cs_check_dev(b200zk_ctx* ctx, int stream, const void* d_a_row_ptr, const void* d_a_col, const void* d_a_val,
+                          const void* d_b_row_ptr, const void* d_b_col, const void* d_b_val, const void* d_c_row_ptr,
+                          const void* d_c_col, const void* d_c_val, size_t n_constraints, const void* d_w, uint64_t* n_failed,
+                          uint64_t* first_failed);
 
 /* ---- proving key (what PackedProvingKeyShare carries, groth16/src/proving_key.rs:19-25,48-65) -- */
 /* a_query, b_g1_query, b_g2_query: n_vars points; l_query: n_vars - n_inputs; h_query: m points.
@@ -200,6 +210,12 @@ int b200zk_groth16_verify(b200zk_ctx* ctx, const uint64_t* alpha_g1, const uint6
                           const uint64_t* delta_g2, const uint64_t* gamma_abc_g1, size_t n_public,
                           const uint64_t* public_inputs, const uint64_t* proof_a, const uint64_t* proof_b,
                           const uint64_t* proof_c, int* is_valid);
+/* vk_alphabeta_12 of the verification key snarkjs `zkey export verificationkey` writes: e(alpha_g1, beta_g2) as snarkjs
+ * computes it, i.e. the pairing of b200zk_groth16_verify raised to ffjavascript's hard-part multiple m = 2u(6u^2 + 3u + 1).
+ * Host buffers: alpha_g1 8, beta_g2 16 Montgomery u64 limbs (infinity all-zero); out: 12 canonical Fq elements (4 u64 limbs
+ * each) in snarkjs's nesting [[c0.a, c0.b, c0.c], [c1.a, c1.b, c1.c]] of Fq2 pairs (c0, c1), over the tower
+ * Fq12 = Fq6[w]/(w^2 - v), Fq6 = Fq2[v]/(v^3 - (9 + u)). */
+int b200zk_vk_alphabeta_12(b200zk_ctx* ctx, const uint64_t alpha_g1[8], const uint64_t beta_g2[16], uint64_t out[48]);
 
 /* ---- ark-serialize Compress::Yes point codec (common/src/utils/serializer.rs:20-49: every proving / verifying key and
  * proof of the reference travels in this form; zk-cli/src/main.rs:130-136) --------------------------------------------
