@@ -102,6 +102,7 @@ SIGNATURES = {
     "b200zk_points_spmv_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, c_vp, c_vp, c_vp, ctypes.c_size_t, c_vp]),
     "b200zk_points_scale_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, ctypes.c_size_t, c_vp, c_vp]),
     "b200zk_points_intt_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, ctypes.c_uint, c_vp]),
+    "b200zk_points_ntt_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, ctypes.c_uint, c_vp]),
     "b200zk_points_mul_powers_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, ctypes.c_size_t, c_vp, c_vp, c_vp]),
     "b200zk_points_sub_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, c_vp, ctypes.c_size_t, c_vp]),
     "b200zk_points_encode_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, ctypes.c_size_t, ctypes.c_int, c_vp]),

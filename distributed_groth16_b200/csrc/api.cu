@@ -713,6 +713,15 @@ int b200zk_points_intt_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_in
     B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
     return points_intt_dev(ctx, sl, g2, d_in, log_n, d_out);
 }
+int b200zk_points_ntt_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_in, unsigned log_n, void* d_out) {
+    if (!ctx) return B200ZK_ERR_ARG;
+    if (!valid_slot(stream) || !d_in || !d_out) return set_error(ctx, B200ZK_ERR_ARG, "points_ntt: null pointer or bad stream slot");
+    if (log_n > 28) return set_error(ctx, B200ZK_ERR_DOMAIN, "points_ntt: log_n > 28 (the two-adicity of Fr)");
+    Slot& sl = ctx->slots[stream];
+    std::lock_guard<std::mutex> g(sl.mu);
+    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    return points_ntt_dev(ctx, sl, g2, d_in, log_n, d_out);
+}
 int b200zk_points_mul_powers_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_points, size_t n, const uint64_t first[4],
                                  const uint64_t ratio[4], void* d_out) {
     if (!ctx) return B200ZK_ERR_ARG;

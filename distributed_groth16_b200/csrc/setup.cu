@@ -468,12 +468,14 @@ int points_scale_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_points, si
     return check_launch(ctx, "k_points_scale_g1");
 }
 
-// ---- inverse NTT over points: out[i] = n^-1 sum_j w_n^(-i j) in[j]  (snarkjs `powersoftau prepare phase2`) ----------
-// The Lagrange levels of a prepared Powers-of-Tau file; orchestration in groth16/ptau.py.  Radix-2 decimation in time:
-// one bit-reversal pass, then log_n in-place butterfly passes over global memory, then n^-1 by points_scale_dev.  Each
+// ---- NTT over points: out[i] = sum_j w_n^(i j) in[j], and the inverse n^-1 sum_j w_n^(-i j) in[j] -----------------------
+// The inverse makes the Lagrange levels of a prepared Powers-of-Tau file (snarkjs `powersoftau prepare phase2`,
+// orchestration in groth16/ptau.py); the forward one moves a zkey's H query into the tau basis of a bellman MPC-params
+// file (snarkjs `zkey export bellman`, groth16/bellman.py).  Radix-2 decimation in time: one bit-reversal pass, then
+// log_n in-place butterfly passes over global memory, then, for the inverse only, n^-1 by points_scale_dev.  Each
 // butterfly costs one full scalar multiplication (w^-j P) against a handful of point additions, so the passes are plain
 // and the work per thread is made uniform instead:
-//   * the twiddles w_n^-i, i < n / 2, are computed once per transform on the device, split with GLV (glv.cuh; on G2
+//   * the twiddles w_n^-+i, i < n / 2, are computed once per transform on the device, split with GLV (glv.cuh; on G2
 //     phi = (beta^2 x, y), right for points of the order-r subgroup) and recoded into 32 signed 4-bit windows per half,
 //     digits in [-7, 8] (|k1|, |k2| < 2^127 leave no carry out of the top window).  Every thread runs the same
 //     32 x (4 doublings + 2 mixed additions) from a per-thread table P, 2P, .., 8P in shared memory (normalised with
@@ -513,11 +515,11 @@ __device__ __forceinline__ TwiddleDigits glv_window_digits(const Fr& k) {
     return dg;
 }
 
-// digits of w_n^-i for i < count
-__global__ void k_intt_twiddle_digits(unsigned log_n, size_t count, TwiddleDigits* out) {
+// digits of w_n^-i (inverse) or w_n^i for i < count
+__global__ void k_intt_twiddle_digits(unsigned log_n, bool inverse, size_t count, TwiddleDigits* out) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;
-    st16(out + i, glv_window_digits(Fr::from_mont(Fr::pow_u64(fr_root_of_unity(log_n, true), i))));
+    st16(out + i, glv_window_digits(Fr::from_mont(Fr::pow_u64(fr_root_of_unity(log_n, inverse), i))));
 }
 
 // out[i] = in[bitrev(i)]; each pair is handled by one thread that reads both before writing, so out may equal in
@@ -551,7 +553,7 @@ __device__ __forceinline__ void build_mul_table(uint4* tab, const affine_t<F>& P
 }
 
 // pass with half-size m = 2^log_m: butterfly t = (j, g), j = t >> lg, g = t mod 2^lg (lg = log2(n / 2m)), on the
-// elements g 2m + j and g 2m + j + m with twiddle w_2m^-j = w_n^-(j << lg)
+// elements g 2m + j and g 2m + j + m with twiddle w_2m^-+j = w_n^-+(j << lg) (the sign is the transform's direction)
 template <class F, int B>
 __global__ void __launch_bounds__(B) k_points_intt_pass(affine_t<F>* a, const TwiddleDigits* __restrict__ tw, unsigned log_n,
                                                         unsigned log_m) {
@@ -612,7 +614,9 @@ __global__ void __launch_bounds__(B) k_points_intt_pass(affine_t<F>* a, const Tw
 }
 
 template <class F, int B>
-static int points_intt_impl(b200zk_ctx* ctx, Slot& sl, int g2, const affine_t<F>* d_in, unsigned log_n, affine_t<F>* d_out) {
+static int points_intt_impl(b200zk_ctx* ctx, Slot& sl, int g2, bool inverse, const affine_t<F>* d_in, unsigned log_n,
+                            affine_t<F>* d_out) {
+    const char* what = inverse ? "points_intt" : "points_ntt";
     cudaStream_t st = sl.stream;
     const size_t n = (size_t)1 << log_n, half = n >> 1;
     TwiddleDigits* tw = nullptr;
@@ -621,8 +625,8 @@ static int points_intt_impl(b200zk_ctx* ctx, Slot& sl, int g2, const affine_t<F>
         if (e != cudaSuccess) {
             cudaGetLastError();                                           // nothing was launched: leave no error behind
             char b[256];
-            snprintf(b, sizeof(b), "points_intt: the twiddle digits of 2^%u points (%zu MB of device memory) do not fit: %s",
-                     log_n, half * sizeof(TwiddleDigits) >> 20, cudaGetErrorString(e));
+            snprintf(b, sizeof(b), "%s: the twiddle digits of 2^%u points (%zu MB of device memory) do not fit: %s",
+                     what, log_n, half * sizeof(TwiddleDigits) >> 20, cudaGetErrorString(e));
             return set_error(ctx, e == cudaErrorMemoryAllocation ? B200ZK_ERR_OOM : B200ZK_ERR_CUDA, b);
         }
     }
@@ -635,7 +639,7 @@ static int points_intt_impl(b200zk_ctx* ctx, Slot& sl, int g2, const affine_t<F>
         if (!half) return B200ZK_OK;
         {
             LaunchScope ls(ctx, st, "points_intt_twiddles");
-            k_intt_twiddle_digits<<<(unsigned)((half + 255) / 256), 256, 0, st>>>(log_n, half, tw);
+            k_intt_twiddle_digits<<<(unsigned)((half + 255) / 256), 256, 0, st>>>(log_n, inverse, half, tw);
         }
         B2_TRY(check_launch(ctx, "k_intt_twiddle_digits"));
         for (unsigned log_m = 0; log_m < log_n; ++log_m) {
@@ -645,6 +649,7 @@ static int points_intt_impl(b200zk_ctx* ctx, Slot& sl, int g2, const affine_t<F>
             }
             B2_TRY(check_launch(ctx, "k_points_intt_pass"));
         }
+        if (!inverse) return B200ZK_OK;
         // n^-1 mod r = r - (r - 1) / n  (n divides r - 1)
         uint32_t q[8], ninv32[8];
         for (int i = 0; i < 8; ++i) q[i] = FrParams::mod(i) & (i ? ~0u : ~1u);
@@ -670,9 +675,19 @@ static int points_intt_impl(b200zk_ctx* ctx, Slot& sl, int g2, const affine_t<F>
     return B200ZK_OK;
 }
 
+static int points_transform(b200zk_ctx* ctx, Slot& sl, int g2, bool inverse, const void* d_in, unsigned log_n, void* d_out) {
+    return g2 ? points_intt_impl<Fq2, INTT_BLOCK_G2>(ctx, sl, 1, inverse, (const affine_t<Fq2>*)d_in, log_n,
+                                                     (affine_t<Fq2>*)d_out)
+              : points_intt_impl<Fq, INTT_BLOCK_G1>(ctx, sl, 0, inverse, (const affine_t<Fq>*)d_in, log_n,
+                                                    (affine_t<Fq>*)d_out);
+}
+
 int points_intt_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_in, unsigned log_n, void* d_out) {
-    return g2 ? points_intt_impl<Fq2, INTT_BLOCK_G2>(ctx, sl, 1, (const affine_t<Fq2>*)d_in, log_n, (affine_t<Fq2>*)d_out)
-              : points_intt_impl<Fq, INTT_BLOCK_G1>(ctx, sl, 0, (const affine_t<Fq>*)d_in, log_n, (affine_t<Fq>*)d_out);
+    return points_transform(ctx, sl, g2, true, d_in, log_n, d_out);
+}
+
+int points_ntt_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_in, unsigned log_n, void* d_out) {
+    return points_transform(ctx, sl, g2, false, d_in, log_n, d_out);
 }
 
 // ---- each point times its own term of a geometric sequence: out[i] = (first ratio^i) points[i]  (snarkjs `powersoftau

@@ -700,6 +700,90 @@ def mpc_params_bytes(params: MPCParams) -> bytes:
     return b"".join(out)
 
 
+# ---- bellman MPC params (snarkjs `zkey export bellman` / `zkey bellman contribute` / `zkey import bellman`) -------------
+BELLMAN_HEADER = (("alpha_g1", 64), ("beta_g1", 64), ("beta_g2", 128), ("gamma_g2", 128), ("delta_g1", 64), ("delta_g2", 128))
+BELLMAN_VECTORS = (("ic", 64), ("h", 64), ("l", 64), ("a", 64), ("b1", 64), ("b2", 128))
+BELLMAN_RECORD = 384                              # U(deltaAfter) U(g1_s) U(g1_sx) U(g2_spx) transcript
+
+
+@dataclass
+class Bellman:
+    """A parsed bellman MPC-params file.  spans[part] = (byte offset, byte length) for every part of BELLMAN_HEADER and
+    BELLMAN_VECTORS (a vector's span excludes its count); counts[part] for the vectors; params_end = the offset of the
+    csHash, so buf[:params_end] is what the circuit hash covers; records_offset = the offset of the first record."""
+    counts: dict
+    spans: dict
+    params_end: int
+    cs_hash: bytes
+    records_offset: int
+    contributions: list
+
+
+def bellman_size(n_ic: int, n_h: int, n_l: int, n_vars: int, n_records: int = 0) -> int:
+    """The byte size of a bellman MPC-params file: the 576-byte header points, six u32-counted vectors (IC, H, L, A, B1 of
+    G1 points, B2 of G2 points, each of n_vars entries for A, B1 and B2), the csHash, a u32 record count and the records."""
+    return 576 + 6 * 4 + 64 * (n_ic + n_h + n_l + 2 * n_vars) + 128 * n_vars + 64 + 4 + BELLMAN_RECORD * n_records
+
+
+def _u_to_limbs(b: bytes, g2: bool, what: str) -> np.ndarray:
+    """ffjavascript toRprUncompressed -> Montgomery limbs on the host (for the handful of record points).  Infinity is
+    0x40 then zeros; otherwise the top two bits of byte 0 are clear and every coordinate is below q.  No curve check."""
+    if b[0] & 0xC0:
+        if b[0] != 0x40 or any(b[1:]):
+            raise FormatError("%s: not an uncompressed point encoding (flag byte 0x%02x)" % (what, b[0]))
+        return np.zeros(16 if g2 else 8, dtype=np.uint64)
+    coords = [int.from_bytes(b[32 * k:32 * k + 32], "big") for k in range(len(b) // 32)]
+    if any(v >= FQ_MODULUS for v in coords):
+        raise FormatError("%s: a coordinate is not below q" % what)
+    if g2:
+        coords = [coords[k] for k in (1, 0, 3, 2)]          # x.c1 x.c0 y.c1 y.c0 -> x.c0 x.c1 y.c0 y.c1
+    mont = [(v << 256) % FQ_MODULUS for v in coords]
+    return np.array([(v >> (64 * i)) & 0xFFFFFFFFFFFFFFFF for v in mont for i in range(4)], dtype=np.uint64)
+
+
+def parse_bellman(buf: bytes) -> Bellman:
+    """A bellman MPC-params file (as snarkjs `zkey export bellman` writes it) -> Bellman.  Byte shuffling only: points stay
+    encoded except the records', which become formats.Contribution (type 0, no name; bellman carries neither).  Raises
+    FormatError for a truncated file, a count that disagrees with the file's length and trailing bytes."""
+    buf = bytes(buf)
+
+    def need(off, n, what):
+        if off + n > len(buf):
+            raise FormatError("bellman params end inside %s (%d + %d > %d bytes)" % (what, off, n, len(buf)))
+
+    spans, counts, off = {}, {}, 0
+    for part, w in BELLMAN_HEADER:
+        need(off, w, part)
+        spans[part] = (off, w)
+        off += w
+    for part, w in BELLMAN_VECTORS:
+        need(off, 4, "the count of %s" % part)
+        cnt = struct.unpack_from(">I", buf, off)[0]
+        off += 4
+        if off + cnt * w > len(buf):
+            raise FormatError("bellman params: %s claims %d points, more than the %d bytes left hold" % (part, cnt, len(buf) - off))
+        counts[part], spans[part] = cnt, (off, cnt * w)
+        off += cnt * w
+    if not counts["a"] == counts["b1"] == counts["b2"]:
+        raise FormatError("bellman params: A, B1 and B2 have %d, %d and %d points (one per variable each)"
+                          % (counts["a"], counts["b1"], counts["b2"]))
+    params_end = off
+    need(off, 68, "the csHash and record count")
+    cs_hash, k = buf[off:off + 64], struct.unpack_from(">I", buf, off + 64)[0]
+    rec = off + 68
+    if len(buf) != rec + BELLMAN_RECORD * k:
+        raise FormatError("bellman params of %d bytes; its counts give %d (%d records)"
+                          % (len(buf), bellman_size(counts["ic"], counts["h"], counts["l"], counts["a"], k), k))
+    out = []
+    for i in range(k):
+        o = rec + BELLMAN_RECORD * i
+        pt = lambda j, w, g2, nm: _u_to_limbs(buf[o + j:o + j + w], g2, "record %d %s" % (i, nm))
+        out.append(Contribution(delta_after=pt(0, 64, False, "deltaAfter"), g1_s=pt(64, 64, False, "g1_s"),
+                                g1_sx=pt(128, 64, False, "g1_sx"), g2_spx=pt(192, 128, True, "g2_spx"),
+                                transcript=buf[o + 320:o + 384]))
+    return Bellman(counts=counts, spans=spans, params_end=params_end, cs_hash=cs_hash, records_offset=rec, contributions=out)
+
+
 def read_wtns(buf: bytes) -> np.ndarray:
     """(n, 4) u64 canonical (non-Montgomery) witness values."""
     secs = _sections(buf, b"wtns")

@@ -164,6 +164,30 @@ def zkey_verify(net: Net, r1cs_bytes: bytes, ptau_path: str, zkey_bytes: bytes, 
     return phase2.verify(net, r1cs_bytes, ptau_path, zkey_bytes, check_cs_hash=check_cs_hash)
 
 
+def zkey_export_bellman(net: Net, zkey_bytes: bytes) -> bytes:
+    """snarkjs `zkey export bellman <zkey> <params>`: the bellman MPC-params bytes a coordinated phase-2 ceremony sends to
+    its contributors, with the H query moved to the tau basis on the device (bellman.export).  Domains up to 2^27."""
+    from . import bellman
+    return bellman.export(net, zkey_bytes)
+
+
+def zkey_bellman_contribute(net: Net, challenge_bytes: bytes, entropy: bytes = b""):
+    """snarkjs `zkey bellman contribute bn128 <challenge> <response>` on the GPU, with a fresh secret x and base g1_s as in
+    zkey_contribute; the secrets are dropped on return.  Returns (response bytes, contribution hash)."""
+    from . import bellman, phase2
+    x, s = _random_scalar(entropy), _random_scalar(entropy)
+    g1_s = phase2._scale_one(net, np.concatenate([_fq_mont_limbs(1), _fq_mont_limbs(2)]), s)
+    return bellman.contribute(net, challenge_bytes, x, g1_s)
+
+
+def zkey_import_bellman(net: Net, zkey_bytes: bytes, response_bytes: bytes, name: str | None = None) -> bytes:
+    """snarkjs `zkey import bellman <zkey> <response> <dst>`: the key with the response's contributions applied, the new
+    records named `name` (bellman.import_response).  It checks that the response answers this key but runs no pairing
+    check: run zkey_verify on the result."""
+    from . import bellman
+    return bellman.import_response(net, zkey_bytes, response_bytes, name=name)
+
+
 def zkey_from_r1cs(net: Net, r1: formats.R1CS, pt: formats.PTau, cs_hash: bool = False) -> bytes:
     """zkey_new on a parsed r1cs and an open ceremony file."""
     import struct

@@ -11,7 +11,8 @@ of a proof into its private part, so the reference's scripts/phase2_proving_key.
 
 Verification rebuilds the initial key from the r1cs and the Powers-of-Tau file, checks every record with same-ratio
 pairings (b200zk_groth16_verify with one pairing pair per side) and the L / H sections with random linear combinations
-(the G1 MSM).
+(the G1 MSM); H is checked in the tau basis, so that a key imported from a bellman MPC-params file (groth16/bellman.py),
+which has infinity in the one tau component the prover never uses, verifies too (_check_h).
 
 Hashing and transcript (restated from snarkjs zkey_utils / misc and ffjavascript; this module is the one place that holds
 them):
@@ -480,9 +481,37 @@ def verify(net, r1cs_bytes: bytes, ptau_path: str, zkey_bytes: bytes, check_cs_h
             continue
         if not a:
             continue
+        if sid == 9:
+            _check_h(net, a, b, g2, d2, fail)
+            continue
         rho = _random_scalars(net, len(a) // 64)
         # e(sum rho P, delta_2) == e(sum rho P_init, G2): every point is the initial one times delta^-1
         if not _same_ratio(net, _rlc(net, b, rho), _rlc(net, a, rho), g2, d2):
             fail("the %s section is not the initial one times delta^-1" % what)
     rep.ok = not rep.failures
     return rep
+
+
+def _check_h(net, init_h: bytes, cur_h: bytes, g2, d2, fail) -> None:
+    """The H section (h_k = L^2n_(2k+1)(tau) delta^-1 G1, k < n) checked in the tau basis, H_i = tau^i (tau^n - 1) delta^-1
+    G1 = -2 w_2n^i sum_k w_n^(i k) h_k.  The prover only uses H_0 .. H_(n-2) (h(X) has degree <= n - 2), and a key that
+    went through a bellman round (groth16/bellman.py) has H_(n-1) = infinity: the MPC-params file does not carry it.  So
+    sum_(i < n-1) rho_i H_i = MSM(h, s) with s = NTT(rho_i (-2) w_2n^i), rho_(n-1) = 0, must be the initial one times
+    delta^-1, and H_(n-1) = MSM(h, t), t = NTT of the same transform of the last unit vector, must be infinity or the
+    initial one times delta^-1."""
+    import torch
+    from .setup import _powers
+    n = len(init_h) // 64
+    w2n = pow(5, (R - 1) // (2 * n), R)
+    rho = _random_scalars(net, n)
+    rho[n - 1] = 0
+    c = _powers(net, w2n, R - 2, n)                                       # -2 w_2n^i
+    net.check(net._lib.b200zk_fr_mul_sub_dev(net._h, 0, c_vp(rho.data_ptr()), c_vp(c.data_ptr()),
+                                             c_vp(torch.zeros_like(c).data_ptr()), c_vp(c.data_ptr()), n))
+    s = net.ntt_dev(c)
+    if not _same_ratio(net, _rlc(net, cur_h, s), _rlc(net, init_h, s), g2, d2):
+        fail("the H section is not the initial one times delta^-1 in its first n - 1 tau components")
+    t = _powers(net, pow(w2n, 2 * (n - 1), R), (R - 2) * pow(w2n, n - 1, R) % R, n)   # NTT(-2 w_2n^(n-1) e_(n-1))
+    x_cur, x_init = _rlc(net, cur_h, t), _rlc(net, init_h, t)
+    if x_cur.any() and not _same_ratio(net, x_cur, x_init, g2, d2):
+        fail("the last tau component of the H section is neither infinity nor the initial one times delta^-1")

@@ -40,6 +40,21 @@ def points_intt(net, points, g2: bool = False, out=None):
     return out
 
 
+def points_ntt(net, points, g2: bool = False, out=None):
+    """out[i] = sum_j w_n^(i j) points[j] on the device (b200zk_points_ntt_dev), the unscaled forward transform of
+    points_intt; points: CUDA int64 (2^k, 8 | 16) affine Montgomery limbs.  out may be points."""
+    import torch
+    points = points.contiguous()
+    n = int(points.shape[0])
+    log_n = n.bit_length() - 1
+    if n == 0 or (1 << log_n) != n:
+        raise ValueError("points_ntt: the number of points must be a power of two, got %d" % n)
+    if out is None:
+        out = torch.empty_like(points)
+    net.check(net._lib.b200zk_points_ntt_dev(net._h, 0, int(g2), c_vp(points.data_ptr()), log_n, c_vp(out.data_ptr())))
+    return out
+
+
 def _tau_level(pt: formats.PTau, sid: int, level: int) -> np.ndarray:
     """The first 2^level points of the tau section behind Lagrange section sid, infinity (all-zero) past its end."""
     src, g2, _ = _SECTIONS[sid]

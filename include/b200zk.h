@@ -282,6 +282,11 @@ int b200zk_points_scale_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_p
  * Temporary device memory: 2^(log_n - 1) x 64 bytes, allocated before anything is launched (B200ZK_ERR_OOM with a message
  * when it does not fit).  log_n > 28: B200ZK_ERR_DOMAIN; a null pointer: B200ZK_ERR_ARG.  Returns once out is complete. */
 int b200zk_points_intt_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_in, unsigned log_n, void* d_out);
+/* out[i] = sum_j omega_n^(i j) * in[j],  n = 2^log_n, unscaled: the forward transform of b200zk_points_intt_dev, the step
+ * of a snarkjs `zkey export bellman` that moves the H query from the zkey's Lagrange form to the tau basis of the MPC
+ * params.  points_ntt(k_j G) == fixed_base_mul(ntt(k)) point for point, and points_intt(points_ntt(P)) == P.  Points,
+ * order, subgroup, aliasing, temporary memory and error codes as b200zk_points_intt_dev.  Returns once out is complete. */
+int b200zk_points_ntt_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_in, unsigned log_n, void* d_out);
 /* out[i] = (first * ratio^i) * points[i], i < n: the step of a snarkjs `powersoftau contribute` that multiplies every point
  * of a ceremony section by its own power of the secret (ffjavascript G.batchApplyKey).  first, ratio: 4 u64 limbs, plain
  * little-endian integers (reduced mod r by the call, like b200zk_points_scale_dev's k), host.  Affine Montgomery points
