@@ -11,6 +11,7 @@
 //       (ark-ec VariableBaseMSM::msm_bigint_wnaf: window c = ln(n)+2 (3 if n<32), signed digits,
 //        windows processed in parallel [rayon <-> OpenMP], running-sum bucket reduction)
 //   * dom.fft / dom.ifft          dist-primitives/src/dfft/mod.rs:17-95   -> orc_ntt
+//   * qap mat-vec                 groth16/src/qap.rs:60-67                -> orc_fr_spmv
 //   * CircomReduction h           ark-circom/src/circom/qap.rs:64-89      -> orc_h_circom
 //   * prove::{A,B,C} + assembly   groth16/src/prove.rs:21-136,
 //                                 groth16/examples/sha256.rs:208-212      -> orc_groth16_prove
@@ -652,6 +653,22 @@ int orc_ntt(u64* data, unsigned log_n, int inverse, int coset, int nthreads) {
 }
 
 void orc_bitrev(u64* data, unsigned log_n) { ensure_init(); bitrev_permute(reinterpret_cast<Fr*>(data), log_n); }
+
+// CSR mat-vec over Fr: out[r] = sum_k val[k] * x[idx[k]], k in [ptr[r], ptr[r+1]) -- the per-row evaluation of qap.rs:60-67
+// (`evaluate_constraint`), with the conventions of b200zk.h (u32 row pointers and column indices, Montgomery values).
+void orc_fr_spmv(const uint32_t* ptr, const uint32_t* idx, const u64* val, const u64* x, size_t n_rows, u64* out,
+                 int nthreads) {
+    ensure_init();
+    const Fr* v = reinterpret_cast<const Fr*>(val);
+    const Fr* xs = reinterpret_cast<const Fr*>(x);
+    Fr* o = reinterpret_cast<Fr*>(out);
+#pragma omp parallel for num_threads(resolve_threads(nthreads)) schedule(dynamic, 4096)
+    for (long long r = 0; r < (long long)n_rows; ++r) {
+        Fr acc = Fr::zero();
+        for (uint32_t k = ptr[r]; k < ptr[r + 1]; ++k) acc = acc + v[k] * xs[idx[k]];
+        o[r] = acc;
+    }
+}
 
 int orc_h_circom(const u64* a, const u64* b, const u64* c, unsigned log_m, u64* h_out, int nthreads) {
     ensure_init();

@@ -142,6 +142,39 @@ def bitrev(data) -> np.ndarray:
     return out
 
 
+def fr_spmv(ptr, idx, val, x, nthreads: int = 0) -> np.ndarray:
+    """CSR mat-vec over Fr: out[r] = sum_k val[k] x[idx[k]], k in [ptr[r], ptr[r+1]).  ptr (n_rows + 1,) and idx (nnz,)
+    u32, val (nnz, 4) and x (n, 4) Montgomery limbs; -> (n_rows, 4)."""
+    ptr = np.ascontiguousarray(ptr, dtype=np.uint32).reshape(-1)
+    idx = np.ascontiguousarray(idx, dtype=np.uint32).reshape(-1)
+    val = np.ascontiguousarray(val, dtype=np.uint64).reshape(-1, 4)
+    x = np.ascontiguousarray(x, dtype=np.uint64).reshape(-1, 4)
+    n_rows = ptr.shape[0] - 1
+    nnz = int(ptr[-1])
+    assert n_rows >= 0 and (np.diff(ptr.astype(np.int64)) >= 0).all() and idx.shape[0] >= nnz and val.shape[0] >= nnz
+    assert nnz == 0 or int(idx[:nnz].max()) < x.shape[0]
+    out = np.zeros((n_rows, 4), dtype=np.uint64)
+    u32p = ctypes.POINTER(ctypes.c_uint32)
+    lib().orc_fr_spmv(ptr.ctypes.data_as(u32p), idx.ctypes.data_as(u32p), _p(val), _p(x), ctypes.c_size_t(n_rows), _p(out),
+                      int(nthreads))
+    return out
+
+
+def qap(a_csr, b_csr, z, nc: int, n_inputs: int, m: int, nthreads: int = 0):
+    """qap::qap (groth16/src/qap.rs:44-91) on CSR matrices: a_i = <A_i, z>, b_i = <B_i, z> for i < nc, a[nc + j] = z[j] for
+    j < n_inputs, c = a * b, zero up to m.  a_csr / b_csr: (ptr, idx, val) as fr_spmv takes them, nc + 1 row pointers each;
+    z: (n_vars, 4) Montgomery limbs.  -> a, b, c as (m, 4) Montgomery limbs."""
+    assert nc + n_inputs <= m
+    z = np.ascontiguousarray(z, dtype=np.uint64).reshape(-1, 4)
+    a, b, c = (np.zeros((m, 4), dtype=np.uint64) for _ in range(3))
+    a[:nc] = fr_spmv(*a_csr, z, nthreads=nthreads)
+    b[:nc] = fr_spmv(*b_csr, z, nthreads=nthreads)
+    a[nc:nc + n_inputs] = z[:n_inputs]
+    diag = np.arange(nc + 1, dtype=np.uint32)                # c_i = a_i b_i: the diagonal matrix of a times b
+    c[:nc] = fr_spmv(diag, diag[:nc], a[:nc], b, nthreads=nthreads)
+    return a, b, c
+
+
 def h_circom(a, b, c, nthreads: int = 0) -> np.ndarray:
     a, b, c = (np.ascontiguousarray(x, dtype=np.uint64) for x in (a, b, c))
     m = a.shape[0]
