@@ -489,6 +489,18 @@ int h_circom_dev(b200zk_ctx* ctx, Slot& sl, const Fr* d_a, const Fr* d_b, const 
 int ntt_batched_post_dev(b200zk_ctx* ctx, Slot& sl, const Fr* d_in, Fr* d_out, unsigned log_t, unsigned batch, bool inverse,
                          unsigned log_base, bool base_is_shift, uint64_t b0, uint64_t alpha, uint64_t beta, uint64_t gamma) {
     if (log_t > 28 || log_base > 28 || log_t == 0) return set_error(ctx, B200ZK_ERR_DOMAIN, "bad transform size for batched NTT");
+    if (base_is_shift && log_base == 0) return set_error(ctx, B200ZK_ERR_DOMAIN, "the shift table needs log_base >= 1");
+    // the post table holds base^e for e < 2^log_base (shift: e < 2^(log_base - 1)); exponents are not reduced, so the largest
+    // one, (batch - 1 + b0)(alpha k_max + beta) + gamma k_max with k_max = 2^log_t - 1, must lie below that bound
+    {
+        typedef unsigned __int128 u128;
+        const u128 bound = (u128)1 << (base_is_shift ? log_base - 1 : log_base);
+        const u128 k_max = ((u128)1 << log_t) - 1;
+        const u128 per_b = (u128)alpha * k_max + beta, b_max = (u128)(batch - 1) + b0;
+        if ((b_max && per_b >= bound) || b_max * per_b + (u128)gamma * k_max >= bound)     // no overflow: per_b < 2^28 or b_max = 0
+            return set_error(ctx, B200ZK_ERR_ARG, "post-factor exponent (batch - 1 + b0)(alpha k + beta) + gamma k exceeds the table of "
+                                                  "base powers");
+    }
     NttPlan *pl, *base_plan;
     B2_TRY(get_plan(ctx, sl.stream, log_t, inverse, &pl));
     const PowTab* tab = nullptr;
@@ -509,6 +521,7 @@ int ntt_batched_post_dev(b200zk_ctx* ctx, Slot& sl, const Fr* d_in, Fr* d_out, u
 
 int fourstep_cols_dev(b200zk_ctx* ctx, Slot& sl, const Fr* d_in, Fr* d_out, unsigned log_rows, unsigned log_cols_local,
                       unsigned log_n, uint64_t global_col0, bool inverse) {
+    if (log_cols_local > 28) return set_error(ctx, B200ZK_ERR_DOMAIN, "bad four-step geometry");
     return ntt_batched_post_dev(ctx, sl, d_in, d_out, log_rows, 1u << log_cols_local, inverse, log_n, false, global_col0, 1, 0, 0);
 }
 
@@ -520,6 +533,11 @@ int fourstep_cols_p2p_dev(b200zk_ctx* ctx, Slot& sl, const Fr* d_in, void* const
     if (log_rows == 0 || log_rows > 28 || log_n > 28) return set_error(ctx, B200ZK_ERR_DOMAIN, "bad four-step geometry");
     unsigned log_p = ceil_log2(n_peers);
     if (log_rows < log_p) return set_error(ctx, B200ZK_ERR_ARG, "fewer rows than peers");
+    if (log_n < log_rows) return set_error(ctx, B200ZK_ERR_ARG, "log_n < log_rows: the transform has fewer elements than one column");
+    // the remote stores write columns [global_col0, global_col0 + 2^log_cols_local) of rows 2^(log_n - log_rows) wide
+    const uint64_t cols_total = (uint64_t)1 << (log_n - log_rows);
+    if (log_cols_local > log_n - log_rows || global_col0 > cols_total - ((uint64_t)1 << log_cols_local))
+        return set_error(ctx, B200ZK_ERR_ARG, "columns [global_col0, global_col0 + 2^log_cols_local) run past the receive rows");
     NttPlan *pl, *base_plan;
     B2_TRY(get_plan(ctx, sl.stream, log_rows, inverse, &pl));
     B2_TRY(get_plan(ctx, sl.stream, log_n, inverse, &base_plan));

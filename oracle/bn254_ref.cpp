@@ -654,6 +654,31 @@ int orc_ntt(u64* data, unsigned log_n, int inverse, int coset, int nthreads) {
 
 void orc_bitrev(u64* data, unsigned log_n) { ensure_init(); bitrev_permute(reinterpret_cast<Fr*>(data), log_n); }
 
+// `batch` contiguous transforms of 2^log_t elements (in place), then output k of transform b times base^e with
+// e = (b + b0)(alpha k + beta) + gamma k and base = w_{2^log_base}, inverted for an inverse transform unless `shift`: the
+// semantics of b200zk_ntt_fr_batched_post_dev.  e is reduced modulo the order of base, so any e gives the exact value.
+int orc_ntt_batched_post(u64* data, unsigned log_t, size_t batch, int inverse, unsigned log_base, int shift, u64 b0, u64 alpha,
+                         u64 beta, u64 gamma, int nthreads) {
+    ensure_init();
+    if (log_t > 28 || log_base > 28) return 2;
+    nthreads = resolve_threads(nthreads);
+    const size_t t = (size_t)1 << log_t;
+    Fr* a = reinterpret_cast<Fr*>(data);
+    Fr base = fr_root_of_unity(log_base);
+    if (inverse && !shift) base = base.inv();
+    const unsigned __int128 mask = ((unsigned __int128)1 << log_base) - 1;
+#pragma omp parallel for num_threads(nthreads) schedule(dynamic, 1)
+    for (long long b = 0; b < (long long)batch; ++b) {
+        ntt_full(a + b * t, log_t, inverse != 0, false, 1);
+        for (size_t k = 0; k < t; ++k) {
+            // wraps modulo 2^128, a multiple of the order 2^log_base
+            const unsigned __int128 e = ((unsigned __int128)(u64)b + b0) * ((unsigned __int128)alpha * k + beta) + (unsigned __int128)gamma * k;
+            a[b * t + k] = a[b * t + k] * fr_pow_u64(base, (u64)(e & mask));
+        }
+    }
+    return 0;
+}
+
 // CSR mat-vec over Fr: out[r] = sum_k val[k] * x[idx[k]], k in [ptr[r], ptr[r+1]) -- the per-row evaluation of qap.rs:60-67
 // (`evaluate_constraint`), with the conventions of b200zk.h (u32 row pointers and column indices, Montgomery values).
 void orc_fr_spmv(const uint32_t* ptr, const uint32_t* idx, const u64* val, const u64* x, size_t n_rows, u64* out,

@@ -135,6 +135,19 @@ def ntt(data, inverse: bool = False, coset: bool = False, nthreads: int = 0) -> 
     return out
 
 
+def ntt_batched_post(data, log_t: int, batch: int, inverse: bool, log_base: int, shift: bool = False, b0: int = 0, alpha: int = 0,
+                     beta: int = 0, gamma: int = 0, nthreads: int = 0) -> np.ndarray:
+    """b200zk_ntt_fr_batched_post_dev: `batch` contiguous NTTs of 2^log_t elements, output k of transform b times
+    base^((b + b0)(alpha k + beta) + gamma k), base = w_{2^log_base} (inverted for an inverse transform unless `shift`).
+    data: (batch * 2^log_t, 4) Montgomery limbs; the same as tests/mgpu_common.OracleBackend.batched_ntt_post."""
+    out = np.array(data, dtype=np.uint64, copy=True, order="C").reshape(-1, 4)
+    assert out.shape[0] == batch << log_t
+    rc = lib().orc_ntt_batched_post(_p(out), log_t, ctypes.c_size_t(batch), int(inverse), log_base, int(shift), ctypes.c_uint64(b0),
+                                    ctypes.c_uint64(alpha), ctypes.c_uint64(beta), ctypes.c_uint64(gamma), nthreads)
+    assert rc == 0
+    return out
+
+
 def bitrev(data) -> np.ndarray:
     out = np.array(data, dtype=np.uint64, copy=True, order="C")
     n = out.shape[0]
