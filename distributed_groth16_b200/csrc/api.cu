@@ -10,6 +10,17 @@ static const char* kVersion = "b200zk 0.1 (sm_90a)";
 
 static bool valid_slot(int s) { return s >= 0 && s < 3; }
 
+// body(slot) with the slot's calls serialised and ctx's device current (the caller may have made another device current, as
+// the multi-GPU groups do)
+template <class Body>
+static int with_slot(b200zk_ctx* ctx, int stream, Body&& body) {
+    if (!ctx || !valid_slot(stream)) return B200ZK_ERR_ARG;
+    Slot& sl = ctx->slots[stream];
+    std::lock_guard<std::mutex> g(sl.mu);
+    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    return body(sl);
+}
+
 extern "C" {
 
 const char* b200zk_version(void) { return kVersion; }
@@ -228,38 +239,36 @@ static int msm_host(b200zk_ctx* ctx, int stream, const uint64_t* bases, size_t n
     const size_t n = n_bases;
     if (n && (!bases || !scalars)) return B200ZK_ERR_ARG;
     const size_t PB = G2 ? 128 : 64, XB = G2 ? 256 : 128;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    B2_CUDA_OK(ctx, sl.small.reserve(1024));
-    char* sm = reinterpret_cast<char*>(sl.small.p);
-    B2_TRY(msm_staged_dev(ctx, sl, G2, bases, scalars, n, sm, false));
-    B2_TRY(G2 ? g2_sum_dev(ctx, sl, sm, 1, sm + XB) : g1_sum_dev(ctx, sl, sm, 1, sm + XB));
-    uint64_t host[17];
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(host, sm + XB, PB + 8, cudaMemcpyDeviceToHost, sl.stream));
-    B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
-    B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.copy_stream));
-    memcpy(out_affine, host, PB);
-    *out_is_inf = (int)host[PB / 8];
-    return B200ZK_OK;
+    return with_slot(ctx, stream, [&](Slot& sl) -> int {
+        B2_CUDA_OK(ctx, sl.small.reserve(1024));
+        char* sm = reinterpret_cast<char*>(sl.small.p);
+        B2_TRY(msm_staged_dev(ctx, sl, G2, bases, scalars, n, sm, false));
+        B2_TRY(G2 ? g2_sum_dev(ctx, sl, sm, 1, sm + XB) : g1_sum_dev(ctx, sl, sm, 1, sm + XB));
+        uint64_t host[17];
+        B2_CUDA_OK(ctx, cudaMemcpyAsync(host, sm + XB, PB + 8, cudaMemcpyDeviceToHost, sl.stream));
+        B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
+        B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.copy_stream));
+        memcpy(out_affine, host, PB);
+        *out_is_inf = (int)host[PB / 8];
+        return B200ZK_OK;
+    });
 }
 
 template <int G2>
 static int sum_host(b200zk_ctx* ctx, int stream, const void* d_xyzz, size_t count, uint64_t* out_affine, int* out_is_inf) {
     if (!ctx || !valid_slot(stream) || !out_affine || !out_is_inf) return B200ZK_ERR_ARG;
     const size_t PB = G2 ? 128 : 64;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    B2_CUDA_OK(ctx, sl.small.reserve(1024));
-    char* sm = reinterpret_cast<char*>(sl.small.p);
-    B2_TRY(G2 ? g2_sum_dev(ctx, sl, d_xyzz, count, sm) : g1_sum_dev(ctx, sl, d_xyzz, count, sm));
-    uint64_t host[17];
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(host, sm, PB + 8, cudaMemcpyDeviceToHost, sl.stream));
-    B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
-    memcpy(out_affine, host, PB);
-    *out_is_inf = (int)host[PB / 8];
-    return B200ZK_OK;
+    return with_slot(ctx, stream, [&](Slot& sl) -> int {
+        B2_CUDA_OK(ctx, sl.small.reserve(1024));
+        char* sm = reinterpret_cast<char*>(sl.small.p);
+        B2_TRY(G2 ? g2_sum_dev(ctx, sl, d_xyzz, count, sm) : g1_sum_dev(ctx, sl, d_xyzz, count, sm));
+        uint64_t host[17];
+        B2_CUDA_OK(ctx, cudaMemcpyAsync(host, sm, PB + 8, cudaMemcpyDeviceToHost, sl.stream));
+        B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
+        memcpy(out_affine, host, PB);
+        *out_is_inf = (int)host[PB / 8];
+        return B200ZK_OK;
+    });
 }
 
 extern "C" {
@@ -278,43 +287,28 @@ int b200zk_msm_staged_dev(b200zk_ctx* ctx, int stream, int g2, const uint64_t* b
     if (!ctx || !valid_slot(stream) || !d_out_xyzz) return B200ZK_ERR_ARG;
     if (n_bases != n_scalars) return set_error(ctx, B200ZK_ERR_LENGTH, std::to_string(n_bases < n_scalars ? n_bases : n_scalars));
     if (n_bases && (!bases || !scalars)) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    return msm_staged_dev(ctx, sl, g2, bases, scalars, n_bases, d_out_xyzz, true);
+    return with_slot(ctx, stream, [&](Slot& sl) { return msm_staged_dev(ctx, sl, g2, bases, scalars, n_bases, d_out_xyzz, true); });
 }
 
 int b200zk_msm_g1_dev(b200zk_ctx* ctx, int stream, const void* d_bases, const void* d_scalars, size_t n, void* d_out) {
     if (!ctx || !valid_slot(stream) || !d_out) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return msm_g1_dev(ctx, sl, d_bases, d_scalars, n, d_out);
+    return with_slot(ctx, stream, [&](Slot& sl) { return msm_g1_dev(ctx, sl, d_bases, d_scalars, n, d_out); });
 }
 int b200zk_msm_g2_dev(b200zk_ctx* ctx, int stream, const void* d_bases, const void* d_scalars, size_t n, void* d_out) {
     if (!ctx || !valid_slot(stream) || !d_out) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return msm_g2_dev(ctx, sl, d_bases, d_scalars, n, d_out);
+    return with_slot(ctx, stream, [&](Slot& sl) { return msm_g2_dev(ctx, sl, d_bases, d_scalars, n, d_out); });
 }
 
 unsigned b200zk_msm_table_windows(unsigned c) { return c ? msm_table_windows(c) : 0; }
 unsigned b200zk_msm_table_auto_window(size_t n) { return msm_table_auto_window(n); }
 int b200zk_msm_table_build_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_bases, size_t n, unsigned c, void* d_table) {
     if (!ctx || !valid_slot(stream) || (n && (!d_bases || !d_table))) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return msm_table_build_dev(ctx, sl, g2, d_bases, n, c, d_table);
+    return with_slot(ctx, stream, [&](Slot& sl) { return msm_table_build_dev(ctx, sl, g2, d_bases, n, c, d_table); });
 }
 int b200zk_msm_table_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_table, const void* d_scalars, size_t n, unsigned c,
                          void* d_out) {
     if (!ctx || !valid_slot(stream) || !d_out) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return msm_table_dev(ctx, sl, g2, d_table, d_scalars, n, c, d_out);
+    return with_slot(ctx, stream, [&](Slot& sl) { return msm_table_dev(ctx, sl, g2, d_table, d_scalars, n, c, d_out); });
 }
 
 int b200zk_g1_sum_dev(b200zk_ctx* ctx, int stream, const void* d, size_t count, uint64_t out[8], int* inf) {
@@ -333,53 +327,48 @@ int b200zk_ntt_fr(b200zk_ctx* ctx, int stream, uint64_t* data, unsigned log_n, i
     if (pad & (pad - 1)) return set_error(ctx, B200ZK_ERR_ARG, "pad must be a power of two");
     const size_t n = (size_t)1 << log_n, n_out = n * pad;
     unsigned log_out = log_n + ceil_log2(pad);
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    B2_CUDA_OK(ctx, sl.io_a.reserve(2 * n_out * sizeof(Fr)));
-    Fr* b0 = reinterpret_cast<Fr*>(sl.io_a.p);
-    Fr* b1 = b0 + n_out;
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(b0, data, n * sizeof(Fr), cudaMemcpyHostToDevice, sl.stream));
-    Fr* cur = b0; Fr* other = b1;
-    if (bitrev_in) { B2_TRY(bitrev_dev(ctx, sl, cur, other, log_n)); std::swap(cur, other); }
-    B2_TRY(ntt_dev(ctx, sl, cur, other, log_n, inverse != 0, coset != 0, 1));
-    std::swap(cur, other);
-    if (pad > 1) B2_CUDA_OK(ctx, cudaMemsetAsync(cur + n, 0, (n_out - n) * sizeof(Fr), sl.stream));
-    if (bitrev_out) { B2_TRY(bitrev_dev(ctx, sl, cur, other, log_out)); std::swap(cur, other); }
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(data, cur, n_out * sizeof(Fr), cudaMemcpyDeviceToHost, sl.stream));
-    B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
-    return B200ZK_OK;
+    return with_slot(ctx, stream, [&](Slot& sl) -> int {
+        B2_CUDA_OK(ctx, sl.io_a.reserve(2 * n_out * sizeof(Fr)));
+        Fr* b0 = reinterpret_cast<Fr*>(sl.io_a.p);
+        Fr* b1 = b0 + n_out;
+        B2_CUDA_OK(ctx, cudaMemcpyAsync(b0, data, n * sizeof(Fr), cudaMemcpyHostToDevice, sl.stream));
+        Fr* cur = b0; Fr* other = b1;
+        if (bitrev_in) { B2_TRY(bitrev_dev(ctx, sl, cur, other, log_n)); std::swap(cur, other); }
+        B2_TRY(ntt_dev(ctx, sl, cur, other, log_n, inverse != 0, coset != 0, 1));
+        std::swap(cur, other);
+        if (pad > 1) B2_CUDA_OK(ctx, cudaMemsetAsync(cur + n, 0, (n_out - n) * sizeof(Fr), sl.stream));
+        if (bitrev_out) { B2_TRY(bitrev_dev(ctx, sl, cur, other, log_out)); std::swap(cur, other); }
+        B2_CUDA_OK(ctx, cudaMemcpyAsync(data, cur, n_out * sizeof(Fr), cudaMemcpyDeviceToHost, sl.stream));
+        B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
+        return B200ZK_OK;
+    });
 }
 
 int b200zk_ntt_fr_dev(b200zk_ctx* ctx, int stream, const void* d_in, void* d_out, unsigned log_n, int inverse, int coset,
                       unsigned batch) {
     if (!ctx || !valid_slot(stream) || !d_in || !d_out || batch == 0) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return ntt_dev(ctx, sl, reinterpret_cast<const Fr*>(d_in), reinterpret_cast<Fr*>(d_out), log_n, inverse != 0,
-                   coset != 0, batch);
+    return with_slot(ctx, stream, [&](Slot& sl) {
+        return ntt_dev(ctx, sl, reinterpret_cast<const Fr*>(d_in), reinterpret_cast<Fr*>(d_out), log_n, inverse != 0, coset != 0, batch);
+    });
 }
 
 int b200zk_ntt_fr_fourstep_cols_dev(b200zk_ctx* ctx, int stream, const void* d_in, void* d_out, unsigned log_rows,
                                     unsigned log_cols_local, unsigned log_n, uint64_t global_col0, int inverse) {
     if (!ctx || !valid_slot(stream)) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return fourstep_cols_dev(ctx, sl, reinterpret_cast<const Fr*>(d_in), reinterpret_cast<Fr*>(d_out), log_rows,
-                             log_cols_local, log_n, global_col0, inverse != 0);
+    return with_slot(ctx, stream, [&](Slot& sl) {
+        return fourstep_cols_dev(ctx, sl, reinterpret_cast<const Fr*>(d_in), reinterpret_cast<Fr*>(d_out), log_rows, log_cols_local,
+                                 log_n, global_col0, inverse != 0);
+    });
 }
 
 int b200zk_ntt_fr_fourstep_cols_p2p_dev(b200zk_ctx* ctx, int stream, const void* d_in, void* const* peer_out, unsigned n_peers,
                                         unsigned log_rows, unsigned log_cols_local, unsigned log_n, uint64_t global_col0,
                                         int inverse) {
     if (!ctx || !valid_slot(stream) || !d_in || !peer_out) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return fourstep_cols_p2p_dev(ctx, sl, reinterpret_cast<const Fr*>(d_in), peer_out, n_peers, log_rows, log_cols_local, log_n,
-                                 global_col0, inverse != 0);
+    return with_slot(ctx, stream, [&](Slot& sl) {
+        return fourstep_cols_p2p_dev(ctx, sl, reinterpret_cast<const Fr*>(d_in), peer_out, n_peers, log_rows, log_cols_local, log_n,
+                                     global_col0, inverse != 0);
+    });
 }
 
 int b200zk_peer_alloc(b200zk_ctx* ctx, size_t bytes, void** d_ptr, uint8_t handle_out[64]) {
@@ -417,56 +406,51 @@ int b200zk_peer_free(b200zk_ctx* ctx, void* d_ptr) {
 int b200zk_msm_exchange_sum_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_partial, void* const* peer_mailboxes, unsigned n_peers,
                                 unsigned rank, uint64_t seq, void* d_out_affine) {
     if (!ctx || !valid_slot(stream) || !d_partial || !peer_mailboxes || !d_out_affine) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    return msm_exchange_sum_dev(ctx, sl, g2, d_partial, peer_mailboxes, n_peers, rank, seq, d_out_affine);
+    return with_slot(ctx, stream, [&](Slot& sl) {
+        return msm_exchange_sum_dev(ctx, sl, g2, d_partial, peer_mailboxes, n_peers, rank, seq, d_out_affine);
+    });
 }
 
 int b200zk_ntt_fr_batched_post_dev(b200zk_ctx* ctx, int stream, const void* d_in, void* d_out, unsigned log_t, unsigned batch,
                                    int inverse, unsigned log_base, int base_is_shift, uint64_t b0, uint64_t alpha,
                                    uint64_t beta, uint64_t gamma) {
     if (!ctx || !valid_slot(stream) || !d_in || !d_out || batch == 0) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return ntt_batched_post_dev(ctx, sl, reinterpret_cast<const Fr*>(d_in), reinterpret_cast<Fr*>(d_out), log_t, batch,
-                                inverse != 0, log_base, base_is_shift != 0, b0, alpha, beta, gamma);
+    return with_slot(ctx, stream, [&](Slot& sl) {
+        return ntt_batched_post_dev(ctx, sl, reinterpret_cast<const Fr*>(d_in), reinterpret_cast<Fr*>(d_out), log_t, batch, inverse != 0,
+                                    log_base, base_is_shift != 0, b0, alpha, beta, gamma);
+    });
 }
 
 int b200zk_fr_mul_sub_dev(b200zk_ctx* ctx, int stream, const void* d_a, const void* d_b, const void* d_c, void* d_out, size_t n) {
     if (!ctx || !valid_slot(stream) || (n && (!d_a || !d_b || !d_c || !d_out))) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return mul_sub_dev(ctx, sl, (const Fr*)d_a, (const Fr*)d_b, (const Fr*)d_c, (Fr*)d_out, n);
+    return with_slot(ctx, stream, [&](Slot& sl) {
+        return mul_sub_dev(ctx, sl, (const Fr*)d_a, (const Fr*)d_b, (const Fr*)d_c, (Fr*)d_out, n);
+    });
 }
 
 // ---- h -----------------------------------------------------------------------------------------
 int b200zk_h_circom_dev(b200zk_ctx* ctx, const void* d_a, const void* d_b, const void* d_c, unsigned log_m, void* d_h) {
     if (!ctx || !d_a || !d_b || !d_c || !d_h) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[0];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return h_circom_dev(ctx, sl, (const Fr*)d_a, (const Fr*)d_b, (const Fr*)d_c, log_m, (Fr*)d_h);
+    return with_slot(ctx, 0, [&](Slot& sl) {
+        return h_circom_dev(ctx, sl, (const Fr*)d_a, (const Fr*)d_b, (const Fr*)d_c, log_m, (Fr*)d_h);
+    });
 }
 
 int b200zk_h_circom(b200zk_ctx* ctx, const uint64_t* a, const uint64_t* b, const uint64_t* c, unsigned log_m, uint64_t* h_out) {
     if (!ctx || !a || !b || !c || !h_out) return B200ZK_ERR_ARG;
     if (log_m + 1 > 28) return set_error(ctx, B200ZK_ERR_DOMAIN, "2m exceeds the 2^28 subgroup (PolynomialDegreeTooLarge)");
     const size_t m = (size_t)1 << log_m;
-    Slot& sl = ctx->slots[0];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    B2_CUDA_OK(ctx, sl.io_a.reserve(4 * m * sizeof(Fr)));
-    Fr* d = reinterpret_cast<Fr*>(sl.io_a.p);
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(d, a, m * sizeof(Fr), cudaMemcpyHostToDevice, sl.stream));
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(d + m, b, m * sizeof(Fr), cudaMemcpyHostToDevice, sl.stream));
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(d + 2 * m, c, m * sizeof(Fr), cudaMemcpyHostToDevice, sl.stream));
-    B2_TRY(h_circom_dev(ctx, sl, d, d + m, d + 2 * m, log_m, d + 3 * m));
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(h_out, d + 3 * m, m * sizeof(Fr), cudaMemcpyDeviceToHost, sl.stream));
-    B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
-    return B200ZK_OK;
+    return with_slot(ctx, 0, [&](Slot& sl) -> int {
+        B2_CUDA_OK(ctx, sl.io_a.reserve(4 * m * sizeof(Fr)));
+        Fr* d = reinterpret_cast<Fr*>(sl.io_a.p);
+        B2_CUDA_OK(ctx, cudaMemcpyAsync(d, a, m * sizeof(Fr), cudaMemcpyHostToDevice, sl.stream));
+        B2_CUDA_OK(ctx, cudaMemcpyAsync(d + m, b, m * sizeof(Fr), cudaMemcpyHostToDevice, sl.stream));
+        B2_CUDA_OK(ctx, cudaMemcpyAsync(d + 2 * m, c, m * sizeof(Fr), cudaMemcpyHostToDevice, sl.stream));
+        B2_TRY(h_circom_dev(ctx, sl, d, d + m, d + 2 * m, log_m, d + 3 * m));
+        B2_CUDA_OK(ctx, cudaMemcpyAsync(h_out, d + 3 * m, m * sizeof(Fr), cudaMemcpyDeviceToHost, sl.stream));
+        B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
+        return B200ZK_OK;
+    });
 }
 
 // ---- qap / conversions -------------------------------------------------------------------------
@@ -474,17 +458,13 @@ int b200zk_qap_dev(b200zk_ctx* ctx, int stream, const void* a_ptr, const void* a
                    const void* b_col, const void* b_val, size_t nc, size_t n_inputs, const void* d_z, unsigned log_m, void* d_a,
                    void* d_b, void* d_c) {
     if (!ctx || !valid_slot(stream) || !a_ptr || !b_ptr || !d_z || !d_a || !d_b || !d_c) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return qap_dev(ctx, sl, a_ptr, a_col, a_val, b_ptr, b_col, b_val, nc, n_inputs, d_z, log_m, d_a, d_b, d_c);
+    return with_slot(ctx, stream, [&](Slot& sl) {
+        return qap_dev(ctx, sl, a_ptr, a_col, a_val, b_ptr, b_col, b_val, nc, n_inputs, d_z, log_m, d_a, d_b, d_c);
+    });
 }
 int b200zk_fr_convert_dev(b200zk_ctx* ctx, int stream, const void* d_in, void* d_out, size_t n, int to_mont, int times) {
     if (!ctx || !valid_slot(stream) || (n && (!d_in || !d_out)) || times < 0) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return fr_convert_dev(ctx, sl, d_in, d_out, n, to_mont, times);
+    return with_slot(ctx, stream, [&](Slot& sl) { return fr_convert_dev(ctx, sl, d_in, d_out, n, to_mont, times); });
 }
 int b200zk_r1cs_check_dev(b200zk_ctx* ctx, int stream, const void* a_ptr, const void* a_col, const void* a_val, const void* b_ptr,
                           const void* b_col, const void* b_val, const void* c_ptr, const void* c_col, const void* c_val, size_t nc,
@@ -497,13 +477,10 @@ int b200zk_r1cs_check_dev(b200zk_ctx* ctx, int stream, const void* a_ptr, const 
     }
     if (!valid_slot(stream) || !a_ptr || !b_ptr || !c_ptr || !d_w || !n_failed || !first_failed)
         return set_error(ctx, B200ZK_ERR_ARG, "r1cs_check: null pointer or bad stream slot");
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
     const void* ptr[3] = {a_ptr, b_ptr, c_ptr};
     const void* col[3] = {a_col, b_col, c_col};
     const void* val[3] = {a_val, b_val, c_val};
-    return r1cs_check_dev(ctx, sl, ptr, col, val, nc, d_w, n_failed, first_failed);
+    return with_slot(ctx, stream, [&](Slot& sl) { return r1cs_check_dev(ctx, sl, ptr, col, val, nc, d_w, n_failed, first_failed); });
 }
 
 // ---- proving key + prove -----------------------------------------------------------------------
@@ -534,11 +511,8 @@ static int pk_build(b200zk_ctx* ctx, const void* a_query, const void* b_g1_query
     if (!rc) rc = upload(ctx, &pk->vk, vk_points, 56 * 8);
     if (!rc && cudaStreamSynchronize(ctx->slots[0].stream) != cudaSuccess) rc = set_error(ctx, B200ZK_ERR_CUDA, "proving-key upload failed");
     if (rc) { b200zk_pk_free(ctx, pk); return rc; }
-    const char* env = getenv("B200ZK_PK_TABLES");
-    if (!(env && env[0] == '0')) {
-        std::lock_guard<std::mutex> g(ctx->slots[0].mu);
-        B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-        rc = pk_precompute_dev(ctx, pk, 0);
+    if (pk_tables_enabled()) {
+        rc = with_slot(ctx, 0, [&](Slot&) { return pk_precompute_dev(ctx, pk, 0); });
         if (rc) { b200zk_pk_free(ctx, pk); return rc; }
     }
     *out = pk;
@@ -569,63 +543,55 @@ void b200zk_pk_free(b200zk_ctx* ctx, b200zk_pk* pk) {
 
 int b200zk_pk_precompute(b200zk_ctx* ctx, b200zk_pk* pk, unsigned c) {
     if (!ctx || !pk) return B200ZK_ERR_ARG;
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    std::lock_guard<std::mutex> g(ctx->slots[0].mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    if (c == 0xFFFFFFFFu) { pk_free_tables(pk); return B200ZK_OK; }
-    return pk_precompute_dev(ctx, pk, c);
+    return with_slot(ctx, 0, [&](Slot&) -> int {
+        if (c == 0xFFFFFFFFu) { pk_free_tables(pk); return B200ZK_OK; }
+        return pk_precompute_dev(ctx, pk, c);
+    });
 }
 size_t b200zk_pk_table_bytes(const b200zk_pk* pk) { return pk ? pk->tab_bytes : 0; }
 
 int b200zk_groth16_prove(b200zk_ctx* ctx, const b200zk_pk* pk, const uint64_t* z, const uint64_t* a, const uint64_t* b,
                          const uint64_t* c, const uint64_t r[4], const uint64_t s[4], int mirror_bg1, uint8_t proof_out[128]) {
     if (!ctx || !pk || !z || !a || !b || !c || !r || !s || !proof_out) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[0];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    const size_t m = pk->m, nv = pk->n_vars;
-    B2_CUDA_OK(ctx, sl.io_a.reserve((nv + 3 * m) * sizeof(Fr)));
-    Fr* d_z = reinterpret_cast<Fr*>(sl.io_a.p);
-    Fr* d_abc = d_z + nv;
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(d_z, z, nv * sizeof(Fr), cudaMemcpyHostToDevice, sl.stream));
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(d_abc, a, m * sizeof(Fr), cudaMemcpyHostToDevice, sl.stream));
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(d_abc + m, b, m * sizeof(Fr), cudaMemcpyHostToDevice, sl.stream));
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(d_abc + 2 * m, c, m * sizeof(Fr), cudaMemcpyHostToDevice, sl.stream));
-    return prove_dev(ctx, pk, d_z, d_abc, d_abc + m, d_abc + 2 * m, r, s, mirror_bg1, proof_out);
+    return with_slot(ctx, 0, [&](Slot& sl) -> int {
+        const size_t m = pk->m, nv = pk->n_vars;
+        B2_CUDA_OK(ctx, sl.io_a.reserve((nv + 3 * m) * sizeof(Fr)));
+        Fr* d_z = reinterpret_cast<Fr*>(sl.io_a.p);
+        Fr* d_abc = d_z + nv;
+        B2_CUDA_OK(ctx, cudaMemcpyAsync(d_z, z, nv * sizeof(Fr), cudaMemcpyHostToDevice, sl.stream));
+        B2_CUDA_OK(ctx, cudaMemcpyAsync(d_abc, a, m * sizeof(Fr), cudaMemcpyHostToDevice, sl.stream));
+        B2_CUDA_OK(ctx, cudaMemcpyAsync(d_abc + m, b, m * sizeof(Fr), cudaMemcpyHostToDevice, sl.stream));
+        B2_CUDA_OK(ctx, cudaMemcpyAsync(d_abc + 2 * m, c, m * sizeof(Fr), cudaMemcpyHostToDevice, sl.stream));
+        return prove_dev(ctx, pk, d_z, d_abc, d_abc + m, d_abc + 2 * m, r, s, mirror_bg1, proof_out);
+    });
 }
 
 int b200zk_groth16_prove_dev(b200zk_ctx* ctx, const b200zk_pk* pk, const void* d_z, const void* d_a, const void* d_b,
                              const void* d_c, const uint64_t r[4], const uint64_t s[4], int mirror_bg1, uint8_t proof_out[128]) {
     if (!ctx || !pk || !d_z || !d_a || !d_b || !d_c || !r || !s || !proof_out) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[0];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    return prove_dev(ctx, pk, (const Fr*)d_z, (const Fr*)d_a, (const Fr*)d_b, (const Fr*)d_c, r, s, mirror_bg1, proof_out);
+    return with_slot(ctx, 0, [&](Slot&) {
+        return prove_dev(ctx, pk, (const Fr*)d_z, (const Fr*)d_a, (const Fr*)d_b, (const Fr*)d_c, r, s, mirror_bg1, proof_out);
+    });
 }
 
 int b200zk_points_compress_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_affine, size_t n, void* d_bytes) {
     if (!ctx || !valid_slot(stream) || (n && (!d_affine || !d_bytes))) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return points_compress_dev(ctx, sl, g2, d_affine, n, d_bytes);
+    return with_slot(ctx, stream, [&](Slot& sl) { return points_compress_dev(ctx, sl, g2, d_affine, n, d_bytes); });
 }
 int b200zk_points_decompress_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_bytes, size_t n, int check_subgroup,
                                  void* d_affine, size_t* n_invalid) {
     if (!ctx || !valid_slot(stream) || (n && (!d_affine || !d_bytes))) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return points_decompress_dev(ctx, sl, g2, d_bytes, n, check_subgroup, d_affine, n_invalid);
+    return with_slot(ctx, stream, [&](Slot& sl) {
+        return points_decompress_dev(ctx, sl, g2, d_bytes, n, check_subgroup, d_affine, n_invalid);
+    });
 }
 
 int b200zk_points_matmul_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_points, size_t n_chunks, size_t l,
                              const void* d_matrix, size_t rows, void* d_out) {
     if (!ctx || !valid_slot(stream) || (n_chunks && rows && (!d_points || !d_matrix || !d_out))) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return points_matmul_dev(ctx, sl, g2, d_points, n_chunks, l, d_matrix, rows, d_out);
+    return with_slot(ctx, stream, [&](Slot& sl) {
+        return points_matmul_dev(ctx, sl, g2, d_points, n_chunks, l, d_matrix, rows, d_out);
+    });
 }
 
 int b200zk_groth16_verify(b200zk_ctx* ctx, const uint64_t* alpha_g1, const uint64_t* beta_g2, const uint64_t* gamma_g2,
@@ -634,131 +600,96 @@ int b200zk_groth16_verify(b200zk_ctx* ctx, const uint64_t* alpha_g1, const uint6
     if (!ctx || !alpha_g1 || !beta_g2 || !gamma_g2 || !delta_g2 || !gamma_abc_g1 || (n_public && !public_inputs) || !proof_a ||
         !proof_b || !proof_c || !is_valid)
         return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[0];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    return groth16_verify_dev(ctx, sl, alpha_g1, beta_g2, gamma_g2, delta_g2, gamma_abc_g1, n_public, public_inputs, proof_a, proof_b,
-                              proof_c, is_valid);
+    return with_slot(ctx, 0, [&](Slot& sl) {
+        return groth16_verify_dev(ctx, sl, alpha_g1, beta_g2, gamma_g2, delta_g2, gamma_abc_g1, n_public, public_inputs, proof_a, proof_b,
+                                  proof_c, is_valid);
+    });
 }
 int b200zk_vk_alphabeta_12(b200zk_ctx* ctx, const uint64_t alpha_g1[8], const uint64_t beta_g2[16], uint64_t out[48]) {
     if (!ctx || !alpha_g1 || !beta_g2 || !out) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[0];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    return vk_alphabeta_12_dev(ctx, sl, alpha_g1, beta_g2, out);
+    return with_slot(ctx, 0, [&](Slot& sl) { return vk_alphabeta_12_dev(ctx, sl, alpha_g1, beta_g2, out); });
 }
 
 int b200zk_xyzz_sum_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_in, size_t count, size_t stride, void* d_out) {
     if (!ctx || !valid_slot(stream) || !d_in || !d_out || count == 0) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return xyzz_sum_dev(ctx, sl, g2, d_in, count, stride, d_out);
+    return with_slot(ctx, stream, [&](Slot& sl) { return xyzz_sum_dev(ctx, sl, g2, d_in, count, stride, d_out); });
 }
 int b200zk_groth16_assemble_dev(b200zk_ctx* ctx, const b200zk_pk* pk, const void* d_msm_a, const void* d_msm_b2,
                                 const void* d_msm_l, const void* d_msm_h, const void* d_msm_b1, const uint64_t r[4],
                                 const uint64_t s[4], int include_zero_terms, uint8_t proof_out[128]) {
     if (!ctx || !pk || !d_msm_a || !d_msm_b2 || !d_msm_l || !d_msm_h || !r || !s || !proof_out) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[0];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return assemble_dev(ctx, sl, pk, d_msm_a, d_msm_b2, d_msm_l, d_msm_h, d_msm_b1, r, s, include_zero_terms, proof_out);
+    return with_slot(ctx, 0, [&](Slot& sl) {
+        return assemble_dev(ctx, sl, pk, d_msm_a, d_msm_b2, d_msm_l, d_msm_h, d_msm_b1, r, s, include_zero_terms, proof_out);
+    });
 }
 
 // ---- setup building blocks -----------------------------------------------------------------------
 int b200zk_fixed_base_mul_dev(b200zk_ctx* ctx, int g2, const void* d_scalars, size_t n, void* d_out) {
     if (!ctx || (n && (!d_scalars || !d_out))) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[0];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    return fixed_base_mul_dev(ctx, sl, g2, d_scalars, n, d_out);
+    return with_slot(ctx, 0, [&](Slot& sl) { return fixed_base_mul_dev(ctx, sl, g2, d_scalars, n, d_out); });
 }
 int b200zk_fr_powers_dev(b200zk_ctx* ctx, const uint64_t base[4], const uint64_t scale[4], size_t n, void* d_out) {
     if (!ctx || !base || !scale || (n && !d_out)) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[0];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return fr_powers_dev(ctx, sl, base, scale, n, d_out);
+    return with_slot(ctx, 0, [&](Slot& sl) { return fr_powers_dev(ctx, sl, base, scale, n, d_out); });
 }
 int b200zk_fr_spmv_dev(b200zk_ctx* ctx, const void* d_ptr, const void* d_idx, const void* d_val, const void* d_x, size_t n_rows,
                        void* d_out) {
     if (!ctx || !d_ptr || !d_x || (n_rows && !d_out)) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[0];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return spmv_dev(ctx, sl, d_ptr, d_idx, d_val, d_x, n_rows, d_out);
+    return with_slot(ctx, 0, [&](Slot& sl) { return spmv_dev(ctx, sl, d_ptr, d_idx, d_val, d_x, n_rows, d_out); });
 }
 int b200zk_points_spmv_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_ptr, const void* d_idx, const void* d_val,
                            const void* d_points, size_t n_rows, void* d_out) {
     if (!ctx || !valid_slot(stream) || (n_rows && (!d_ptr || !d_idx || !d_val || !d_points || !d_out))) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return points_spmv_dev(ctx, sl, g2, d_ptr, d_idx, d_val, d_points, n_rows, d_out);
+    return with_slot(ctx, stream, [&](Slot& sl) {
+        return points_spmv_dev(ctx, sl, g2, d_ptr, d_idx, d_val, d_points, n_rows, d_out);
+    });
 }
 int b200zk_points_scale_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_points, size_t n, const uint64_t k[4],
                             void* d_out) {
     if (!ctx || !k || !valid_slot(stream) || (n && (!d_points || !d_out))) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return points_scale_dev(ctx, sl, g2, d_points, n, k, d_out);
+    return with_slot(ctx, stream, [&](Slot& sl) { return points_scale_dev(ctx, sl, g2, d_points, n, k, d_out); });
 }
 int b200zk_points_intt_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_in, unsigned log_n, void* d_out) {
     if (!ctx) return B200ZK_ERR_ARG;
     if (!valid_slot(stream) || !d_in || !d_out) return set_error(ctx, B200ZK_ERR_ARG, "points_intt: null pointer or bad stream slot");
     if (log_n > 28) return set_error(ctx, B200ZK_ERR_DOMAIN, "points_intt: log_n > 28 (the two-adicity of Fr)");
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return points_intt_dev(ctx, sl, g2, d_in, log_n, d_out);
+    return with_slot(ctx, stream, [&](Slot& sl) { return points_intt_dev(ctx, sl, g2, d_in, log_n, d_out); });
 }
 int b200zk_points_ntt_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_in, unsigned log_n, void* d_out) {
     if (!ctx) return B200ZK_ERR_ARG;
     if (!valid_slot(stream) || !d_in || !d_out) return set_error(ctx, B200ZK_ERR_ARG, "points_ntt: null pointer or bad stream slot");
     if (log_n > 28) return set_error(ctx, B200ZK_ERR_DOMAIN, "points_ntt: log_n > 28 (the two-adicity of Fr)");
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    return points_ntt_dev(ctx, sl, g2, d_in, log_n, d_out);
+    return with_slot(ctx, stream, [&](Slot& sl) { return points_ntt_dev(ctx, sl, g2, d_in, log_n, d_out); });
 }
 int b200zk_points_mul_powers_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_points, size_t n, const uint64_t first[4],
                                  const uint64_t ratio[4], void* d_out) {
     if (!ctx) return B200ZK_ERR_ARG;
     if (!valid_slot(stream) || !first || !ratio || (n && (!d_points || !d_out)))
         return set_error(ctx, B200ZK_ERR_ARG, "points_mul_powers: null pointer or bad stream slot");
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return points_mul_powers_dev(ctx, sl, g2, d_points, n, first, ratio, d_out);
+    return with_slot(ctx, stream, [&](Slot& sl) {
+        return points_mul_powers_dev(ctx, sl, g2, d_points, n, first, ratio, d_out);
+    });
 }
 int b200zk_points_sub_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_a, const void* d_b, size_t n, void* d_out) {
     if (!ctx) return B200ZK_ERR_ARG;
     if (!valid_slot(stream) || (n && (!d_a || !d_b || !d_out)))
         return set_error(ctx, B200ZK_ERR_ARG, "points_sub: null pointer or bad stream slot");
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return points_sub_dev(ctx, sl, g2, d_a, d_b, n, d_out);
+    return with_slot(ctx, stream, [&](Slot& sl) { return points_sub_dev(ctx, sl, g2, d_a, d_b, n, d_out); });
 }
 int b200zk_points_encode_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_affine, size_t n, int fmt, void* d_bytes) {
     if (!ctx) return B200ZK_ERR_ARG;
     if (!valid_slot(stream) || (n && (!d_affine || !d_bytes)))
         return set_error(ctx, B200ZK_ERR_ARG, "points_encode: null pointer or bad stream slot");
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return points_encode_dev(ctx, sl, g2, d_affine, n, fmt, d_bytes);
+    return with_slot(ctx, stream, [&](Slot& sl) { return points_encode_dev(ctx, sl, g2, d_affine, n, fmt, d_bytes); });
 }
 int b200zk_points_decode_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_bytes, size_t n, int fmt, int check_subgroup,
                              void* d_affine, size_t* n_invalid, size_t* first_invalid) {
     if (!ctx) return B200ZK_ERR_ARG;
     if (!valid_slot(stream) || (n && (!d_bytes || !d_affine)))
         return set_error(ctx, B200ZK_ERR_ARG, "points_decode: null pointer or bad stream slot");
-    Slot& sl = ctx->slots[stream];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return points_decode_dev(ctx, sl, g2, d_bytes, n, fmt, check_subgroup, d_affine, n_invalid, first_invalid);
+    return with_slot(ctx, stream, [&](Slot& sl) {
+        return points_decode_dev(ctx, sl, g2, d_bytes, n, fmt, check_subgroup, d_affine, n_invalid, first_invalid);
+    });
 }
 
 // ---- Blake2b-512 with an exported state (csrc/blake2b.cuh): host only, no context --------------------------------------
@@ -788,33 +719,21 @@ int b200zk_blake2b512_final(const uint8_t state[216], uint8_t out[64]) {
 int b200zk_fr_lincomb_dev(b200zk_ctx* ctx, const void* d_a, const void* d_b, const void* d_c, const uint64_t s[16], size_t n,
                           void* d_out) {
     if (!ctx || !s || (n && (!d_a || !d_b || !d_c || !d_out))) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[0];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return fr_lincomb_dev(ctx, sl, d_a, d_b, d_c, s, n, d_out);
+    return with_slot(ctx, 0, [&](Slot& sl) { return fr_lincomb_dev(ctx, sl, d_a, d_b, d_c, s, n, d_out); });
 }
 
 // ---- generators / self-test --------------------------------------------------------------------
 int b200zk_g1_generate_dev(b200zk_ctx* ctx, uint64_t seed, size_t n, void* d_out) {
     if (!ctx || (n && !d_out)) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[0];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return generate_points_dev(ctx, sl, 0, seed, n, d_out);
+    return with_slot(ctx, 0, [&](Slot& sl) { return generate_points_dev(ctx, sl, 0, seed, n, d_out); });
 }
 int b200zk_g2_generate_dev(b200zk_ctx* ctx, uint64_t seed, size_t n, void* d_out) {
     if (!ctx || (n && !d_out)) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[0];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return generate_points_dev(ctx, sl, 1, seed, n, d_out);
+    return with_slot(ctx, 0, [&](Slot& sl) { return generate_points_dev(ctx, sl, 1, seed, n, d_out); });
 }
 int b200zk_fr_generate_dev(b200zk_ctx* ctx, uint64_t seed, size_t n, void* d_out) {
     if (!ctx || (n && !d_out)) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[0];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));     // the caller may have made another device current (multi-GPU groups)
-    return generate_fr_dev(ctx, sl, seed, n, d_out);
+    return with_slot(ctx, 0, [&](Slot& sl) { return generate_fr_dev(ctx, sl, seed, n, d_out); });
 }
 
 int b200zk_fr_op(b200zk_ctx* ctx, int op, const uint64_t* a, const uint64_t* b, uint64_t* out, size_t n) {
@@ -824,17 +743,16 @@ int b200zk_fr_op(b200zk_ctx* ctx, int op, const uint64_t* a, const uint64_t* b, 
 
 int b200zk_test_field_op(b200zk_ctx* ctx, int field, int op, const uint64_t* a, const uint64_t* b, uint64_t* out, size_t n) {
     if (!ctx || !a || !b || !out) return B200ZK_ERR_ARG;
-    Slot& sl = ctx->slots[0];
-    std::lock_guard<std::mutex> g(sl.mu);
-    B2_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    B2_CUDA_OK(ctx, sl.io_a.reserve(3 * n * 32 + 64));
-    char* d = reinterpret_cast<char*>(sl.io_a.p);
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(d, a, n * 32, cudaMemcpyHostToDevice, sl.stream));
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(d + n * 32, b, n * 32, cudaMemcpyHostToDevice, sl.stream));
-    B2_TRY(field_op_dev(ctx, sl, field, op, d, d + n * 32, d + 2 * n * 32, n));
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(out, d + 2 * n * 32, n * 32, cudaMemcpyDeviceToHost, sl.stream));
-    B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
-    return B200ZK_OK;
+    return with_slot(ctx, 0, [&](Slot& sl) -> int {
+        B2_CUDA_OK(ctx, sl.io_a.reserve(3 * n * 32 + 64));
+        char* d = reinterpret_cast<char*>(sl.io_a.p);
+        B2_CUDA_OK(ctx, cudaMemcpyAsync(d, a, n * 32, cudaMemcpyHostToDevice, sl.stream));
+        B2_CUDA_OK(ctx, cudaMemcpyAsync(d + n * 32, b, n * 32, cudaMemcpyHostToDevice, sl.stream));
+        B2_TRY(field_op_dev(ctx, sl, field, op, d, d + n * 32, d + 2 * n * 32, n));
+        B2_CUDA_OK(ctx, cudaMemcpyAsync(out, d + 2 * n * 32, n * 32, cudaMemcpyDeviceToHost, sl.stream));
+        B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
+        return B200ZK_OK;
+    });
 }
 
 }  // extern "C"

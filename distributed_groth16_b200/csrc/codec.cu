@@ -54,13 +54,12 @@ __global__ void __launch_bounds__(128) k_g2_decompress(const uint8_t* in, uint32
 int points_compress_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_affine, size_t n, void* d_bytes) {
     if (n == 0) return B200ZK_OK;
     if (n >= (1ull << 32)) return set_error(ctx, B200ZK_ERR_ARG, "too many points");
-    {
-        LaunchScope ls(ctx, sl.stream, "points_compress");
-        unsigned grid = (unsigned)((n + 127) / 128);
-        if (g2) k_g2_compress<<<grid, 128, 0, sl.stream>>>(reinterpret_cast<const affine_t<Fq2>*>(d_affine), (uint32_t)n, (uint8_t*)d_bytes);
-        else k_g1_compress<<<grid, 128, 0, sl.stream>>>(reinterpret_cast<const affine_t<Fq>*>(d_affine), (uint32_t)n, (uint8_t*)d_bytes);
-    }
-    return check_launch(ctx, "k_compress");
+    const unsigned grid = (unsigned)((n + 127) / 128);
+    if (g2)
+        return launch(ctx, sl.stream, "points_compress", k_g2_compress, grid, 128, 0, reinterpret_cast<const affine_t<Fq2>*>(d_affine),
+                      (uint32_t)n, (uint8_t*)d_bytes);
+    return launch(ctx, sl.stream, "points_compress", k_g1_compress, grid, 128, 0, reinterpret_cast<const affine_t<Fq>*>(d_affine),
+                  (uint32_t)n, (uint8_t*)d_bytes);
 }
 
 // ffjavascript encodings (codec.cuh ffjs_encode): the bytes a phase-1 contribution hashes, about 2.4 GB at power 22 --
@@ -82,20 +81,14 @@ int points_encode_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_affine, s
     if (n == 0) return B200ZK_OK;
     if (n >= ((size_t)1 << 31) * 128) return set_error(ctx, B200ZK_ERR_ARG, "points_encode: too many points");
     const unsigned grid = (unsigned)((n + 127) / 128);
-    {
-        LaunchScope ls(ctx, sl.stream, "points_encode");
-        uint8_t* out = (uint8_t*)d_bytes;
-        if (g2) {
-            const affine_t<Fq2>* in = reinterpret_cast<const affine_t<Fq2>*>(d_affine);
-            if (fmt) k_points_encode<Fq2, true><<<grid, 128, 0, sl.stream>>>(in, n, out);
-            else k_points_encode<Fq2, false><<<grid, 128, 0, sl.stream>>>(in, n, out);
-        } else {
-            const affine_t<Fq>* in = reinterpret_cast<const affine_t<Fq>*>(d_affine);
-            if (fmt) k_points_encode<Fq, true><<<grid, 128, 0, sl.stream>>>(in, n, out);
-            else k_points_encode<Fq, false><<<grid, 128, 0, sl.stream>>>(in, n, out);
-        }
+    uint8_t* out = (uint8_t*)d_bytes;
+    if (g2) {
+        const affine_t<Fq2>* in = reinterpret_cast<const affine_t<Fq2>*>(d_affine);
+        return launch(ctx, sl.stream, "points_encode", fmt ? k_points_encode<Fq2, true> : k_points_encode<Fq2, false>, grid, 128, 0, in, n,
+                      out);
     }
-    return check_launch(ctx, "k_points_encode");
+    const affine_t<Fq>* in = reinterpret_cast<const affine_t<Fq>*>(d_affine);
+    return launch(ctx, sl.stream, "points_encode", fmt ? k_points_encode<Fq, true> : k_points_encode<Fq, false>, grid, 128, 0, in, n, out);
 }
 
 // The inverse (codec.cuh ffjs_decode): one square root per compressed point, one curve-equation check per uncompressed
@@ -133,20 +126,13 @@ int points_decode_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_bytes, si
     B2_CUDA_OK(ctx, cudaMemsetAsync(bad, 0, 8, sl.stream));
     B2_CUDA_OK(ctx, cudaMemsetAsync(bad + 1, 0xFF, 8, sl.stream));
     const unsigned grid = (unsigned)((n + 127) / 128);
-    {
-        LaunchScope ls(ctx, sl.stream, "points_decode");
-        const uint8_t* in = (const uint8_t*)d_bytes;
-        if (g2) {
-            affine_t<Fq2>* out = reinterpret_cast<affine_t<Fq2>*>(d_affine);
-            if (fmt) k_points_decode<Fq2, true><<<grid, 128, 0, sl.stream>>>(in, n, check_subgroup, out, bad);
-            else k_points_decode<Fq2, false><<<grid, 128, 0, sl.stream>>>(in, n, check_subgroup, out, bad);
-        } else {
-            affine_t<Fq>* out = reinterpret_cast<affine_t<Fq>*>(d_affine);
-            if (fmt) k_points_decode<Fq, true><<<grid, 128, 0, sl.stream>>>(in, n, check_subgroup, out, bad);
-            else k_points_decode<Fq, false><<<grid, 128, 0, sl.stream>>>(in, n, check_subgroup, out, bad);
-        }
-    }
-    B2_TRY(check_launch(ctx, "k_points_decode"));
+    const uint8_t* in = (const uint8_t*)d_bytes;
+    if (g2)
+        B2_TRY(launch(ctx, sl.stream, "points_decode", fmt ? k_points_decode<Fq2, true> : k_points_decode<Fq2, false>, grid, 128, 0, in, n,
+                      check_subgroup, reinterpret_cast<affine_t<Fq2>*>(d_affine), bad));
+    else
+        B2_TRY(launch(ctx, sl.stream, "points_decode", fmt ? k_points_decode<Fq, true> : k_points_decode<Fq, false>, grid, 128, 0, in, n,
+                      check_subgroup, reinterpret_cast<affine_t<Fq>*>(d_affine), bad));
     unsigned long long h_bad[2] = {0, 0};
     B2_CUDA_OK(ctx, cudaMemcpyAsync(h_bad, bad, 16, cudaMemcpyDeviceToHost, sl.stream));
     B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
@@ -169,14 +155,13 @@ int points_decompress_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_bytes
     B2_CUDA_OK(ctx, sl.small.reserve(1024));
     uint32_t* bad = reinterpret_cast<uint32_t*>(sl.small.p);
     B2_CUDA_OK(ctx, cudaMemsetAsync(bad, 0, 4, sl.stream));
-    {
-        LaunchScope ls(ctx, sl.stream, "points_decompress");
-        unsigned grid = (unsigned)((n + 127) / 128);
-        if (g2) k_g2_decompress<<<grid, 128, 0, sl.stream>>>((const uint8_t*)d_bytes, (uint32_t)n, check_subgroup,
-                                                            reinterpret_cast<affine_t<Fq2>*>(d_affine), bad);
-        else k_g1_decompress<<<grid, 128, 0, sl.stream>>>((const uint8_t*)d_bytes, (uint32_t)n, reinterpret_cast<affine_t<Fq>*>(d_affine), bad);
-    }
-    B2_TRY(check_launch(ctx, "k_decompress"));
+    const unsigned grid = (unsigned)((n + 127) / 128);
+    if (g2)
+        B2_TRY(launch(ctx, sl.stream, "points_decompress", k_g2_decompress, grid, 128, 0, (const uint8_t*)d_bytes, (uint32_t)n,
+                      check_subgroup, reinterpret_cast<affine_t<Fq2>*>(d_affine), bad));
+    else
+        B2_TRY(launch(ctx, sl.stream, "points_decompress", k_g1_decompress, grid, 128, 0, (const uint8_t*)d_bytes, (uint32_t)n,
+                      reinterpret_cast<affine_t<Fq>*>(d_affine), bad));
     uint32_t h_bad = 0;
     B2_CUDA_OK(ctx, cudaMemcpyAsync(&h_bad, bad, 4, cudaMemcpyDeviceToHost, sl.stream));
     B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));

@@ -10,6 +10,7 @@
 #include <mutex>
 #include <string>
 #include <tuple>
+#include <utility>
 #include <vector>
 
 #include "../../include/b200zk.h"
@@ -159,6 +160,18 @@ inline int check_launch(b200zk_ctx* ctx, const char* what) {
     return B200ZK_OK;
 }
 
+// Every kernel launch of the library: counted, timed under the profile name `name` while profiling is on, and checked.
+// Arguments convert to the kernel's parameter types as in a direct launch; default arguments do not apply.
+template <class... P, class... A>
+int launch(b200zk_ctx* ctx, cudaStream_t st, const char* name, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem,
+           A&&... args) {
+    {
+        LaunchScope ls(ctx, st, name);
+        kernel<<<grid, block, smem, st>>>(std::forward<A>(args)...);
+    }
+    return check_launch(ctx, name);
+}
+
 static inline unsigned ceil_log2(size_t n) {
     unsigned l = 0;
     while (((size_t)1 << l) < n) ++l;
@@ -243,6 +256,18 @@ int assemble_dev(b200zk_ctx* ctx, Slot& sl, const b200zk_pk* pk, const void* msm
                  uint8_t proof_out[128]);
 int pk_precompute_dev(b200zk_ctx* ctx, b200zk_pk* pk, unsigned c);
 void pk_free_tables(b200zk_pk* pk);
+// false when B200ZK_PK_TABLES=0: proving keys are then uploaded without fixed-base tables
+bool pk_tables_enabled();
+// The fixed-base window tables (msm.cu section 7) of a proving key's five queries src[k] of cnt[k] points (a, b_g1, b_g2, l, h;
+// k = 2 is the G2 one), built on sl's stream with window c_req, or msm_table_auto_window(cnt[k]) per query for c_req = 0.
+// Queries under 64 points get none.  All or nothing: when a table would reach 2^31 entries, when the tables would exceed
+// B200ZK_PK_TABLE_MAX_GB (default: 60% of the HBM free right now) or when an allocation fails, none is kept and the generic MSM
+// runs on the queries.  tab / tab_c / *bytes: what was built (tab_c[k] = 0: no table).
+int pk_tables_build(b200zk_ctx* ctx, Slot& sl, const void* const src[5], const size_t cnt[5], unsigned c_req, void* tab[5],
+                    unsigned tab_c[5], size_t* bytes);
+// MSM over query k (numbered as for pk_tables_build): over tab[k] when tab_c[k] != 0, else the generic MSM on `query`
+int query_msm(b200zk_ctx* ctx, Slot& sl, int k, const void* query, void* const tab[5], const unsigned tab_c[5], const Fr* scalars,
+              size_t n, void* out);
 int prove_dev(b200zk_ctx* ctx, const b200zk_pk* pk, const Fr* d_z, const Fr* d_a, const Fr* d_b, const Fr* d_c,
               const uint64_t r[4], const uint64_t s[4], int mirror_bg1, uint8_t proof_out[128]);
 

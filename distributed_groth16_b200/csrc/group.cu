@@ -98,19 +98,14 @@ struct Blob128 { uint4 v[8]; };
 
 template <class T>
 int transpose_dev(b200zk_ctx* ctx, cudaStream_t st, const void* in, void* out, size_t R, size_t C) {
-    dim3 grid((unsigned)((C + 15) / 16), (unsigned)((R + 15) / 16)), block(16, 16);
-    {
-        LaunchScope ls(ctx, st, "transpose");
-        k_transpose<T><<<grid, block, 0, st>>>(reinterpret_cast<const T*>(in), reinterpret_cast<T*>(out), (uint32_t)R, (uint32_t)C);
-    }
-    return check_launch(ctx, "k_transpose");
+    return launch(ctx, st, "transpose", k_transpose<T>, dim3((unsigned)((C + 15) / 16), (unsigned)((R + 15) / 16)), dim3(16, 16), 0,
+                  reinterpret_cast<const T*>(in), reinterpret_cast<T*>(out), (uint32_t)R, (uint32_t)C);
 }
 
 void split_log(unsigned log_n, unsigned* log_rows, unsigned* log_cols) {
     *log_rows = (log_n + 1) / 2;
     *log_cols = log_n / 2;
 }
-unsigned ilog2(size_t x) { unsigned l = 0; while (((size_t)1 << l) < x) ++l; return l; }
 
 // every device's stream waits until all devices have passed `ev[g]` (recorded on their streams just before)
 int cross_barrier(b200zk_group* grp, std::vector<cudaEvent_t>& ev) {
@@ -155,7 +150,7 @@ int sharded_ntt(b200zk_group* grp, Fr* const* in, Fr* const* out, unsigned log_r
     for (int g = 0; g < P; ++g) {
         b200zk_ctx* ctx = grp->ctx[g];
         G_CUDA_OK(grp, cudaSetDevice(ctx->device));
-        G_TRY(grp, g, fourstep_cols_p2p_dev(ctx, ctx->slots[0], in[g], grp->recv[b], (unsigned)P, log_rows, ilog2(cg), log_rows + log_cols,
+        G_TRY(grp, g, fourstep_cols_p2p_dev(ctx, ctx->slots[0], in[g], grp->recv[b], (unsigned)P, log_rows, ceil_log2(cg), log_rows + log_cols,
                                             (uint64_t)g * cg, inverse));
     }
     rc = cross_barrier(grp, grp->ev_col);          // all column kernels (= all peer stores) are complete
@@ -437,7 +432,7 @@ int b200zk_group_pk_upload(b200zk_group* grp, const uint64_t* a_query, const uin
     if (n_vars == 0 || n_inputs == 0 || n_inputs > n_vars) return gerr(grp, B200ZK_ERR_ARG, "need 1 <= n_inputs <= n_vars");
     if (m == 0 || (m & (m - 1))) return gerr(grp, B200ZK_ERR_DOMAIN, "h_query length must be a power of two");
     const int P = grp->n;
-    const unsigned log_m = ilog2(m);
+    const unsigned log_m = ceil_log2(m);
     unsigned log_rows, log_cols;
     split_log(log_m, &log_rows, &log_cols);
     const size_t rows = (size_t)1 << log_rows, cols = (size_t)1 << log_cols;
@@ -447,8 +442,7 @@ int b200zk_group_pk_upload(b200zk_group* grp, const uint64_t* a_query, const uin
     pk->n = P; pk->n_vars = n_vars; pk->n_inputs = n_inputs; pk->m = m; pk->log_m = log_m;
     pk->shard.resize(P);
     const size_t n_aux = n_vars - n_inputs;
-    const char* tab_env = getenv("B200ZK_PK_TABLES");
-    const bool want_tables = !(tab_env && tab_env[0] == '0');
+    const bool want_tables = pk_tables_enabled();
     auto fail = [&](int rc) { b200zk_group_pk_free(grp, pk); return rc; };
     for (int g = 0; g < P; ++g) {
         b200zk_ctx* ctx = grp->ctx[g];
@@ -477,32 +471,11 @@ int b200zk_group_pk_upload(b200zk_group* grp, const uint64_t* a_query, const uin
             int rc = gfrom(grp, g, transpose_dev<Blob64>(ctx, sl.stream, sl.io_a.p, S.q[4], rows, cg));
             if (rc) return fail(rc);
         }
-        if (want_tables) {
-            // same policy as pk_precompute_dev (prove.cu): window ~ log2(count), all five tables or none, <= 60% of the free HBM
-            double max_gb = 48.0;
-            size_t free_b = 0, total_b = 0;
-            if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess) max_gb = 0.6 * (double)free_b / 1073741824.0;
-            if (const char* env = getenv("B200ZK_PK_TABLE_MAX_GB")) max_gb = atof(env);
-            unsigned cs[5];
-            size_t total = 0;
-            bool ok = true;
-            for (int k = 0; k < 5; ++k) {
-                cs[k] = msm_table_auto_window(cnt[k]);
-                if ((uint64_t)msm_table_windows(cs[k]) * cnt[k] >= (1ull << 31)) ok = false;
-                total += (size_t)msm_table_windows(cs[k]) * cnt[k] * psz[k];
-            }
-            if (ok && (double)total <= max_gb * 1073741824.0) {
-                for (int k = 0; k < 5 && ok; ++k) {
-                    if (cnt[k] < 64) continue;
-                    const size_t bytes = (size_t)msm_table_windows(cs[k]) * cnt[k] * psz[k];
-                    if (cudaMalloc(&S.tab[k], bytes) != cudaSuccess) { cudaGetLastError(); S.tab[k] = nullptr; ok = false; break; }
-                    int rc = gfrom(grp, g, msm_table_build_dev(ctx, sl, k == 2, S.q[k], cnt[k], cs[k], S.tab[k]));
-                    if (rc) return fail(rc);
-                    S.tab_c[k] = cs[k];
-                    pk->table_bytes += bytes;
-                }
-                if (!ok) for (int k = 0; k < 5; ++k) { if (S.tab[k]) { cudaFree(S.tab[k]); S.tab[k] = nullptr; } S.tab_c[k] = 0; }
-            }
+        if (want_tables) {          // automatic windows only: B200ZK_PK_TABLE_WINDOW is not read here
+            size_t bytes = 0;
+            int rc = gfrom(grp, g, pk_tables_build(ctx, sl, S.q, cnt, 0, S.tab, S.tab_c, &bytes));
+            if (rc) return fail(rc);
+            pk->table_bytes += bytes;
         }
     }
     // device 0 keeps the vk points for the final assembly (queries of the tiny pk object are never read: include_zero_terms = 0)
@@ -568,15 +541,14 @@ int b200zk_group_groth16_prove(b200zk_group* grp, const b200zk_group_pk* pk, con
         char* sm = reinterpret_cast<char*>(sl.small.p);
         const Fr* dz = reinterpret_cast<const Fr*>(vz[g]);
         const Fr* dzaux = dz + (S.v1 - S.v0);
-        auto msm = [&](int k, int g2, const Fr* scalars, size_t n, void* out) -> int {
-            if (S.tab_c[k]) return msm_table_dev(ctx, sl, g2, S.tab[k], scalars, n, S.tab_c[k], out);
-            return g2 ? msm_g2_dev(ctx, sl, S.q[k], scalars, n, out) : msm_g1_dev(ctx, sl, S.q[k], scalars, n, out);
+        auto msm = [&](int k, const Fr* scalars, size_t n, void* out) {
+            return query_msm(ctx, sl, k, S.q[k], S.tab, S.tab_c, scalars, n, out);
         };
-        G_TRY(grp, g, msm(2, 1, dz, S.v1 - S.v0, sm + 512));                       // the G2 MSM first: the longest
-        G_TRY(grp, g, msm(0, 0, dz, S.v1 - S.v0, sm + 0));
-        G_TRY(grp, g, msm(3, 0, dzaux, S.l1 - S.l0, sm + 128));
-        G_TRY(grp, g, msm(4, 0, reinterpret_cast<const Fr*>(t2[g]), S.hn, sm + 256));
-        if (need_b1) G_TRY(grp, g, msm(1, 0, dz, S.v1 - S.v0, sm + 384));
+        G_TRY(grp, g, msm(2, dz, S.v1 - S.v0, sm + 512));                       // the G2 MSM first: the longest
+        G_TRY(grp, g, msm(0, dz, S.v1 - S.v0, sm + 0));
+        G_TRY(grp, g, msm(3, dzaux, S.l1 - S.l0, sm + 128));
+        G_TRY(grp, g, msm(4, reinterpret_cast<const Fr*>(t2[g]), S.hn, sm + 256));
+        if (need_b1) G_TRY(grp, g, msm(1, dz, S.v1 - S.v0, sm + 384));
         else G_CUDA_OK(grp, cudaMemsetAsync(sm + 384, 0, 128, sl.stream));
         G_CUDA_OK(grp, cudaEventRecord(grp->ev_done[g], sl.stream));
     }

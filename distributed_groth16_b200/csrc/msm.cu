@@ -511,19 +511,9 @@ static unsigned choose_window(size_t n) {
 
 static int exclusive_scan(b200zk_ctx* ctx, cudaStream_t st, const uint32_t* in, uint32_t* out, uint32_t* sums, uint32_t n) {
     uint32_t nblk = (n + SCAN_TILE - 1) / SCAN_TILE;
-    {
-        LaunchScope ls(ctx, st, "msm_scan");
-        k_scan_local<<<nblk, SCAN_THREADS, 0, st>>>(in, out, sums, n);
-    }
-    {
-        LaunchScope ls(ctx, st, "msm_scan");
-        k_scan_sums<<<1, SCAN_THREADS, 0, st>>>(sums, nblk);
-    }
-    {
-        LaunchScope ls(ctx, st, "msm_scan");
-        k_scan_add<<<nblk, SCAN_THREADS, 0, st>>>(out, sums, n);
-    }
-    return check_launch(ctx, "scan");
+    B2_TRY(launch(ctx, st, "msm_scan", k_scan_local, nblk, SCAN_THREADS, 0, in, out, sums, n));
+    B2_TRY(launch(ctx, st, "msm_scan", k_scan_sums, 1, SCAN_THREADS, 0, sums, nblk));
+    return launch(ctx, st, "msm_scan", k_scan_add, nblk, SCAN_THREADS, 0, out, sums, n);
 }
 
 // event `idx` of MSM channel `ch` (common.cuh), created on first use; only called under the owning slot's mutex
@@ -576,13 +566,7 @@ static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, c
     size_t n = 0, n_max = 0;                                 // all parts together / the largest part
     for (unsigned p = 0; p < nparts; ++p) { n += parts[p].n; n_max = parts[p].n > n_max ? parts[p].n : n_max; }
     xyzz_t<F>* out = reinterpret_cast<xyzz_t<F>*>(d_out);
-    if (n == 0) {
-        {
-            LaunchScope ls(ctx, ms.acc, "msm_small");
-            k_set_identity<F><<<1, 32, 0, ms.acc>>>(out);
-        }
-        return check_launch(ctx, "k_set_identity");
-    }
+    if (n == 0) return launch(ctx, ms.acc, "msm_small", k_set_identity<F>, 1, 32, 0, out);
     if (n >= (1ull << 31)) return set_error(ctx, B200ZK_ERR_ARG, "MSM length must be < 2^31");
     // tab_c != 0: the bases are a fixed-base table of msm_table_windows(tab_c) x n points (section 7); all digit windows
     // then share one bucket set and the Horner chain disappears
@@ -746,14 +730,8 @@ static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, c
         // ---- digits + scan of part p on seq (its scalars may still be arriving) ----------------------------------------------
         if (P.scalars_ready) B2_CUDA_OK(ctx, cudaStreamWaitEvent(st, P.scalars_ready, 0));
         B2_CUDA_OK(ctx, cudaMemsetAsync(counts, 0, ((size_t)nb + 1) * 4, st));
-        {
-            LaunchScope ls(ctx, st, "msm_digits");
-            if (fold) k_msm_digits<<<(unsigned)((np + 255) / 256), 256, 0, st>>>(reinterpret_cast<const Fr*>(P.scalars), (uint32_t)np, c, W,
-                                                                               keys, ranks, counts);
-            else k_msm_digits_glv<<<(unsigned)((np + 255) / 256), 256, 0, st>>>(reinterpret_cast<const Fr*>(P.scalars), (uint32_t)np, c,
-                                                                                Wh, keys, ranks, counts);
-        }
-        B2_TRY(check_launch(ctx, "k_msm_digits"));
+        B2_TRY(launch(ctx, st, "msm_digits", fold ? k_msm_digits : k_msm_digits_glv, (unsigned)((np + 255) / 256), 256, 0,
+                      reinterpret_cast<const Fr*>(P.scalars), (uint32_t)np, c, fold ? W : Wh, keys, ranks, counts));
         B2_TRY(exclusive_scan(ctx, st, counts, offsets, sums, nb + 1));
         B2_CUDA_OK(ctx, cudaMemsetAsync(multi_all, 0, (size_t)ngroups * 8, st));          // [2 g], [2 g + 1] = big / small counts
         B2_CUDA_OK(ctx, cudaMemsetAsync(hist_all, 0, (size_t)ngroups * (MAX_TASK_LEN + 1) * 4, st));
@@ -767,37 +745,19 @@ static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, c
             uint32_t* task_rank = task_rank_all + G.task_base;
             uint32_t* order = order_all + G.task_base;
             uint32_t* hist = hist_all + (size_t)g * (MAX_TASK_LEN + 1);
-            {
-                LaunchScope ls(ctx, st, "msm_tasks");
-                k_msm_task_counts<<<(G.nbk + 1 + 255) / 256, 256, 0, st>>>(offsets + G.b0, G.nbk, task_len, ntasks);
-            }
-            B2_TRY(check_launch(ctx, "k_msm_task_counts"));
+            const unsigned task_grid = (unsigned)((G.task_cap + 255) / 256);
+            B2_TRY(launch(ctx, st, "msm_tasks", k_msm_task_counts, (G.nbk + 1 + 255) / 256, 256, 0, offsets + G.b0, G.nbk, task_len, ntasks));
             B2_TRY(exclusive_scan(ctx, st, ntasks, task_off, sums, G.nbk + 1));
-            {
-                LaunchScope ls(ctx, st, "msm_tasks");
-                k_msm_fill_tasks<<<(G.nbk + 255) / 256, 256, 0, st>>>(task_off, G.nbk, task_bucket, multi_all + G.list_base, G.list_cap,
-                                                                      multi_all + 2 * g);
-            }
-            B2_TRY(check_launch(ctx, "k_msm_fill_tasks"));
-            {
-                LaunchScope ls(ctx, st, "msm_tasks");
-                k_msm_task_hist<<<(unsigned)((G.task_cap + 255) / 256), 256, 0, st>>>(offsets + G.b0, task_off, task_bucket, G.nbk, task_len, hist, task_rank);
-            }
-            {
-                LaunchScope ls(ctx, st, "msm_tasks");
-                k_msm_task_hist_scan<<<1, 1, 0, st>>>(hist, task_len);
-            }
-            {
-                LaunchScope ls(ctx, st, "msm_tasks");
-                k_msm_task_order<<<(unsigned)((G.task_cap + 255) / 256), 256, 0, st>>>(offsets + G.b0, task_off, task_bucket, G.nbk, task_len, hist, task_rank, order);
-            }
-            B2_TRY(check_launch(ctx, "k_msm_task_order"));
-            {
-                const size_t t0 = fold ? 0 : (size_t)G.set0 * np, cnt = fold ? total : (size_t)G.nsets * np;
-                LaunchScope ls(ctx, st, "msm_scatter");
-                k_msm_scatter<<<(unsigned)((cnt + 255) / 256), 256, 0, st>>>(keys, ranks, offsets, (uint32_t)np, t0, cnt, fold ? 1u : 0u, entries);
-            }
-            B2_TRY(check_launch(ctx, "k_msm_scatter"));
+            B2_TRY(launch(ctx, st, "msm_tasks", k_msm_fill_tasks, (G.nbk + 255) / 256, 256, 0, task_off, G.nbk, task_bucket,
+                          multi_all + G.list_base, G.list_cap, multi_all + 2 * g));
+            B2_TRY(launch(ctx, st, "msm_tasks", k_msm_task_hist, task_grid, 256, 0, offsets + G.b0, task_off, task_bucket, G.nbk, task_len,
+                          hist, task_rank));
+            B2_TRY(launch(ctx, st, "msm_tasks", k_msm_task_hist_scan, 1, 1, 0, hist, task_len));
+            B2_TRY(launch(ctx, st, "msm_tasks", k_msm_task_order, task_grid, 256, 0, offsets + G.b0, task_off, task_bucket, G.nbk, task_len,
+                          hist, task_rank, order));
+            const size_t t0 = fold ? 0 : (size_t)G.set0 * np, cnt = fold ? total : (size_t)G.nsets * np;
+            B2_TRY(launch(ctx, st, "msm_scatter", k_msm_scatter, (unsigned)((cnt + 255) / 256), 256, 0, keys, ranks, offsets, (uint32_t)np, t0,
+                          cnt, fold ? 1u : 0u, entries));
             B2_CUDA_OK(ctx, cudaEventRecord(prepped[(size_t)p * ngroups + g], st));
         }
 
@@ -807,30 +767,17 @@ static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, c
         for (unsigned g = 0; g < ngroups; ++g) {
             const Group& G = groups[g];
             B2_CUDA_OK(ctx, cudaStreamWaitEvent(ast, prepped[(size_t)p * ngroups + g], 0));
-            {
-                LaunchScope ls(ctx, ast, acc_name);
-                const unsigned grid = (unsigned)((G.task_cap + 127) / 128);
-                const uint32_t wave = (uint32_t)ctx->sm_count * (sizeof(F) > 32 ? ACC_MINBLOCKS_G2 : ACC_MINBLOCKS);
-                const affine_t<F>* bp = reinterpret_cast<const affine_t<F>*>(P.bases);
-                if (rmw) k_msm_accumulate<F, true><<<grid, 128, 0, ast>>>(bp, entries, offsets + G.b0, task_off_all + G.b0 + g, task_bucket_all + G.task_base,
-                                                                       order_all + G.task_base, G.nbk, task_len, wave, buckets + G.b0, task_sums_all + G.task_base);
-                else k_msm_accumulate<F, false><<<grid, 128, 0, ast>>>(bp, entries, offsets + G.b0, task_off_all + G.b0 + g, task_bucket_all + G.task_base,
-                                                                        order_all + G.task_base, G.nbk, task_len, wave, buckets + G.b0, task_sums_all + G.task_base);
-            }
-            B2_TRY(check_launch(ctx, "k_msm_accumulate"));
+            const uint32_t wave = (uint32_t)ctx->sm_count * (sizeof(F) > 32 ? ACC_MINBLOCKS_G2 : ACC_MINBLOCKS);
+            B2_TRY(launch(ctx, ast, acc_name, rmw ? k_msm_accumulate<F, true> : k_msm_accumulate<F, false>,
+                          (unsigned)((G.task_cap + 127) / 128), 128, 0, reinterpret_cast<const affine_t<F>*>(P.bases), entries,
+                          offsets + G.b0, task_off_all + G.b0 + g, task_bucket_all + G.task_base, order_all + G.task_base, G.nbk,
+                          task_len, wave, buckets + G.b0, task_sums_all + G.task_base));
             if (rmw) {
                 // several parts: the next part's bucket kernel reads what this part's merges write, so they stay on `acc`
-                {
-                    LaunchScope ls(ctx, ast, "msm_merge");
-                    k_msm_merge_tasks<F><<<2 * ctx->sm_count, 128, 0, ast>>>(multi_all + G.list_base, multi_all + 2 * g, task_off_all + G.b0 + g,
-                                                                            task_sums_all + G.task_base, rmw, buckets + G.b0);
-                }
-                {
-                    LaunchScope ls(ctx, ast, "msm_merge");
-                    k_msm_merge_small<F><<<4 * ctx->sm_count, 128, 0, ast>>>(multi_all + G.list_base, G.list_cap, multi_all + 2 * g + 1,
-                                                                            task_off_all + G.b0 + g, task_sums_all + G.task_base, rmw, buckets + G.b0);
-                }
-                B2_TRY(check_launch(ctx, "k_msm_merge_tasks"));
+                B2_TRY(launch(ctx, ast, "msm_merge", k_msm_merge_tasks<F>, 2 * ctx->sm_count, 128, 0, multi_all + G.list_base, multi_all + 2 * g,
+                              task_off_all + G.b0 + g, task_sums_all + G.task_base, rmw, buckets + G.b0));
+                B2_TRY(launch(ctx, ast, "msm_merge", k_msm_merge_small<F>, 4 * ctx->sm_count, 128, 0, multi_all + G.list_base, G.list_cap,
+                              multi_all + 2 * g + 1, task_off_all + G.b0 + g, task_sums_all + G.task_base, rmw, buckets + G.b0));
             }
             B2_CUDA_OK(ctx, cudaEventRecord(accumulated[(size_t)p * ngroups + g], ast));
         }
@@ -843,42 +790,26 @@ static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, c
             uint32_t* multi_all = reinterpret_cast<uint32_t*>(ws + pw[0].multi);
             uint32_t* task_off = reinterpret_cast<uint32_t*>(ws + pw[0].taskoff) + G.b0 + g;
             xyzz_t<F>* task_sums = reinterpret_cast<xyzz_t<F>*>(ws + pw[0].tasksums) + G.task_base;
-            {
-                LaunchScope ls(ctx, st, "msm_merge");
-                k_msm_merge_tasks<F><<<2 * ctx->sm_count, 128, 0, st>>>(multi_all + G.list_base, multi_all + 2 * g, task_off, task_sums, 0u, buckets + G.b0);
-            }
-            {
-                LaunchScope ls(ctx, st, "msm_merge");
-                k_msm_merge_small<F><<<4 * ctx->sm_count, 128, 0, st>>>(multi_all + G.list_base, G.list_cap, multi_all + 2 * g + 1, task_off, task_sums,
-                                                                       0u, buckets + G.b0);
-            }
-            B2_TRY(check_launch(ctx, "k_msm_merge_tasks"));
+            B2_TRY(launch(ctx, st, "msm_merge", k_msm_merge_tasks<F>, 2 * ctx->sm_count, 128, 0, multi_all + G.list_base, multi_all + 2 * g,
+                          task_off, task_sums, 0u, buckets + G.b0));
+            B2_TRY(launch(ctx, st, "msm_merge", k_msm_merge_small<F>, 4 * ctx->sm_count, 128, 0, multi_all + G.list_base, G.list_cap,
+                          multi_all + 2 * g + 1, task_off, task_sums, 0u, buckets + G.b0));
         }
-        {
-            LaunchScope ls(ctx, st, "msm_reduce");
-            if (quad_reduce)                                       // latency-bound: fewer segments than the machine has warps
-                k_msm_reduce_segments_quad<F><<<(G.nsets * nseg * 4 + 127) / 128, 128, 0, st>>>(buckets + G.b0, G.nsets, B, seg_len,
-                                                                                               partials + (size_t)G.set0 * nseg);
-            else
-                k_msm_reduce_segments<F><<<(G.nsets * nseg + 127) / 128, 128, 0, st>>>(buckets + G.b0, G.nsets, B, seg_len,
-                                                                                      partials + (size_t)G.set0 * nseg);
-        }
-        B2_TRY(check_launch(ctx, "k_msm_reduce_segments"));
-        {
-            LaunchScope ls(ctx, st, "msm_window_sum");
-            constexpr int T = sizeof(F) > 32 ? 128 : 256;
-            // fold: the single bucket set's partials are summed by `wsplit` blocks, then added up by the Horner kernel
-            // with zero doublings per step
-            k_msm_window_sum<F, T><<<G.nsets * wsplit, T, 0, st>>>(partials + (size_t)G.set0 * nseg, nseg / wsplit, wsum + (size_t)G.set0 * wsplit);
-        }
-        B2_TRY(check_launch(ctx, "k_msm_window_sum"));
-        {
-            LaunchScope ls(ctx, st, "msm_combine");
-            const uint32_t first = g == 0, last = g + 1 == ngroups;
-            if (fold) k_msm_horner<F><<<1, 32, 0, st>>>(wsum, wsplit, 0u, first, last, hstate, out);
-            else k_msm_horner_glv<F><<<1, 32, 0, st>>>(wsum + G.set0, G.nsets / 2, c, first, last, hstate, out);
-        }
-        B2_TRY(check_launch(ctx, "k_msm_horner"));
+        xyzz_t<F>* group_partials = partials + (size_t)G.set0 * nseg;
+        if (quad_reduce)                                           // latency-bound: fewer segments than the machine has warps
+            B2_TRY(launch(ctx, st, "msm_reduce", k_msm_reduce_segments_quad<F>, (G.nsets * nseg * 4 + 127) / 128, 128, 0, buckets + G.b0,
+                          G.nsets, B, seg_len, group_partials));
+        else
+            B2_TRY(launch(ctx, st, "msm_reduce", k_msm_reduce_segments<F>, (G.nsets * nseg + 127) / 128, 128, 0, buckets + G.b0, G.nsets, B,
+                          seg_len, group_partials));
+        // fold: the single bucket set's partials are summed by `wsplit` blocks, then added up by the Horner kernel with zero
+        // doublings per step
+        constexpr int T = sizeof(F) > 32 ? 128 : 256;
+        B2_TRY(launch(ctx, st, "msm_window_sum", k_msm_window_sum<F, T>, G.nsets * wsplit, T, 0, group_partials, nseg / wsplit,
+                      wsum + (size_t)G.set0 * wsplit));
+        const uint32_t first = g == 0, last = g + 1 == ngroups;
+        if (fold) B2_TRY(launch(ctx, st, "msm_combine", k_msm_horner<F>, 1, 32, 0, wsum, wsplit, 0u, first, last, hstate, out));
+        else B2_TRY(launch(ctx, st, "msm_combine", k_msm_horner_glv<F>, 1, 32, 0, wsum + G.set0, G.nsets / 2, c, first, last, hstate, out));
     }
     return finish();
 }
@@ -953,12 +884,8 @@ static int table_build_impl(b200zk_ctx* ctx, cudaStream_t st, const void* d_base
     if (n == 0) return B200ZK_OK;
     const unsigned W = msm_table_windows(c);
     if ((uint64_t)W * n >= (1ull << 31)) return set_error(ctx, B200ZK_ERR_ARG, "table too large (W * n >= 2^31)");
-    {
-        LaunchScope ls(ctx, st, "msm_table_build");
-        k_msm_table_build<F><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(reinterpret_cast<const affine_t<F>*>(d_bases), (uint32_t)n,
-                                                                      c, W, reinterpret_cast<affine_t<F>*>(d_table));
-    }
-    return check_launch(ctx, "k_msm_table_build");
+    return launch(ctx, st, "msm_table_build", k_msm_table_build<F>, (unsigned)((n + 127) / 128), 128, 0,
+                  reinterpret_cast<const affine_t<F>*>(d_bases), (uint32_t)n, c, W, reinterpret_cast<affine_t<F>*>(d_table));
 }
 int msm_table_build_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_bases, size_t n, unsigned c, void* d_table) {
     return g2 ? table_build_impl<Fq2>(ctx, sl.stream, d_bases, n, c, d_table)
@@ -1000,23 +927,18 @@ __global__ void k_sum_xyzz(const xyzz_t<F>* pts, uint32_t count, uint32_t stride
     st16(out, acc);
 }
 int xyzz_sum_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_in, size_t count, size_t stride, void* d_out) {
-    {
-        LaunchScope ls(ctx, sl.stream, "point_sum");
-        if (g2) k_sum_xyzz<Fq2><<<1, 32, 0, sl.stream>>>((const xyzz_t<Fq2>*)d_in, (uint32_t)count, (uint32_t)stride, (xyzz_t<Fq2>*)d_out);
-        else k_sum_xyzz<Fq><<<1, 32, 0, sl.stream>>>((const xyzz_t<Fq>*)d_in, (uint32_t)count, (uint32_t)stride, (xyzz_t<Fq>*)d_out);
-    }
-    return check_launch(ctx, "k_sum_xyzz");
+    if (g2)
+        return launch(ctx, sl.stream, "point_sum", k_sum_xyzz<Fq2>, 1, 32, 0, (const xyzz_t<Fq2>*)d_in, (uint32_t)count, (uint32_t)stride,
+                      (xyzz_t<Fq2>*)d_out);
+    return launch(ctx, sl.stream, "point_sum", k_sum_xyzz<Fq>, 1, 32, 0, (const xyzz_t<Fq>*)d_in, (uint32_t)count, (uint32_t)stride,
+                  (xyzz_t<Fq>*)d_out);
 }
 
 template <class F>
 static int sum_impl(b200zk_ctx* ctx, Slot& sl, const void* d_xyzz, size_t count, void* d_out_affine) {
     affine_t<F>* out = reinterpret_cast<affine_t<F>*>(d_out_affine);
-    {
-        LaunchScope ls(ctx, sl.stream, "point_normalise");
-        k_sum_to_affine<F><<<1, 32, 0, sl.stream>>>(reinterpret_cast<const xyzz_t<F>*>(d_xyzz), (uint32_t)count, out,
-                                                     reinterpret_cast<uint64_t*>(out + 1));
-    }
-    return check_launch(ctx, "k_sum_to_affine");
+    return launch(ctx, sl.stream, "point_normalise", k_sum_to_affine<F>, 1, 32, 0, reinterpret_cast<const xyzz_t<F>*>(d_xyzz),
+                  (uint32_t)count, out, reinterpret_cast<uint64_t*>(out + 1));
 }
 int g1_sum_dev(b200zk_ctx* ctx, Slot& sl, const void* d, size_t count, void* d_out) { return sum_impl<Fq>(ctx, sl, d, count, d_out); }
 int g2_sum_dev(b200zk_ctx* ctx, Slot& sl, const void* d, size_t count, void* d_out) { return sum_impl<Fq2>(ctx, sl, d, count, d_out); }
@@ -1082,17 +1004,14 @@ int msm_exchange_sum_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_partia
     if (n_peers == 0 || n_peers > XCH_MAX_PEERS || rank >= n_peers || seq == 0) return set_error(ctx, B200ZK_ERR_ARG, "bad peer exchange geometry");
     PeerMailboxes pm;
     for (unsigned g = 0; g < XCH_MAX_PEERS; ++g) pm.box[g] = g < n_peers ? reinterpret_cast<char*>(peer_boxes[g]) : nullptr;
-    {
-        LaunchScope ls(ctx, sl.stream, "msm_exchange_sum");
-        if (g2) {
-            affine_t<Fq2>* o = reinterpret_cast<affine_t<Fq2>*>(d_out_affine);
-            k_msm_exchange_sum<Fq2><<<1, 32, 0, sl.stream>>>(reinterpret_cast<const xyzz_t<Fq2>*>(d_partial), pm, n_peers, rank, seq, o, reinterpret_cast<uint64_t*>(o + 1));
-        } else {
-            affine_t<Fq>* o = reinterpret_cast<affine_t<Fq>*>(d_out_affine);
-            k_msm_exchange_sum<Fq><<<1, 32, 0, sl.stream>>>(reinterpret_cast<const xyzz_t<Fq>*>(d_partial), pm, n_peers, rank, seq, o, reinterpret_cast<uint64_t*>(o + 1));
-        }
+    if (g2) {
+        affine_t<Fq2>* o = reinterpret_cast<affine_t<Fq2>*>(d_out_affine);
+        return launch(ctx, sl.stream, "msm_exchange_sum", k_msm_exchange_sum<Fq2>, 1, 32, 0, reinterpret_cast<const xyzz_t<Fq2>*>(d_partial),
+                      pm, n_peers, rank, seq, o, reinterpret_cast<uint64_t*>(o + 1));
     }
-    return check_launch(ctx, "k_msm_exchange_sum");
+    affine_t<Fq>* o = reinterpret_cast<affine_t<Fq>*>(d_out_affine);
+    return launch(ctx, sl.stream, "msm_exchange_sum", k_msm_exchange_sum<Fq>, 1, 32, 0, reinterpret_cast<const xyzz_t<Fq>*>(d_partial), pm,
+                  n_peers, rank, seq, o, reinterpret_cast<uint64_t*>(o + 1));
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1146,31 +1065,21 @@ __global__ void k_field_op(int op, const F* a, const F* b, F* out, size_t n) {
 
 int generate_points_dev(b200zk_ctx* ctx, Slot& sl, int g2, uint64_t seed, size_t n, void* d_out) {
     if (n == 0) return B200ZK_OK;
-    {
-        LaunchScope ls(ctx, sl.stream, "generate_points");
-        unsigned grid = (unsigned)((n + 127) / 128);
-        if (g2) k_generate_points<Fq2><<<grid, 128, 0, sl.stream>>>(seed, n, reinterpret_cast<affine_t<Fq2>*>(d_out));
-        else k_generate_points<Fq><<<grid, 128, 0, sl.stream>>>(seed, n, reinterpret_cast<affine_t<Fq>*>(d_out));
-    }
-    return check_launch(ctx, "k_generate_points");
+    const unsigned grid = (unsigned)((n + 127) / 128);
+    if (g2)
+        return launch(ctx, sl.stream, "generate_points", k_generate_points<Fq2>, grid, 128, 0, seed, n, reinterpret_cast<affine_t<Fq2>*>(d_out));
+    return launch(ctx, sl.stream, "generate_points", k_generate_points<Fq>, grid, 128, 0, seed, n, reinterpret_cast<affine_t<Fq>*>(d_out));
 }
 int generate_fr_dev(b200zk_ctx* ctx, Slot& sl, uint64_t seed, size_t n, void* d_out) {
     if (n == 0) return B200ZK_OK;
-    {
-        LaunchScope ls(ctx, sl.stream, "generate_fr");
-        k_generate_fr<<<(unsigned)((n + 255) / 256), 256, 0, sl.stream>>>(seed, n, reinterpret_cast<Fr*>(d_out));
-    }
-    return check_launch(ctx, "k_generate_fr");
+    return launch(ctx, sl.stream, "generate_fr", k_generate_fr, (unsigned)((n + 255) / 256), 256, 0, seed, n, reinterpret_cast<Fr*>(d_out));
 }
 int field_op_dev(b200zk_ctx* ctx, Slot& sl, int field, int op, const void* d_a, const void* d_b, void* d_out, size_t n) {
     if (n == 0) return B200ZK_OK;
-    {
-        LaunchScope ls(ctx, sl.stream, "field_op");
-        unsigned grid = (unsigned)((n + 255) / 256);
-        if (field == 0) k_field_op<Fq><<<grid, 256, 0, sl.stream>>>(op, (const Fq*)d_a, (const Fq*)d_b, (Fq*)d_out, n);
-        else k_field_op<Fr><<<grid, 256, 0, sl.stream>>>(op, (const Fr*)d_a, (const Fr*)d_b, (Fr*)d_out, n);
-    }
-    return check_launch(ctx, "k_field_op");
+    const unsigned grid = (unsigned)((n + 255) / 256);
+    if (field == 0)
+        return launch(ctx, sl.stream, "field_op", k_field_op<Fq>, grid, 256, 0, op, (const Fq*)d_a, (const Fq*)d_b, (Fq*)d_out, n);
+    return launch(ctx, sl.stream, "field_op", k_field_op<Fr>, grid, 256, 0, op, (const Fr*)d_a, (const Fr*)d_b, (Fr*)d_out, n);
 }
 
 }  // namespace b200zk

@@ -240,18 +240,11 @@ static int build_powtab(b200zk_ctx* ctx, cudaStream_t st, NttPlan* pl, const Fr*
     pl->allocs.push_back(lo);
     B2_CUDA_OK(ctx, cudaMalloc(&hi, sizeof(Fr) << hi_bits));
     pl->allocs.push_back(hi);
-    {
-        LaunchScope ls(ctx, st, "ntt_build_tables");
-        uint32_t cnt = 1u << lo_bits;
-        k_build_pow<<<(cnt + 127) / 128, 128, 0, st>>>(base, lo, cnt, 0);
-    }
-    {
-        LaunchScope ls(ctx, st, "ntt_build_tables");
-        uint32_t cnt = 1u << hi_bits;
-        k_build_pow<<<(cnt + 127) / 128, 128, 0, st>>>(base, hi, cnt, lo_bits);
-    }
+    const uint32_t n_lo = 1u << lo_bits, n_hi = 1u << hi_bits;
+    B2_TRY(launch(ctx, st, "ntt_build_tables", k_build_pow, (n_lo + 127) / 128, 128, 0, base, lo, n_lo, 0u, nullptr));
+    B2_TRY(launch(ctx, st, "ntt_build_tables", k_build_pow, (n_hi + 127) / 128, 128, 0, base, hi, n_hi, lo_bits, nullptr));
     out->lo = lo; out->hi = hi; out->lo_bits = lo_bits;
-    return check_launch(ctx, "k_build_pow");
+    return B200ZK_OK;
 }
 
 static int get_plan(b200zk_ctx* ctx, cudaStream_t st, unsigned log_n, bool inverse, NttPlan** out) {
@@ -268,19 +261,14 @@ static int get_plan(b200zk_ctx* ctx, cudaStream_t st, unsigned log_n, bool inver
     }
     B2_CUDA_OK(ctx, cudaMalloc(&pl->consts, 4 * sizeof(Fr)));
     pl->allocs.push_back(pl->consts);
-    {
-        LaunchScope ls(ctx, st, "ntt_build_tables");
-        k_plan_consts<<<1, 1, 0, st>>>(log_n, inverse ? 1 : 0, pl->consts);
-    }
-    B2_TRY(check_launch(ctx, "k_plan_consts"));
+    B2_TRY(launch(ctx, st, "ntt_build_tables", k_plan_consts, 1, 1, 0, log_n, inverse ? 1 : 0, pl->consts));
     for (unsigned i = 0; i < pl->npass; ++i) {
         uint32_t cnt = 1u << (pl->logR[i] - 1);
         B2_CUDA_OK(ctx, cudaMalloc(&pl->twR[i], sizeof(Fr) * cnt));
         pl->allocs.push_back(pl->twR[i]);
-        LaunchScope ls(ctx, st, "ntt_build_tables");
-        k_build_pow<<<(cnt + 127) / 128, 128, 0, st>>>(pl->consts, pl->twR[i], cnt, log_n - pl->logR[i]);
+        B2_TRY(launch(ctx, st, "ntt_build_tables", k_build_pow, (cnt + 127) / 128, 128, 0, pl->consts, pl->twR[i], cnt,
+                      log_n - pl->logR[i], nullptr));
     }
-    B2_TRY(check_launch(ctx, "k_build_pow(twR)"));
     B2_TRY(build_powtab(ctx, st, pl, pl->consts, log_n, &pl->tw));
     {
         unsigned logL = 0;
@@ -302,14 +290,11 @@ static int get_plan(b200zk_ctx* ctx, cudaStream_t st, unsigned log_n, bool inver
                     continue;
                 }
                 pl->allocs.push_back(t);
-                {
-                    LaunchScope ls(ctx, st, "ntt_build_tables");
-                    uint32_t cnt = 1u << range;
-                    const bool fold_scale = first_big && inverse;
-                    k_build_pow<<<(cnt + 127) / 128, 128, 0, st>>>(pl->consts, t, cnt, logL, fold_scale ? pl->consts + 1 : nullptr);
-                    if (fold_scale) pl->scale_folded = true;
-                }
-                B2_TRY(check_launch(ctx, "k_build_pow(tw_pass)"));
+                const uint32_t cnt = 1u << range;
+                const bool fold_scale = first_big && inverse;
+                B2_TRY(launch(ctx, st, "ntt_build_tables", k_build_pow, (cnt + 127) / 128, 128, 0, pl->consts, t, cnt, logL,
+                              fold_scale ? pl->consts + 1 : nullptr));
+                if (fold_scale) pl->scale_folded = true;
                 pl->tw_pass[i].lo = t; pl->tw_pass[i].hi = t; pl->tw_pass[i].lo_bits = range;
                 pl->has_tw_pass[i] = true;
             }
@@ -333,12 +318,8 @@ static int plan_lazy_tab(b200zk_ctx* ctx, cudaStream_t st, NttPlan* pl, int whic
         if (pl->log_n <= bigtab && cudaMalloc(&tab, sizeof(Fr) << pl->log_n) != cudaSuccess) { cudaGetLastError(); tab = nullptr; }
         if (tab) {
             pl->allocs.push_back(tab);
-            {
-                LaunchScope ls(ctx, st, "ntt_build_tables");
-                uint32_t cnt = 1u << pl->log_n;
-                k_build_pow<<<(cnt + 127) / 128, 128, 0, st>>>(pl->consts + which, tab, cnt, 0);
-            }
-            B2_TRY(check_launch(ctx, "k_build_pow(lazy)"));
+            const uint32_t cnt = 1u << pl->log_n;
+            B2_TRY(launch(ctx, st, "ntt_build_tables", k_build_pow, (cnt + 127) / 128, 128, 0, pl->consts + which, tab, cnt, 0u, nullptr));
             t->hi = tab; t->lo_bits = pl->log_n; t->lo = tab;
         } else {
             B2_TRY(build_powtab(ctx, st, pl, pl->consts + which, pl->log_n, t));
@@ -419,11 +400,7 @@ static int ntt_run(b200zk_ctx* ctx, Slot& sl, NttPlan* pl, const Fr* d_in, Fr* d
             smem = (size_t)(2 * RG + (1u << p.logR)) * sizeof(uint4);
             grid = dim3((unsigned)((size_t)1 << log_cols), batch >> LOG_G);
         }
-        {
-            LaunchScope ls(ctx, st, "ntt_pass");
-            k_ntt_pass<<<grid, threads, smem, st>>>(p);
-        }
-        B2_TRY(check_launch(ctx, "k_ntt_pass"));
+        B2_TRY(launch(ctx, st, "ntt_pass", k_ntt_pass, grid, threads, smem, p));
         if (bounce) B2_CUDA_OK(ctx, cudaMemcpyAsync(d_out, dst, bytes, cudaMemcpyDeviceToDevice, st));
         cur = dst;
         logL += pl->logR[i];
@@ -444,11 +421,7 @@ int ntt_dev(b200zk_ctx* ctx, Slot& sl, const Fr* d_in, Fr* d_out, unsigned log_n
 
 int bitrev_dev(b200zk_ctx* ctx, Slot& sl, const Fr* d_in, Fr* d_out, unsigned log_n) {
     size_t n = (size_t)1 << log_n;
-    {
-        LaunchScope ls(ctx, sl.stream, "bitrev");
-        k_bitrev<<<(unsigned)((n + 255) / 256), 256, 0, sl.stream>>>(d_in, d_out, log_n);
-    }
-    return check_launch(ctx, "k_bitrev");
+    return launch(ctx, sl.stream, "bitrev", k_bitrev, (unsigned)((n + 255) / 256), 256, 0, d_in, d_out, log_n);
 }
 
 // h = (NTT(shift(iNTT a)) * NTT(shift(iNTT b))) - NTT(shift(iNTT c)),  shift: coeff j *= w_2m^j
@@ -475,11 +448,7 @@ int h_circom_dev(b200zk_ctx* ctx, Slot& sl, const Fr* d_a, const Fr* d_b, const 
         B2_TRY(ntt_run(ctx, sl, inv, buf0, buf1, 3, nullptr, shift, inv->consts + 1));
         B2_TRY(ntt_run(ctx, sl, fwd, buf1, buf1, 3, nullptr, nullptr, nullptr));
     }
-    {
-        LaunchScope ls(ctx, st, "h_pointwise");
-        k_h_pointwise<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(buf1, buf1 + m, buf1 + 2 * m, d_h, m);
-    }
-    return check_launch(ctx, "k_h_pointwise");
+    return launch(ctx, st, "h_pointwise", k_h_pointwise, (unsigned)((m + 255) / 256), 256, 0, buf1, buf1 + m, buf1 + 2 * m, d_h, m);
 }
 
 // Batched transform of size 2^log_t over `batch` contiguous vectors with a per-batch post factor
@@ -556,11 +525,7 @@ int fourstep_cols_p2p_dev(b200zk_ctx* ctx, Slot& sl, const Fr* d_in, void* const
 // out[i] = a[i]*b[i] - c[i]   (ext_wit.rs:88-92 on device-resident vectors)
 int mul_sub_dev(b200zk_ctx* ctx, Slot& sl, const Fr* a, const Fr* b, const Fr* c, Fr* out, size_t n) {
     if (n == 0) return B200ZK_OK;
-    {
-        LaunchScope ls(ctx, sl.stream, "h_pointwise");
-        k_h_pointwise<<<(unsigned)((n + 255) / 256), 256, 0, sl.stream>>>(a, b, c, out, n);
-    }
-    return check_launch(ctx, "k_h_pointwise");
+    return launch(ctx, sl.stream, "h_pointwise", k_h_pointwise, (unsigned)((n + 255) / 256), 256, 0, a, b, c, out, n);
 }
 
 }  // namespace b200zk

@@ -33,16 +33,13 @@ int points_matmul_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_points, s
     if (l == 0 || l > 1024 || rows > 4096 || n_chunks * rows >= (1ull << 32))
         return set_error(ctx, B200ZK_ERR_ARG, "points_matmul: need 1 <= l <= 1024, rows <= 4096, n_chunks * rows < 2^32");
     unsigned grid = (unsigned)((n_chunks * rows + 127) / 128);
-    {
-        LaunchScope ls(ctx, sl.stream, "points_matmul");
-        if (g2) k_points_matmul<Fq2><<<grid, 128, 0, sl.stream>>>(reinterpret_cast<const affine_t<Fq2>*>(d_points), (uint32_t)n_chunks,
-                                                                  (uint32_t)l, reinterpret_cast<const Fr*>(d_matrix), (uint32_t)rows,
-                                                                  reinterpret_cast<affine_t<Fq2>*>(d_out));
-        else k_points_matmul<Fq><<<grid, 128, 0, sl.stream>>>(reinterpret_cast<const affine_t<Fq>*>(d_points), (uint32_t)n_chunks,
-                                                              (uint32_t)l, reinterpret_cast<const Fr*>(d_matrix), (uint32_t)rows,
-                                                              reinterpret_cast<affine_t<Fq>*>(d_out));
-    }
-    return check_launch(ctx, "k_points_matmul");
+    if (g2)
+        return launch(ctx, sl.stream, "points_matmul", k_points_matmul<Fq2>, grid, 128, 0, reinterpret_cast<const affine_t<Fq2>*>(d_points),
+                      (uint32_t)n_chunks, (uint32_t)l, reinterpret_cast<const Fr*>(d_matrix), (uint32_t)rows,
+                      reinterpret_cast<affine_t<Fq2>*>(d_out));
+    return launch(ctx, sl.stream, "points_matmul", k_points_matmul<Fq>, grid, 128, 0, reinterpret_cast<const affine_t<Fq>*>(d_points),
+                  (uint32_t)n_chunks, (uint32_t)l, reinterpret_cast<const Fr*>(d_matrix), (uint32_t)rows,
+                  reinterpret_cast<affine_t<Fq>*>(d_out));
 }
 
 }  // namespace b200zk

@@ -99,55 +99,94 @@ __global__ void __launch_bounds__(96) k_prove_finalize(FinalizeArgs f) {
     compress_g1(C, f.out + 96);
 }
 
-void pk_free_tables(b200zk_pk* pk) {
+static void free_tables(void* tab[5], unsigned tab_c[5], size_t* bytes) {
     for (int k = 0; k < 5; ++k) {
-        if (pk->tab[k]) cudaFree(pk->tab[k]);
-        pk->tab[k] = nullptr;
-        pk->tab_c[k] = 0;
+        if (tab[k]) cudaFree(tab[k]);
+        tab[k] = nullptr;
+        tab_c[k] = 0;
     }
-    pk->tab_bytes = 0;
+    *bytes = 0;
 }
 
-// Window tables for the five query vectors (msm.cu section 7).  c = 0: msm_table_auto_window(n) per query
-// (B200ZK_PK_TABLE_WINDOW overrides).  Skipped as a whole -- the generic MSM keeps running on the queries -- when
-// the tables would exceed B200ZK_PK_TABLE_MAX_GB (default: 60% of the free HBM) or the allocation fails.
-int pk_precompute_dev(b200zk_ctx* ctx, b200zk_pk* pk, unsigned c_req) {
-    pk_free_tables(pk);
-    Slot& sl = ctx->slots[0];
-    const size_t n1 = pk->n_vars - 1, n_aux = pk->n_vars - pk->n_inputs;
-    const void* src[5] = {(const char*)pk->a_query + 64, (const char*)pk->b_g1_query + 64, (const char*)pk->b_g2_query + 128,
-                          pk->l_query, pk->h_query};
-    const size_t cnt[5] = {n1, n1, n1, n_aux, pk->m};
-    const size_t psz[5] = {64, 64, 128, 64, 64};
-    if (const char* env = getenv("B200ZK_PK_TABLE_WINDOW")) { int v = atoi(env); if (v >= 2 && v <= 24) c_req = (unsigned)v; }
+void pk_free_tables(b200zk_pk* pk) { free_tables(pk->tab, pk->tab_c, &pk->tab_bytes); }
+
+bool pk_tables_enabled() {
+    const char* env = getenv("B200ZK_PK_TABLES");
+    return !(env && env[0] == '0');
+}
+
+int pk_tables_build(b200zk_ctx* ctx, Slot& sl, const void* const src[5], const size_t cnt[5], unsigned c_req, void* tab[5],
+                    unsigned tab_c[5], size_t* bytes) {
+    for (int k = 0; k < 5; ++k) { tab[k] = nullptr; tab_c[k] = 0; }
+    *bytes = 0;
     // budget: B200ZK_PK_TABLE_MAX_GB, else 60% of the HBM that is free right now (2^24 constraints: 84 GB of tables)
     double max_gb = 48.0;
     size_t free_b = 0, total_b = 0;
     if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess) max_gb = 0.6 * (double)free_b / 1073741824.0;
     if (const char* env = getenv("B200ZK_PK_TABLE_MAX_GB")) max_gb = atof(env);
     unsigned cs[5];
-    size_t total = 0;
+    size_t size[5], total = 0;
     for (int k = 0; k < 5; ++k) {
         cs[k] = c_req ? c_req : msm_table_auto_window(cnt[k]);
-        const unsigned c = cs[k];
-        if ((uint64_t)msm_table_windows(c) * cnt[k] >= (1ull << 31)) return B200ZK_OK;       // generic path keeps working
-        total += (size_t)msm_table_windows(c) * cnt[k] * psz[k];
+        const uint64_t entries = (uint64_t)msm_table_windows(cs[k]) * cnt[k];
+        if (entries >= (1ull << 31)) return B200ZK_OK;                    // generic path keeps working
+        size[k] = (size_t)entries * (k == 2 ? 128 : 64);
+        total += size[k];
     }
     if ((double)total > max_gb * 1073741824.0) return B200ZK_OK;
     for (int k = 0; k < 5; ++k) {
         if (cnt[k] < 64) continue;                   // tiny query: nothing to gain
-        size_t bytes = (size_t)msm_table_windows(cs[k]) * cnt[k] * psz[k];
-        if (cudaMalloc(&pk->tab[k], bytes) != cudaSuccess) {
+        if (cudaMalloc(&tab[k], size[k]) != cudaSuccess) {
             cudaGetLastError();
-            pk->tab[k] = nullptr;
-            pk_free_tables(pk);
+            tab[k] = nullptr;
+            free_tables(tab, tab_c, bytes);
             return B200ZK_OK;
         }
-        int rc = msm_table_build_dev(ctx, sl, k == 2, src[k], cnt[k], cs[k], pk->tab[k]);
-        if (rc) { pk_free_tables(pk); return rc; }
-        pk->tab_c[k] = cs[k];
-        pk->tab_bytes += bytes;
+        const int rc = msm_table_build_dev(ctx, sl, k == 2, src[k], cnt[k], cs[k], tab[k]);
+        if (rc) { free_tables(tab, tab_c, bytes); return rc; }
+        tab_c[k] = cs[k];
+        *bytes += size[k];
     }
+    return B200ZK_OK;
+}
+
+int query_msm(b200zk_ctx* ctx, Slot& sl, int k, const void* query, void* const tab[5], const unsigned tab_c[5], const Fr* scalars,
+              size_t n, void* out) {
+    if (tab_c[k]) return msm_table_dev(ctx, sl, k == 2, tab[k], scalars, n, tab_c[k], out);
+    return k == 2 ? msm_g2_dev(ctx, sl, query, scalars, n, out) : msm_g1_dev(ctx, sl, query, scalars, n, out);
+}
+
+// c = 0: msm_table_auto_window(n) per query (B200ZK_PK_TABLE_WINDOW overrides)
+int pk_precompute_dev(b200zk_ctx* ctx, b200zk_pk* pk, unsigned c_req) {
+    pk_free_tables(pk);
+    Slot& sl = ctx->slots[0];
+    const size_t n1 = pk->n_vars - 1;
+    const void* src[5] = {(const char*)pk->a_query + 64, (const char*)pk->b_g1_query + 64, (const char*)pk->b_g2_query + 128,
+                          pk->l_query, pk->h_query};
+    const size_t cnt[5] = {n1, n1, n1, pk->n_vars - pk->n_inputs, pk->m};
+    if (const char* env = getenv("B200ZK_PK_TABLE_WINDOW")) { int v = atoi(env); if (v >= 2 && v <= 24) c_req = (unsigned)v; }
+    B2_TRY(pk_tables_build(ctx, sl, src, cnt, c_req, pk->tab, pk->tab_c, &pk->tab_bytes));
+    B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
+    return B200ZK_OK;
+}
+
+// Slot::small of prove_dev and assemble_dev: r, s (Montgomery) at SMALL_RS, uploaded by the caller; the proof at SMALL_PROOF
+static const size_t SMALL_RS = 768, SMALL_PROOF = 832;
+
+// k_prove_finalize over the five MSM partials (msm_b1 may be null) and the key's query[0] points and vk on sl's stream, then
+// the 128 proof bytes to the host
+static int finalize_dev(b200zk_ctx* ctx, Slot& sl, const b200zk_pk* pk, const void* msm_a, const void* msm_b2, const void* msm_l,
+                        const void* msm_h, const void* msm_b1, int add_zero_terms, uint8_t proof_out[128]) {
+    char* sm = reinterpret_cast<char*>(sl.small.p);
+    FinalizeArgs f;
+    f.msm_a = msm_a; f.msm_b2 = msm_b2; f.msm_l = msm_l; f.msm_h = msm_h; f.msm_b1 = msm_b1;
+    f.a0 = pk->a_query; f.b1_0 = pk->b_g1_query; f.b2_0 = pk->b_g2_query;
+    f.vk = pk->vk;
+    f.rs = reinterpret_cast<const Fr*>(sm + SMALL_RS);
+    f.out = reinterpret_cast<uint8_t*>(sm + SMALL_PROOF);
+    f.add_zero_terms = add_zero_terms;
+    B2_TRY(launch(ctx, sl.stream, "prove_finalize", k_prove_finalize, 1, 96, 0, f));
+    B2_CUDA_OK(ctx, cudaMemcpyAsync(proof_out, sm + SMALL_PROOF, 128, cudaMemcpyDeviceToHost, sl.stream));
     B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
     return B200ZK_OK;
 }
@@ -167,13 +206,13 @@ int prove_dev(b200zk_ctx* ctx, const b200zk_pk* pk, const Fr* d_z, const Fr* d_a
     bool need_b1 = r_nonzero || mirror_bg1;
 
     // small device block: 5 partials (3 G1 + 1 G2 + 1 G1) + r,s + 128-byte proof, then the h vector
-    const size_t o_a = 0, o_l = 128, o_h = 256, o_b1 = 384, o_b2 = 512, o_rs = 768, o_out = 832, o_hvec = 1024;
+    const size_t o_a = 0, o_l = 128, o_h = 256, o_b1 = 384, o_b2 = 512, o_hvec = 1024;
     B2_CUDA_OK(ctx, s0.small.reserve(o_hvec + m * sizeof(Fr)));
     char* sm = reinterpret_cast<char*>(s0.small.p);
     Fr* d_h = reinterpret_cast<Fr*>(sm + o_hvec);
     uint64_t rs_host[8];
     memcpy(rs_host, r, 32); memcpy(rs_host + 4, s, 32);
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(sm + o_rs, rs_host, 64, cudaMemcpyHostToDevice, st));
+    B2_CUDA_OK(ctx, cudaMemcpyAsync(sm + SMALL_RS, rs_host, 64, cudaMemcpyHostToDevice, st));
 
     // inputs (z, a, b, c) were produced on slot 0's stream: the other slots wait for them
     cudaEvent_t ev_in, ev1, ev2;
@@ -197,47 +236,21 @@ int prove_dev(b200zk_ctx* ctx, const b200zk_pk* pk, const Fr* d_z, const Fr* d_a
     // and the reductions then compete with the bucket kernels (tools/prove_timeline.py).
     ctx->msm_seg_hint = 32;            // bucket reduction in 32-bucket segments: 21% fewer group operations than 16, and
                                        // its longer dependency chains are hidden by the concurrent MSMs
-    auto msm = [&](Slot& sl, int k, int g2, const void* query, const Fr* scalars, size_t n, void* out) -> int {
-        if (pk->tab_c[k]) return msm_table_dev(ctx, sl, g2, pk->tab[k], scalars, n, pk->tab_c[k], out);
-        return g2 ? msm_g2_dev(ctx, sl, query, scalars, n, out) : msm_g1_dev(ctx, sl, query, scalars, n, out);
-    };
-    int rc = msm(s1, 2, 1, b2q + 128, d_z + 1, n1, sm + o_b2);
-    if (!rc) rc = msm(s2, 0, 0, aq + 64, d_z + 1, n1, sm + o_a);
-    if (!rc) rc = msm(s2, 3, 0, pk->l_query, d_z + pk->n_inputs, n_aux, sm + o_l);
-    if (!rc && need_b1) rc = msm(s2, 1, 0, b1q + 64, d_z + 1, n1, sm + o_b1);
+    int rc = query_msm(ctx, s1, 2, b2q + 128, pk->tab, pk->tab_c, d_z + 1, n1, sm + o_b2);
+    if (!rc) rc = query_msm(ctx, s2, 0, aq + 64, pk->tab, pk->tab_c, d_z + 1, n1, sm + o_a);
+    if (!rc) rc = query_msm(ctx, s2, 3, pk->l_query, pk->tab, pk->tab_c, d_z + pk->n_inputs, n_aux, sm + o_l);
+    if (!rc && need_b1) rc = query_msm(ctx, s2, 1, b1q + 64, pk->tab, pk->tab_c, d_z + 1, n1, sm + o_b1);
     if (!rc) rc = h_circom_dev(ctx, s0, d_a, d_b, d_c, log_m, d_h);
-    if (!rc) rc = msm(s0, 4, 0, pk->h_query, d_h, m, sm + o_h);
+    if (!rc) rc = query_msm(ctx, s0, 4, pk->h_query, pk->tab, pk->tab_c, d_h, m, sm + o_h);
     cudaEventRecord(ev1, s1.stream);
     cudaEventRecord(ev2, s2.stream);
     cudaStreamWaitEvent(st, ev1, 0);
     cudaStreamWaitEvent(st, ev2, 0);
     ctx->msm_seg_hint = 0;
-    if (rc) {
-        cudaStreamSynchronize(st);
-        cudaEventDestroy(ev_in); cudaEventDestroy(ev1); cudaEventDestroy(ev2);
-        return rc;
-    }
-
-    FinalizeArgs f;
-    f.msm_a = sm + o_a; f.msm_b2 = sm + o_b2; f.msm_l = sm + o_l; f.msm_h = sm + o_h;
-    f.msm_b1 = need_b1 ? sm + o_b1 : nullptr;
-    f.a0 = aq; f.b1_0 = b1q; f.b2_0 = b2q;
-    f.vk = pk->vk;
-    f.rs = reinterpret_cast<const Fr*>(sm + o_rs);
-    f.out = reinterpret_cast<uint8_t*>(sm + o_out);
-    f.add_zero_terms = 1;
-    {
-        LaunchScope ls(ctx, st, "prove_finalize");
-        k_prove_finalize<<<1, 96, 0, st>>>(f);
-    }
-    rc = check_launch(ctx, "k_prove_finalize");
-    cudaError_t e1 = cudaMemcpyAsync(proof_out, sm + o_out, 128, cudaMemcpyDeviceToHost, st);
-    cudaError_t e2 = cudaStreamSynchronize(st);
+    if (!rc) rc = finalize_dev(ctx, s0, pk, sm + o_a, sm + o_b2, sm + o_l, sm + o_h, need_b1 ? sm + o_b1 : nullptr, 1, proof_out);
+    if (rc) cudaStreamSynchronize(st);
     cudaEventDestroy(ev_in); cudaEventDestroy(ev1); cudaEventDestroy(ev2);
-    if (rc) return rc;
-    B2_CUDA_OK(ctx, e1);
-    B2_CUDA_OK(ctx, e2);
-    return B200ZK_OK;
+    return rc;
 }
 
 // Final assembly from externally combined MSM results (multi-GPU prove: every rank contributes partial sums,
@@ -246,29 +259,13 @@ int prove_dev(b200zk_ctx* ctx, const b200zk_pk* pk, const Fr* d_z, const Fr* d_a
 int assemble_dev(b200zk_ctx* ctx, Slot& sl, const b200zk_pk* pk, const void* msm_a, const void* msm_b2, const void* msm_l,
                  const void* msm_h, const void* msm_b1, const uint64_t r[4], const uint64_t s[4], int include_zero_terms,
                  uint8_t proof_out[128]) {
-    cudaStream_t st = sl.stream;
     bool r_nonzero = (r[0] | r[1] | r[2] | r[3]) != 0;
     if (r_nonzero && !msm_b1) return set_error(ctx, B200ZK_ERR_ARG, "r != 0 needs the b_g1_query MSM");
     B2_CUDA_OK(ctx, sl.small.reserve(1024));
-    char* sm = reinterpret_cast<char*>(sl.small.p);
     uint64_t rs_host[8];
     memcpy(rs_host, r, 32); memcpy(rs_host + 4, s, 32);
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(sm + 768, rs_host, 64, cudaMemcpyHostToDevice, st));
-    FinalizeArgs f;
-    f.msm_a = msm_a; f.msm_b2 = msm_b2; f.msm_l = msm_l; f.msm_h = msm_h; f.msm_b1 = msm_b1;
-    f.a0 = pk->a_query; f.b1_0 = pk->b_g1_query; f.b2_0 = pk->b_g2_query;
-    f.vk = pk->vk;
-    f.rs = reinterpret_cast<const Fr*>(sm + 768);
-    f.out = reinterpret_cast<uint8_t*>(sm + 832);
-    f.add_zero_terms = include_zero_terms;
-    {
-        LaunchScope ls(ctx, st, "prove_finalize");
-        k_prove_finalize<<<1, 96, 0, st>>>(f);
-    }
-    B2_TRY(check_launch(ctx, "k_prove_finalize"));
-    B2_CUDA_OK(ctx, cudaMemcpyAsync(proof_out, sm + 832, 128, cudaMemcpyDeviceToHost, st));
-    B2_CUDA_OK(ctx, cudaStreamSynchronize(st));
-    return B200ZK_OK;
+    B2_CUDA_OK(ctx, cudaMemcpyAsync(reinterpret_cast<char*>(sl.small.p) + SMALL_RS, rs_host, 64, cudaMemcpyHostToDevice, sl.stream));
+    return finalize_dev(ctx, sl, pk, msm_a, msm_b2, msm_l, msm_h, msm_b1, include_zero_terms, proof_out);
 }
 
 }  // namespace b200zk

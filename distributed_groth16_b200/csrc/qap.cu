@@ -76,11 +76,8 @@ __global__ void __launch_bounds__(256) k_qap_warp(const uint32_t* a_ptr, const u
 
 int fr_convert_dev(b200zk_ctx* ctx, Slot& sl, const void* d_in, void* d_out, size_t n, int to_mont, int times) {
     if (n == 0) return B200ZK_OK;
-    {
-        LaunchScope ls(ctx, sl.stream, "fr_convert");
-        k_fr_convert<<<(unsigned)((n + 255) / 256), 256, 0, sl.stream>>>((const Fr*)d_in, (Fr*)d_out, n, to_mont, times);
-    }
-    return check_launch(ctx, "k_fr_convert");
+    return launch(ctx, sl.stream, "fr_convert", k_fr_convert, (unsigned)((n + 255) / 256), 256, 0, (const Fr*)d_in, (Fr*)d_out, n, to_mont,
+                  times);
 }
 
 int qap_dev(b200zk_ctx* ctx, Slot& sl, const void* a_ptr, const void* a_col, const void* a_val, const void* b_ptr,
@@ -89,17 +86,11 @@ int qap_dev(b200zk_ctx* ctx, Slot& sl, const void* a_ptr, const void* a_col, con
     if (log_m > 28) return set_error(ctx, B200ZK_ERR_DOMAIN, "domain too large (PolynomialDegreeTooLarge)");
     size_t m = (size_t)1 << log_m;
     if (nc + n_inputs > m) return set_error(ctx, B200ZK_ERR_DOMAIN, "num_constraints + num_inputs exceeds the domain size");
-    {
-        LaunchScope ls(ctx, sl.stream, "qap_matvec");
-        const uint32_t *ap = (const uint32_t*)a_ptr, *ac = (const uint32_t*)a_col, *bp = (const uint32_t*)b_ptr, *bc = (const uint32_t*)b_col;
-        if (m <= ((size_t)1 << 18))          // warp per row while rows x 32 lanes still fit a few waves
-            k_qap_warp<<<(unsigned)((m * 32 + 255) / 256), 256, 0, sl.stream>>>(ap, ac, (const Fr*)a_val, bp, bc, (const Fr*)b_val, (const Fr*)d_z,
-                                                                                (uint32_t)nc, (uint32_t)n_inputs, (uint32_t)m, (Fr*)d_a, (Fr*)d_b, (Fr*)d_c);
-        else
-            k_qap<<<(unsigned)((m + 127) / 128), 128, 0, sl.stream>>>(ap, ac, (const Fr*)a_val, bp, bc, (const Fr*)b_val, (const Fr*)d_z,
-                                                                       (uint32_t)nc, (uint32_t)n_inputs, (uint32_t)m, (Fr*)d_a, (Fr*)d_b, (Fr*)d_c);
-    }
-    return check_launch(ctx, "k_qap");
+    const uint32_t *ap = (const uint32_t*)a_ptr, *ac = (const uint32_t*)a_col, *bp = (const uint32_t*)b_ptr, *bc = (const uint32_t*)b_col;
+    const bool warp = m <= ((size_t)1 << 18);          // warp per row while rows x 32 lanes still fit a few waves
+    return launch(ctx, sl.stream, "qap_matvec", warp ? k_qap_warp : k_qap, (unsigned)(warp ? (m * 32 + 255) / 256 : (m + 127) / 128),
+                  warp ? 256 : 128, 0, ap, ac, (const Fr*)a_val, bp, bc, (const Fr*)b_val, (const Fr*)d_z, (uint32_t)nc,
+                  (uint32_t)n_inputs, (uint32_t)m, (Fr*)d_a, (Fr*)d_b, (Fr*)d_c);
 }
 
 // R1CS satisfaction (snarkjs `wtns check`): constraint i holds iff <A_i, w> <B_i, w> = <C_i, w>.  The same mat-vec as k_qap
@@ -145,14 +136,10 @@ int r1cs_check_dev(b200zk_ctx* ctx, Slot& sl, const void* const ptr[3], const vo
     unsigned long long* bad = reinterpret_cast<unsigned long long*>(sl.small.p);
     B2_CUDA_OK(ctx, cudaMemsetAsync(bad, 0, 8, sl.stream));
     B2_CUDA_OK(ctx, cudaMemsetAsync(bad + 1, 0xFF, 8, sl.stream));
-    {
-        LaunchScope ls(ctx, sl.stream, "r1cs_check");
-        if (nc <= ((size_t)1 << 18))           // the warp-per-row rule of qap_dev
-            k_r1cs_check_warp<<<(unsigned)((nc * 32 + 255) / 256), 256, 0, sl.stream>>>(m[0], m[1], m[2], (const Fr*)d_w, (uint32_t)nc, bad);
-        else
-            k_r1cs_check<<<(unsigned)((nc + 127) / 128), 128, 0, sl.stream>>>(m[0], m[1], m[2], (const Fr*)d_w, (uint32_t)nc, bad);
-    }
-    B2_TRY(check_launch(ctx, "k_r1cs_check"));
+    const bool warp = nc <= ((size_t)1 << 18);          // the warp-per-row rule of qap_dev
+    B2_TRY(launch(ctx, sl.stream, "r1cs_check", warp ? k_r1cs_check_warp : k_r1cs_check,
+                  (unsigned)(warp ? (nc * 32 + 255) / 256 : (nc + 127) / 128), warp ? 256 : 128, 0, m[0], m[1], m[2], (const Fr*)d_w,
+                  (uint32_t)nc, bad));
     unsigned long long h_bad[2] = {0, 0};
     B2_CUDA_OK(ctx, cudaMemcpyAsync(h_bad, bad, 16, cudaMemcpyDeviceToHost, sl.stream));
     B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));

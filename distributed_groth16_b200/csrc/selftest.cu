@@ -260,24 +260,27 @@ static int arith_launch(b200zk_ctx* ctx, Slot& sl, int op, const uint64_t* d_in,
     const unsigned grid1 = (unsigned)((n + ARITH_BLOCK - 1) / ARITH_BLOCK);
     const unsigned grid4 = (unsigned)((4 * n + ARITH_BLOCK - 1) / ARITH_BLOCK);
     const unsigned grid32 = (unsigned)((32 * n + ARITH_BLOCK - 1) / ARITH_BLOCK);
-    LaunchScope ls(ctx, sl.stream, "arith");
+    const cudaStream_t st = sl.stream;
     switch (op) {
 #define B2_ARITH_CASE(OP, IN, OUT) \
-        case OP: k_arith<OP><<<grid1, ARITH_BLOCK, 0, sl.stream>>>(d_in, d_out, n, in_w, out_w); break;
+        case OP: return launch(ctx, st, "arith", k_arith<OP>, grid1, ARITH_BLOCK, 0, d_in, d_out, n, in_w, out_w);
         B2_ARITH_OPS(B2_ARITH_CASE)
 #undef B2_ARITH_CASE
-        case ARITH_FR_ROOT: k_arith_fr_root<<<grid1, ARITH_BLOCK, 0, sl.stream>>>(d_in, d_out, n); break;
-        case ARITH_G1 + EC_QUAD_ADD: k_arith_quad<Fq, false, false><<<grid4, ARITH_BLOCK, 0, sl.stream>>>(d_in, d_out, n); break;
-        case ARITH_G1 + EC_QUAD_DBL: k_arith_quad<Fq, false, true><<<grid4, ARITH_BLOCK, 0, sl.stream>>>(d_in, d_out, n); break;
-        case ARITH_G1 + EC_QUAD_ADD_FULLWARP: k_arith_quad<Fq, true, false><<<grid32, ARITH_BLOCK, 0, sl.stream>>>(d_in, d_out, n); break;
-        case ARITH_G1 + EC_QUAD_DBL_FULLWARP: k_arith_quad<Fq, true, true><<<grid32, ARITH_BLOCK, 0, sl.stream>>>(d_in, d_out, n); break;
-        case ARITH_G2 + EC_QUAD_ADD: k_arith_quad<Fq2, false, false><<<grid4, ARITH_BLOCK, 0, sl.stream>>>(d_in, d_out, n); break;
-        case ARITH_G2 + EC_QUAD_DBL: k_arith_quad<Fq2, false, true><<<grid4, ARITH_BLOCK, 0, sl.stream>>>(d_in, d_out, n); break;
-        case ARITH_G2 + EC_QUAD_ADD_FULLWARP: k_arith_quad<Fq2, true, false><<<grid32, ARITH_BLOCK, 0, sl.stream>>>(d_in, d_out, n); break;
-        case ARITH_G2 + EC_QUAD_DBL_FULLWARP: k_arith_quad<Fq2, true, true><<<grid32, ARITH_BLOCK, 0, sl.stream>>>(d_in, d_out, n); break;
+        case ARITH_FR_ROOT: return launch(ctx, st, "arith", k_arith_fr_root, grid1, ARITH_BLOCK, 0, d_in, d_out, n);
+        case ARITH_G1 + EC_QUAD_ADD: return launch(ctx, st, "arith", k_arith_quad<Fq, false, false>, grid4, ARITH_BLOCK, 0, d_in, d_out, n);
+        case ARITH_G1 + EC_QUAD_DBL: return launch(ctx, st, "arith", k_arith_quad<Fq, false, true>, grid4, ARITH_BLOCK, 0, d_in, d_out, n);
+        case ARITH_G1 + EC_QUAD_ADD_FULLWARP:
+            return launch(ctx, st, "arith", k_arith_quad<Fq, true, false>, grid32, ARITH_BLOCK, 0, d_in, d_out, n);
+        case ARITH_G1 + EC_QUAD_DBL_FULLWARP:
+            return launch(ctx, st, "arith", k_arith_quad<Fq, true, true>, grid32, ARITH_BLOCK, 0, d_in, d_out, n);
+        case ARITH_G2 + EC_QUAD_ADD: return launch(ctx, st, "arith", k_arith_quad<Fq2, false, false>, grid4, ARITH_BLOCK, 0, d_in, d_out, n);
+        case ARITH_G2 + EC_QUAD_DBL: return launch(ctx, st, "arith", k_arith_quad<Fq2, false, true>, grid4, ARITH_BLOCK, 0, d_in, d_out, n);
+        case ARITH_G2 + EC_QUAD_ADD_FULLWARP:
+            return launch(ctx, st, "arith", k_arith_quad<Fq2, true, false>, grid32, ARITH_BLOCK, 0, d_in, d_out, n);
+        case ARITH_G2 + EC_QUAD_DBL_FULLWARP:
+            return launch(ctx, st, "arith", k_arith_quad<Fq2, true, true>, grid32, ARITH_BLOCK, 0, d_in, d_out, n);
         default: return set_error(ctx, B200ZK_ERR_ARG, "b200zk_test_arith: no such op");
     }
-    return check_launch(ctx, "k_arith");
 }
 #endif  // __CUDACC__
 

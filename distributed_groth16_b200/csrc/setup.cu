@@ -133,35 +133,24 @@ static int points_spmv_impl(b200zk_ctx* ctx, Slot& sl, const uint32_t* d_ptr, co
         size_t lo = 0;
         for (size_t i = 0; i <= long_rows.size(); ++i) {
             const size_t hi = i < long_rows.size() ? ptr[long_rows[i]] : nnz;
-            if (hi > lo) {
-                LaunchScope ls(ctx, st, "points_spmv_products");
-                k_points_spmv_products<F><<<(unsigned)((hi - lo + 127) / 128), 128, 0, st>>>(d_idx, d_val, d_points, lo, hi, prod);
-            }
-            B2_TRY(check_launch(ctx, "k_points_spmv_products"));
+            if (hi > lo)
+                B2_TRY(launch(ctx, st, "points_spmv_products", k_points_spmv_products<F>, (unsigned)((hi - lo + 127) / 128), 128, 0,
+                              d_idx, d_val, d_points, lo, hi, prod));
             if (i < long_rows.size()) lo = ptr[long_rows[i] + 1];
         }
-        {
-            LaunchScope ls(ctx, st, "points_spmv_sum");
-            k_points_spmv_sum<F><<<(unsigned)((n_rows + 127) / 128), 128, 0, st>>>(d_ptr, prod, n_rows, d_out);
-        }
-        B2_TRY(check_launch(ctx, "k_points_spmv_sum"));
+        B2_TRY(launch(ctx, st, "points_spmv_sum", k_points_spmv_sum<F>, (unsigned)((n_rows + 127) / 128), 128, 0, d_ptr, prod, n_rows,
+                      d_out));
         if (long_rows.empty()) return B200ZK_OK;
         B2_CUDA_OK(ctx, cudaMalloc(&gathered, longest * sizeof(affine_t<F>)));
         B2_CUDA_OK(ctx, cudaMalloc(&msm_out, sizeof(xyzz_t<F>)));
         for (size_t r : long_rows) {
             const size_t b = ptr[r], len = ptr[r + 1] - ptr[r];
-            {
-                LaunchScope ls(ctx, st, "points_gather");
-                k_points_gather<F><<<(unsigned)((len + 255) / 256), 256, 0, st>>>(d_idx + b, d_points, len, gathered);
-            }
-            B2_TRY(check_launch(ctx, "k_points_gather"));
+            B2_TRY(launch(ctx, st, "points_gather", k_points_gather<F>, (unsigned)((len + 255) / 256), 256, 0, d_idx + b, d_points, len,
+                          gathered));
             B2_TRY(sizeof(F) > 32 ? msm_g2_dev(ctx, sl, gathered, d_val + b, len, msm_out)
                                   : msm_g1_dev(ctx, sl, gathered, d_val + b, len, msm_out));
-            {
-                LaunchScope ls(ctx, st, "xyzz_to_affine");
-                k_xyzz_to_affine_one<F><<<1, 32, 0, st>>>(reinterpret_cast<const xyzz_t<F>*>(msm_out), d_out + r);
-            }
-            B2_TRY(check_launch(ctx, "k_xyzz_to_affine_one"));
+            B2_TRY(launch(ctx, st, "xyzz_to_affine", k_xyzz_to_affine_one<F>, 1, 32, 0, reinterpret_cast<const xyzz_t<F>*>(msm_out),
+                          d_out + r));
         }
         return B200ZK_OK;
     };
@@ -197,21 +186,13 @@ static int fixed_base_impl(b200zk_ctx* ctx, Slot& sl, void** table_slot, const v
     cudaStream_t st = sl.stream;
     if (!*table_slot) {
         B2_CUDA_OK(ctx, cudaMalloc(table_slot, 64 * 15 * sizeof(affine_t<F>)));
-        {
-            LaunchScope ls(ctx, st, "fixed_base_table");
-            k_fixed_base_table<F><<<2, 32, 0, st>>>(reinterpret_cast<affine_t<F>*>(*table_slot));
-        }
-        B2_TRY(check_launch(ctx, "k_fixed_base_table"));
+        B2_TRY(launch(ctx, st, "fixed_base_table", k_fixed_base_table<F>, 2, 32, 0, reinterpret_cast<affine_t<F>*>(*table_slot)));
         B2_CUDA_OK(ctx, cudaStreamSynchronize(st));
     }
     if (n == 0) return B200ZK_OK;
-    {
-        LaunchScope ls(ctx, st, "fixed_base_mul");
-        k_fixed_base_mul<F><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(reinterpret_cast<const affine_t<F>*>(*table_slot),
-                                                                           reinterpret_cast<const Fr*>(d_scalars), n,
-                                                                           reinterpret_cast<affine_t<F>*>(d_out));
-    }
-    return check_launch(ctx, "k_fixed_base_mul");
+    return launch(ctx, st, "fixed_base_mul", k_fixed_base_mul<F>, (unsigned)((n + 127) / 128), 128, 0,
+                  reinterpret_cast<const affine_t<F>*>(*table_slot), reinterpret_cast<const Fr*>(d_scalars), n,
+                  reinterpret_cast<affine_t<F>*>(d_out));
 }
 
 int fixed_base_mul_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_scalars, size_t n, void* d_out) {
@@ -226,24 +207,16 @@ int fr_powers_dev(b200zk_ctx* ctx, Slot& sl, const uint64_t base[4], const uint6
     uint64_t h[8];
     memcpy(h, base, 32); memcpy(h + 4, scale, 32);
     B2_CUDA_OK(ctx, cudaMemcpyAsync(reinterpret_cast<char*>(sl.small.p) + 896, h, 64, cudaMemcpyHostToDevice, sl.stream));
-    {
-        LaunchScope ls(ctx, sl.stream, "fr_powers");
-        k_fr_powers<<<(unsigned)((n + 255) / 256), 256, 0, sl.stream>>>(reinterpret_cast<const Fr*>(reinterpret_cast<char*>(sl.small.p) + 896), n,
-                                                                         reinterpret_cast<Fr*>(d_out));
-    }
-    B2_TRY(check_launch(ctx, "k_fr_powers"));
+    B2_TRY(launch(ctx, sl.stream, "fr_powers", k_fr_powers, (unsigned)((n + 255) / 256), 256, 0,
+                  reinterpret_cast<const Fr*>(reinterpret_cast<char*>(sl.small.p) + 896), n, reinterpret_cast<Fr*>(d_out)));
     B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));      // the staging words are reused by the next call
     return B200ZK_OK;
 }
 
 int spmv_dev(b200zk_ctx* ctx, Slot& sl, const void* ptr, const void* idx, const void* val, const void* x, size_t n_rows, void* out) {
     if (n_rows == 0) return B200ZK_OK;
-    {
-        LaunchScope ls(ctx, sl.stream, "spmv");
-        k_spmv<<<(unsigned)((n_rows + 127) / 128), 128, 0, sl.stream>>>((const uint32_t*)ptr, (const uint32_t*)idx, (const Fr*)val,
-                                                                         (const Fr*)x, n_rows, (Fr*)out);
-    }
-    return check_launch(ctx, "k_spmv");
+    return launch(ctx, sl.stream, "spmv", k_spmv, (unsigned)((n_rows + 127) / 128), 128, 0, (const uint32_t*)ptr, (const uint32_t*)idx,
+                  (const Fr*)val, (const Fr*)x, n_rows, (Fr*)out);
 }
 
 int fr_lincomb_dev(b200zk_ctx* ctx, Slot& sl, const void* a, const void* b, const void* c, const uint64_t s[16], size_t n, void* out) {
@@ -251,12 +224,8 @@ int fr_lincomb_dev(b200zk_ctx* ctx, Slot& sl, const void* a, const void* b, cons
     B2_CUDA_OK(ctx, sl.small.reserve(1024));
     char* stage = reinterpret_cast<char*>(sl.small.p) + 768;
     B2_CUDA_OK(ctx, cudaMemcpyAsync(stage, s, 128, cudaMemcpyHostToDevice, sl.stream));
-    {
-        LaunchScope ls(ctx, sl.stream, "fr_lincomb");
-        k_fr_lincomb<<<(unsigned)((n + 255) / 256), 256, 0, sl.stream>>>((const Fr*)a, (const Fr*)b, (const Fr*)c,
-                                                                          reinterpret_cast<const Fr*>(stage), n, (Fr*)out);
-    }
-    B2_TRY(check_launch(ctx, "k_fr_lincomb"));
+    B2_TRY(launch(ctx, sl.stream, "fr_lincomb", k_fr_lincomb, (unsigned)((n + 255) / 256), 256, 0, (const Fr*)a, (const Fr*)b,
+                  (const Fr*)c, reinterpret_cast<const Fr*>(stage), n, (Fr*)out));
     B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
     return B200ZK_OK;
 }
@@ -435,12 +404,8 @@ int points_scale_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_points, si
         for (int i = 0; i < 4; ++i) { k[2 * i] = (uint32_t)k64[i]; k[2 * i + 1] = (uint32_t)(k64[i] >> 32); }
         ScaleK sk;
         memcpy(sk.k, k, sizeof(k));
-        {
-            LaunchScope ls(ctx, sl.stream, "points_scale_g2");
-            k_points_scale_g2_ladder<<<(unsigned)((n + 127) / 128), 128, 0, sl.stream>>>(
-                sk, reinterpret_cast<const affine_t<Fq2>*>(d_points), n, reinterpret_cast<affine_t<Fq2>*>(d_out));
-        }
-        return check_launch(ctx, "k_points_scale_g2");
+        return launch(ctx, sl.stream, "points_scale_g2", k_points_scale_g2_ladder, (unsigned)((n + 127) / 128), 128, 0, sk,
+                      reinterpret_cast<const affine_t<Fq2>*>(d_points), n, reinterpret_cast<affine_t<Fq2>*>(d_out));
     }
     reduce_mod_r(k64, k);
     const GlvSplit sp = glv_decompose(k);
@@ -460,12 +425,8 @@ int points_scale_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_points, si
     }
     dg.top = top;
     if (n >= ((size_t)1 << 31) * SCALE_BLOCK) return set_error(ctx, B200ZK_ERR_ARG, "points_scale: too many points");
-    {
-        LaunchScope ls(ctx, sl.stream, "points_scale_g1");
-        k_points_scale_g1<<<(unsigned)((n + SCALE_BLOCK - 1) / SCALE_BLOCK), SCALE_BLOCK, 0, sl.stream>>>(
-            dg, reinterpret_cast<const affine_t<Fq>*>(d_points), n, reinterpret_cast<affine_t<Fq>*>(d_out));
-    }
-    return check_launch(ctx, "k_points_scale_g1");
+    return launch(ctx, sl.stream, "points_scale_g1", k_points_scale_g1, (unsigned)((n + SCALE_BLOCK - 1) / SCALE_BLOCK), SCALE_BLOCK, 0,
+                  dg, reinterpret_cast<const affine_t<Fq>*>(d_points), n, reinterpret_cast<affine_t<Fq>*>(d_out));
 }
 
 // ---- NTT over points: out[i] = sum_j w_n^(i j) in[j], and the inverse n^-1 sum_j w_n^(-i j) in[j] -----------------------
@@ -631,24 +592,13 @@ static int points_intt_impl(b200zk_ctx* ctx, Slot& sl, int g2, bool inverse, con
         }
     }
     auto run = [&]() -> int {
-        {
-            LaunchScope ls(ctx, st, "points_intt_bitrev");
-            k_points_bitrev<F><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_in, d_out, log_n);
-        }
-        B2_TRY(check_launch(ctx, "k_points_bitrev"));
+        B2_TRY(launch(ctx, st, "points_intt_bitrev", k_points_bitrev<F>, (unsigned)((n + 255) / 256), 256, 0, d_in, d_out, log_n));
         if (!half) return B200ZK_OK;
-        {
-            LaunchScope ls(ctx, st, "points_intt_twiddles");
-            k_intt_twiddle_digits<<<(unsigned)((half + 255) / 256), 256, 0, st>>>(log_n, inverse, half, tw);
-        }
-        B2_TRY(check_launch(ctx, "k_intt_twiddle_digits"));
-        for (unsigned log_m = 0; log_m < log_n; ++log_m) {
-            {
-                LaunchScope ls(ctx, st, g2 ? "points_intt_pass_g2" : "points_intt_pass_g1");
-                k_points_intt_pass<F, B><<<(unsigned)((half + B - 1) / B), B, 0, st>>>(d_out, tw, log_n, log_m);
-            }
-            B2_TRY(check_launch(ctx, "k_points_intt_pass"));
-        }
+        B2_TRY(launch(ctx, st, "points_intt_twiddles", k_intt_twiddle_digits, (unsigned)((half + 255) / 256), 256, 0, log_n, inverse,
+                      half, tw));
+        for (unsigned log_m = 0; log_m < log_n; ++log_m)
+            B2_TRY(launch(ctx, st, g2 ? "points_intt_pass_g2" : "points_intt_pass_g1", k_points_intt_pass<F, B>,
+                          (unsigned)((half + B - 1) / B), B, 0, d_out, tw, log_n, log_m));
         if (!inverse) return B200ZK_OK;
         // n^-1 mod r = r - (r - 1) / n  (n divides r - 1)
         uint32_t q[8], ninv32[8];
@@ -745,16 +695,9 @@ static int points_mul_powers_impl(b200zk_ctx* ctx, Slot& sl, const affine_t<F>* 
         }
     }
     auto run = [&]() -> int {
-        {
-            LaunchScope ls(ctx, st, "powers_digits");
-            k_powers_digits<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, n, dg);
-        }
-        B2_TRY(check_launch(ctx, "k_powers_digits"));
-        {
-            LaunchScope ls(ctx, st, sizeof(F) > 32 ? "points_mul_powers_g2" : "points_mul_powers_g1");
-            k_points_mul_powers<F, B><<<(unsigned)((n + B - 1) / B), B, 0, st>>>(d_points, dg, n, d_out);
-        }
-        return check_launch(ctx, "k_points_mul_powers");
+        B2_TRY(launch(ctx, st, "powers_digits", k_powers_digits, (unsigned)((n + 255) / 256), 256, 0, c, n, dg));
+        return launch(ctx, st, sizeof(F) > 32 ? "points_mul_powers_g2" : "points_mul_powers_g1", k_points_mul_powers<F, B>,
+                      (unsigned)((n + B - 1) / B), B, 0, d_points, dg, n, d_out);
     };
     const int rc = run();
     const cudaError_t e = cudaStreamSynchronize(st);                     // the digits are freed below
@@ -795,14 +738,11 @@ int points_sub_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_a, const voi
     if (n == 0) return B200ZK_OK;
     if (n >= ((size_t)1 << 31) * SUB_BLOCK) return set_error(ctx, B200ZK_ERR_ARG, "points_sub: too many points");
     const unsigned grid = (unsigned)((n + SUB_BLOCK - 1) / SUB_BLOCK);
-    {
-        LaunchScope ls(ctx, sl.stream, g2 ? "points_sub_g2" : "points_sub_g1");
-        if (g2) k_points_sub<Fq2><<<grid, SUB_BLOCK, 0, sl.stream>>>((const affine_t<Fq2>*)d_a, (const affine_t<Fq2>*)d_b, n,
-                                                                     (affine_t<Fq2>*)d_out);
-        else k_points_sub<Fq><<<grid, SUB_BLOCK, 0, sl.stream>>>((const affine_t<Fq>*)d_a, (const affine_t<Fq>*)d_b, n,
-                                                                 (affine_t<Fq>*)d_out);
-    }
-    return check_launch(ctx, "k_points_sub");
+    if (g2)
+        return launch(ctx, sl.stream, "points_sub_g2", k_points_sub<Fq2>, grid, SUB_BLOCK, 0, (const affine_t<Fq2>*)d_a,
+                      (const affine_t<Fq2>*)d_b, n, (affine_t<Fq2>*)d_out);
+    return launch(ctx, sl.stream, "points_sub_g1", k_points_sub<Fq>, grid, SUB_BLOCK, 0, (const affine_t<Fq>*)d_a, (const affine_t<Fq>*)d_b,
+                  n, (affine_t<Fq>*)d_out);
 }
 
 }  // namespace b200zk

@@ -83,11 +83,7 @@ int groth16_verify_dev(b200zk_ctx* ctx, Slot& sl, const uint64_t* alpha_g1, cons
     v.b = reinterpret_cast<const affine_t<Fq2>*>(d + o_b);
     v.c = reinterpret_cast<const affine_t<Fq>*>(d + o_c);
     v.result = reinterpret_cast<uint32_t*>(d + o_res);
-    {
-        LaunchScope ls(ctx, st, "groth16_verify");
-        k_groth16_verify<<<1, 128, 0, st>>>(v);
-    }
-    B2_TRY(check_launch(ctx, "k_groth16_verify"));
+    B2_TRY(launch(ctx, st, "groth16_verify", k_groth16_verify, 1, 128, 0, v));
     uint32_t res = 0;
     B2_CUDA_OK(ctx, cudaMemcpyAsync(&res, d + o_res, 4, cudaMemcpyDeviceToHost, st));
     B2_CUDA_OK(ctx, cudaStreamSynchronize(st));
@@ -124,12 +120,8 @@ int vk_alphabeta_12_dev(b200zk_ctx* ctx, Slot& sl, const uint64_t* alpha_g1, con
     char* d = reinterpret_cast<char*>(sl.io_b.p);
     B2_CUDA_OK(ctx, cudaMemcpyAsync(d, alpha_g1, 64, cudaMemcpyHostToDevice, st));
     B2_CUDA_OK(ctx, cudaMemcpyAsync(d + 64, beta_g2, 128, cudaMemcpyHostToDevice, st));
-    {
-        LaunchScope ls(ctx, st, "vk_alphabeta_12");
-        k_vk_alphabeta_12<<<1, 1, 0, st>>>(reinterpret_cast<const affine_t<Fq>*>(d), reinterpret_cast<const affine_t<Fq2>*>(d + 64),
-                                            reinterpret_cast<Fq*>(d + 192));
-    }
-    B2_TRY(check_launch(ctx, "k_vk_alphabeta_12"));
+    B2_TRY(launch(ctx, st, "vk_alphabeta_12", k_vk_alphabeta_12, 1, 1, 0, reinterpret_cast<const affine_t<Fq>*>(d),
+                  reinterpret_cast<const affine_t<Fq2>*>(d + 64), reinterpret_cast<Fq*>(d + 192)));
     B2_CUDA_OK(ctx, cudaMemcpyAsync(out, d + 192, 384, cudaMemcpyDeviceToHost, st));
     B2_CUDA_OK(ctx, cudaStreamSynchronize(st));
     return B200ZK_OK;
