@@ -639,7 +639,7 @@ int b200zk_fr_spmv_dev(b200zk_ctx* ctx, const void* d_ptr, const void* d_idx, co
 }
 int b200zk_points_spmv_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_ptr, const void* d_idx, const void* d_val,
                            const void* d_points, size_t n_rows, void* d_out) {
-    if (!ctx || !valid_slot(stream) || (n_rows && (!d_ptr || !d_idx || !d_val || !d_points || !d_out))) return B200ZK_ERR_ARG;
+    if (!ctx || !valid_slot(stream) || (n_rows && (!d_ptr || !d_points || !d_out))) return B200ZK_ERR_ARG;   // idx, val: in the impl
     return with_slot(ctx, stream, [&](Slot& sl) {
         return points_spmv_dev(ctx, sl, g2, d_ptr, d_idx, d_val, d_points, n_rows, d_out);
     });

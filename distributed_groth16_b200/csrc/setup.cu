@@ -116,6 +116,8 @@ static int points_spmv_impl(b200zk_ctx* ctx, Slot& sl, const uint32_t* d_ptr, co
     B2_CUDA_OK(ctx, cudaMemcpyAsync(ptr.data(), d_ptr, (n_rows + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     B2_CUDA_OK(ctx, cudaStreamSynchronize(st));
     const size_t nnz = ptr[n_rows];
+    // a matrix with no non-zeros (an empty B, say) arrives with empty, hence null, idx and val: nothing reads them
+    if (nnz && (!d_idx || !d_val)) return set_error(ctx, B200ZK_ERR_ARG, "points_spmv: idx or val is null and nnz > 0");
     std::vector<size_t> long_rows;
     for (size_t r = 0; r < n_rows; ++r) {
         if (ptr[r + 1] < ptr[r]) return set_error(ctx, B200ZK_ERR_ARG, "points_spmv: row pointers decrease");

@@ -263,8 +263,8 @@ int b200zk_fr_spmv_dev(b200zk_ctx* ctx, const void* d_ptr, const void* d_idx, co
  * snarkjs `zkey new` that turns a Powers-of-Tau file's Lagrange bases into the query vectors, and (over the odd points of
  * the doubled domain) the h-query convention of ark-circom/src/circom/qap.rs:11-15.  Conventions as
  * b200zk_fr_spmv_dev: ptr n_rows + 1 x u32, idx nnz x u32, val nnz x 4 limbs Montgomery; points / out affine (g2 = 0: G1,
- * 8 u64 limbs; 1: G2, 16), infinity all-zero, an empty row gives infinity.  Rows of more than 256 entries go through the
- * MSM.  Reads ptr to the host and returns once out is complete; temporary device memory: nnz XYZZ points. */
+ * 8 u64 limbs; 1: G2, 16), infinity all-zero, an empty row gives infinity; idx and val may be null when
+ * nnz = ptr[n_rows] = 0.  Rows of more than 256 entries go through the MSM.  Reads ptr to the host and returns once out is complete; temporary device memory: nnz XYZZ points. */
 int b200zk_points_spmv_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_ptr, const void* d_idx, const void* d_val,
                            const void* d_points, size_t n_rows, void* d_out);
 /* One scalar times many points, out[i] = k * points[i] -- the step of a snarkjs `zkey contribute` / `zkey beacon` that
