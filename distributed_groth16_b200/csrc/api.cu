@@ -43,9 +43,7 @@ int b200zk_ctx_create(int device, b200zk_ctx** out) {
         }
         ctx->slots[i].owns_stream = true;
         bool ok = cudaStreamCreateWithFlags(&ctx->slots[i].copy_stream, cudaStreamNonBlocking) == cudaSuccess &&
-                  cudaStreamCreateWithFlags(&ctx->slots[i].aux_stream, cudaStreamNonBlocking) == cudaSuccess &&
-                  cudaEventCreateWithFlags(&ctx->slots[i].copy_done, cudaEventDisableTiming) == cudaSuccess &&
-                  cudaEventCreateWithFlags(&ctx->slots[i].aux_done, cudaEventDisableTiming) == cudaSuccess;
+                  cudaEventCreateWithFlags(&ctx->slots[i].copy_done, cudaEventDisableTiming) == cudaSuccess;
         for (int k = 0; ok && k < 32; ++k) ok = cudaEventCreateWithFlags(&ctx->slots[i].stage_ev[k], cudaEventDisableTiming) == cudaSuccess;
         if (!ok) {
             delete ctx;
@@ -56,7 +54,7 @@ int b200zk_ctx_create(int device, b200zk_ctx** out) {
         int lo = 0, hi = 0;
         cudaDeviceGetStreamPriorityRange(&lo, &hi);
         bool ok = true;
-        for (int k = 0; ok && k < 6; ++k) ok = cudaStreamCreateWithPriority(&ctx->msm_side[k], cudaStreamNonBlocking, hi) == cudaSuccess;
+        for (int k = 0; ok && k < 3; ++k) ok = cudaStreamCreateWithPriority(&ctx->msm_side[k], cudaStreamNonBlocking, hi) == cudaSuccess;
         if (!ok) { b200zk_ctx_destroy(ctx); return B200ZK_ERR_CUDA; }
     }
     *out = ctx;
@@ -74,14 +72,11 @@ void b200zk_ctx_destroy(b200zk_ctx* ctx) {
         Slot& s = ctx->slots[i];
         s.ws_msm.release(); s.ws_ntt.release(); s.io_a.release(); s.io_b.release(); s.small.release();
         if (s.owns_stream && s.stream) cudaStreamDestroy(s.stream);
-        s.ws_msm_aux.release();
         if (s.copy_stream) cudaStreamDestroy(s.copy_stream);
-        if (s.aux_stream) cudaStreamDestroy(s.aux_stream);
         if (s.copy_done) cudaEventDestroy(s.copy_done);
-        if (s.aux_done) cudaEventDestroy(s.aux_done);
         for (int k = 0; k < 32; ++k) if (s.stage_ev[k]) cudaEventDestroy(s.stage_ev[k]);
     }
-    for (int k = 0; k < 6; ++k) if (ctx->msm_side[k]) cudaStreamDestroy(ctx->msm_side[k]);
+    for (int k = 0; k < 3; ++k) if (ctx->msm_side[k]) cudaStreamDestroy(ctx->msm_side[k]);
     for (auto& v : ctx->msm_events) for (cudaEvent_t e : v) cudaEventDestroy(e);
     for (auto& e : ctx->prof_pending) { cudaEventDestroy(e.start); cudaEventDestroy(e.stop); }
     delete ctx;
@@ -292,11 +287,11 @@ int b200zk_msm_staged_dev(b200zk_ctx* ctx, int stream, int g2, const uint64_t* b
 
 int b200zk_msm_g1_dev(b200zk_ctx* ctx, int stream, const void* d_bases, const void* d_scalars, size_t n, void* d_out) {
     if (!ctx || !valid_slot(stream) || !d_out) return B200ZK_ERR_ARG;
-    return with_slot(ctx, stream, [&](Slot& sl) { return msm_g1_dev(ctx, sl, d_bases, d_scalars, n, d_out); });
+    return with_slot(ctx, stream, [&](Slot& sl) { return msm_g1_dev(ctx, sl, d_bases, d_scalars, n, d_out, 0); });
 }
 int b200zk_msm_g2_dev(b200zk_ctx* ctx, int stream, const void* d_bases, const void* d_scalars, size_t n, void* d_out) {
     if (!ctx || !valid_slot(stream) || !d_out) return B200ZK_ERR_ARG;
-    return with_slot(ctx, stream, [&](Slot& sl) { return msm_g2_dev(ctx, sl, d_bases, d_scalars, n, d_out); });
+    return with_slot(ctx, stream, [&](Slot& sl) { return msm_g2_dev(ctx, sl, d_bases, d_scalars, n, d_out, 0); });
 }
 
 unsigned b200zk_msm_table_windows(unsigned c) { return c ? msm_table_windows(c) : 0; }
@@ -308,7 +303,7 @@ int b200zk_msm_table_build_dev(b200zk_ctx* ctx, int stream, int g2, const void* 
 int b200zk_msm_table_dev(b200zk_ctx* ctx, int stream, int g2, const void* d_table, const void* d_scalars, size_t n, unsigned c,
                          void* d_out) {
     if (!ctx || !valid_slot(stream) || !d_out) return B200ZK_ERR_ARG;
-    return with_slot(ctx, stream, [&](Slot& sl) { return msm_table_dev(ctx, sl, g2, d_table, d_scalars, n, c, d_out); });
+    return with_slot(ctx, stream, [&](Slot& sl) { return msm_table_dev(ctx, sl, g2, d_table, d_scalars, n, c, d_out, 0); });
 }
 
 int b200zk_g1_sum_dev(b200zk_ctx* ctx, int stream, const void* d, size_t count, uint64_t out[8], int* inf) {

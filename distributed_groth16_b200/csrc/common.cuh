@@ -51,9 +51,6 @@ struct Slot {                 // one per MultiplexedStreamID
     DevBuf small;             // results
     cudaStream_t copy_stream = nullptr;   // second stream for overlapped H2D staging (host-buffer entry points)
     cudaEvent_t copy_done = nullptr;
-    cudaStream_t aux_stream = nullptr;    // second compute stream + workspace: host-staged MSMs run as two halves
-    DevBuf ws_msm_aux;
-    cudaEvent_t aux_done = nullptr;
     cudaEvent_t stage_ev[32] = {};        // host-staged MSM: arrival of part p's scalars [2 p] / bases [2 p + 1]
 };
 
@@ -63,7 +60,6 @@ struct b200zk_ctx {
     int device = 0;
     int sm_count = 132;
     b200zk::Slot slots[3];
-    unsigned msm_seg_hint = 0;      // set by prove_dev around its MSM launches (it holds every slot lock): reduction segment length
     std::string last_error;
     std::mutex err_mu;
     // profiling
@@ -79,12 +75,11 @@ struct b200zk_ctx {
     std::mutex plan_mu;
     std::map<uint32_t, b200zk::NttPlan*> plans;
     void *fb_table_g1 = nullptr, *fb_table_g2 = nullptr;     // fixed-base window tables of the generators (setup.cu)
-    // MSM channels (msm.cu, window-group pipeline): 0..5 = slot i's main / aux workspace (2 i + aux).
-    // msm_side[ch]: high-priority helper stream that runs the sort phases and the reduction / Horner tail of one window
-    // group while the bucket kernel of the next group occupies the SMs; msm_events[ch]: its event pool (grown on demand,
-    // only ever touched under the owning slot's mutex).
-    cudaStream_t msm_side[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    std::vector<cudaEvent_t> msm_events[6];
+    // MSM window-group pipeline (msm.cu), one per slot: msm_side[i], a high-priority helper stream that runs the sort phases
+    // and the reduction / Horner tail of one window group while the bucket kernel of the next group occupies the SMs;
+    // msm_events[i], the event pool of slot i's MSMs (grown on demand, only ever touched under the slot's mutex).
+    cudaStream_t msm_side[3] = {nullptr, nullptr, nullptr};
+    std::vector<cudaEvent_t> msm_events[3];
 };
 
 struct b200zk_pk {
@@ -193,11 +188,10 @@ int fourstep_cols_p2p_dev(b200zk_ctx* ctx, Slot& sl, const Fr* d_in, void* const
 int mul_sub_dev(b200zk_ctx* ctx, Slot& sl, const Fr* a, const Fr* b, const Fr* c, Fr* out, size_t n);
 void ntt_free_plans(b200zk_ctx* ctx);
 // msm.cu
-// aux != 0: run on the slot's second compute stream / workspace (aux_stream, ws_msm_aux)
-int msm_g1_dev(b200zk_ctx* ctx, Slot& sl, const void* d_bases, const void* d_scalars, size_t n, void* d_out_xyzz,
-               cudaEvent_t bases_ready = nullptr, int aux = 0);
-int msm_g2_dev(b200zk_ctx* ctx, Slot& sl, const void* d_bases, const void* d_scalars, size_t n, void* d_out_xyzz,
-               cudaEvent_t bases_ready = nullptr, int aux = 0);
+// seg: buckets per segment of the bucket reduction; 0, or more than one window's buckets, keeps the default of 16 (small bucket
+// sets take 8 whatever seg says)
+int msm_g1_dev(b200zk_ctx* ctx, Slot& sl, const void* d_bases, const void* d_scalars, size_t n, void* d_out_xyzz, unsigned seg);
+int msm_g2_dev(b200zk_ctx* ctx, Slot& sl, const void* d_bases, const void* d_scalars, size_t n, void* d_out_xyzz, unsigned seg);
 int msm_parts_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_bases, const void* d_scalars, const size_t* cnt, unsigned nparts,
                   const cudaEvent_t* ev_scalars, const cudaEvent_t* ev_bases, void* d_out_xyzz);
 // api.cu: host buffers -> device partial, staged in parts
@@ -206,7 +200,7 @@ unsigned msm_table_windows(unsigned c);
 unsigned msm_table_auto_window(size_t n);
 int msm_table_build_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_bases, size_t n, unsigned c, void* d_table);
 int msm_table_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_table, const void* d_scalars, size_t n, unsigned c,
-                  void* d_out_xyzz, int aux = 0);
+                  void* d_out_xyzz, unsigned seg);
 int g1_sum_dev(b200zk_ctx* ctx, Slot& sl, const void* d_xyzz, size_t count, void* d_out_affine);
 int g2_sum_dev(b200zk_ctx* ctx, Slot& sl, const void* d_xyzz, size_t count, void* d_out_affine);
 int xyzz_sum_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_in, size_t count, size_t stride, void* d_out);
@@ -265,9 +259,10 @@ bool pk_tables_enabled();
 // runs on the queries.  tab / tab_c / *bytes: what was built (tab_c[k] = 0: no table).
 int pk_tables_build(b200zk_ctx* ctx, Slot& sl, const void* const src[5], const size_t cnt[5], unsigned c_req, void* tab[5],
                     unsigned tab_c[5], size_t* bytes);
-// MSM over query k (numbered as for pk_tables_build): over tab[k] when tab_c[k] != 0, else the generic MSM on `query`
+// MSM over query k (numbered as for pk_tables_build): over tab[k] when tab_c[k] != 0, else the generic MSM on `query`;
+// seg as for msm_g1_dev
 int query_msm(b200zk_ctx* ctx, Slot& sl, int k, const void* query, void* const tab[5], const unsigned tab_c[5], const Fr* scalars,
-              size_t n, void* out);
+              size_t n, void* out, unsigned seg);
 int prove_dev(b200zk_ctx* ctx, const b200zk_pk* pk, const Fr* d_z, const Fr* d_a, const Fr* d_b, const Fr* d_c,
               const uint64_t r[4], const uint64_t s[4], int mirror_bg1, uint8_t proof_out[128]);
 

@@ -542,7 +542,7 @@ int b200zk_group_groth16_prove(b200zk_group* grp, const b200zk_group_pk* pk, con
         const Fr* dz = reinterpret_cast<const Fr*>(vz[g]);
         const Fr* dzaux = dz + (S.v1 - S.v0);
         auto msm = [&](int k, const Fr* scalars, size_t n, void* out) {
-            return query_msm(ctx, sl, k, S.q[k], S.tab, S.tab_c, scalars, n, out);
+            return query_msm(ctx, sl, k, S.q[k], S.tab, S.tab_c, scalars, n, out, 0);
         };
         G_TRY(grp, g, msm(2, dz, S.v1 - S.v0, sm + 512));                       // the G2 MSM first: the longest
         G_TRY(grp, g, msm(0, dz, S.v1 - S.v0, sm + 0));

@@ -15,6 +15,8 @@
 //   5 reduce     per window sum_b b * bucket_b as segment running sums + small scalar multiples,
 //                tree-combined per window in shared memory
 //   6 combine    Horner over windows (c doublings each)
+#include <type_traits>
+
 #include "common.cuh"
 #include "glv.cuh"
 
@@ -296,6 +298,11 @@ __device__ __forceinline__ xyzz_t<F> add_sel(const xyzz_t<F>& a, const xyzz_t<F>
     if (sizeof(F) == 32) return xyzz_t<F>::add_inl(a, b);      // G1: inline (see k_msm_reduce_segments)
     return xyzz_t<F>::add(a, b);
 }
+template <class F>
+__device__ __forceinline__ xyzz_t<F> dbl_sel(const xyzz_t<F>& a) {
+    if (sizeof(F) == 32) return xyzz_t<F>::dbl_inl(a);
+    return xyzz_t<F>::dbl(a);
+}
 
 // buckets[g] = sum of the task sums of g, for every multi-task bucket; one block per bucket, grid-strided
 template <class F>
@@ -352,21 +359,20 @@ __global__ void __launch_bounds__(128) k_msm_reduce_segments(const xyzz_t<F>* bu
     uint32_t lo = seg * seg_len;
     const xyzz_t<F>* bw = buckets + (size_t)w * B;
     xyzz_t<F> run = xyzz_t<F>::identity(), acc = xyzz_t<F>::identity();
-    // G1: the group law is inlined here (an out-of-line call moves 3 x 128 B through local memory per
+    // G1: the group law is inlined here (add_sel / dbl_sel: an out-of-line call moves 3 x 128 B through local memory per
     // operation, which dominated this latency-bound chain); G2 keeps the calls to bound code size.
-    constexpr bool INL = sizeof(F) == 32;
     for (uint32_t k = lo + seg_len; k-- > lo;) {
         xyzz_t<F> bk = ld16(bw + k);
-        if (INL) { run = xyzz_t<F>::add_inl(run, bk); acc = xyzz_t<F>::add_inl(acc, run); }
-        else { run = xyzz_t<F>::add(run, bk); acc = xyzz_t<F>::add(acc, run); }
+        run = add_sel<F>(run, bk);
+        acc = add_sel<F>(acc, run);
     }
     if (lo) {   // + lo * run
         xyzz_t<F> m = xyzz_t<F>::identity();
         for (int bit = 31 - __clz(lo); bit >= 0; --bit) {
-            if (INL) m = xyzz_t<F>::dbl_inl(m); else m = xyzz_t<F>::dbl(m);
-            if ((lo >> bit) & 1) { if (INL) m = xyzz_t<F>::add_inl(m, run); else m = xyzz_t<F>::add(m, run); }
+            m = dbl_sel<F>(m);
+            if ((lo >> bit) & 1) m = add_sel<F>(m, run);
         }
-        if (INL) acc = xyzz_t<F>::add_inl(acc, m); else acc = xyzz_t<F>::add(acc, m);
+        acc = add_sel<F>(acc, m);
     }
     st16(partials + t, acc);
 }
@@ -516,25 +522,6 @@ static int exclusive_scan(b200zk_ctx* ctx, cudaStream_t st, const uint32_t* in, 
     return launch(ctx, st, "msm_scan", k_scan_add, nblk, SCAN_THREADS, 0, out, sums, n);
 }
 
-// event `idx` of MSM channel `ch` (common.cuh), created on first use; only called under the owning slot's mutex
-static cudaEvent_t msm_event(b200zk_ctx* ctx, int ch, size_t idx) {
-    std::vector<cudaEvent_t>& v = ctx->msm_events[ch];
-    while (v.size() <= idx) {
-        cudaEvent_t e = nullptr;
-        if (cudaEventCreateWithFlags(&e, cudaEventDisableTiming) != cudaSuccess) return nullptr;
-        v.push_back(e);
-    }
-    return v[idx];
-}
-
-// Streams of one MSM.  `seq`: digit / sort phases and, per window group, merge + bucket reduction + Horner step;
-// `acc`: the bucket kernels, on the caller's stream, which the result is ordered on.  `seq` is the channel's
-// high-priority side stream.
-struct MsmStreams {
-    cudaStream_t seq, acc;
-    int channel;
-};
-
 // One input part of an MSM: `n` pairs, and (host-staged callers) the events that signal the arrival of its scalars / bases.
 struct MsmPart {
     const void* bases;
@@ -543,14 +530,159 @@ struct MsmPart {
     cudaEvent_t bases_ready, scalars_ready;
 };
 
+// What one MSM computes: every size and threshold of its launches and of its workspace, from the part sizes, the fixed-base
+// table window tab_c (0: GLV digits over the bases themselves) and the caller's bucket-reduction segment length seg (0: default).
+struct MsmPlan {
+    size_t n, n_max;                    // pairs in all parts / in the largest part
+    unsigned nparts;
+    bool fold;                          // tab_c != 0: all digit windows share one bucket set, and there is no Horner chain
+    unsigned c, Wh, W, WB;              // window bits, windows per GLV half, digit windows, bucket sets
+    uint32_t B, nb;                     // buckets per set, in all
+    bool quad_reduce;                   // one quad per reduction segment (k_msm_reduce_segments_quad)
+    uint32_t seg_len, nseg, wsplit;     // buckets per reduction segment, segments per set, window-sum blocks per set
+    uint32_t rmw;                       // several parts: the bucket kernels add into the shared buckets
+    size_t total_max;                   // sort entries of the largest part
+    uint32_t task_len;
+    size_t max_tasks;                   // task array length per part, all groups together
+    unsigned ngroups;
+    struct Group {                      // window group: consecutive bucket sets, with the same task-table geometry in every part
+        uint32_t set0, nsets, b0, nbk;  // bucket sets [set0, set0 + nsets), buckets [b0, b0 + nbk)
+        size_t task_cap, task_base;     // task arrays: [task_base, task_base + task_cap)
+        uint32_t list_cap; size_t list_base;    // multi-task bucket list
+    } group[4];
+};
+
+// pl.n == 0: nothing else is set, the MSM is the identity
+static int msm_plan(b200zk_ctx* ctx, const MsmPart* parts, unsigned nparts, unsigned tab_c, unsigned seg, MsmPlan& pl) {
+    pl = MsmPlan{};
+    pl.nparts = nparts;
+    for (unsigned p = 0; p < nparts; ++p) { pl.n += parts[p].n; pl.n_max = parts[p].n > pl.n_max ? parts[p].n : pl.n_max; }
+    if (pl.n == 0) return B200ZK_OK;
+    if (pl.n >= (1ull << 31)) return set_error(ctx, B200ZK_ERR_ARG, "MSM length must be < 2^31");
+    // tab_c != 0: the bases are a fixed-base table of msm_table_windows(tab_c) x n points (section 7); all digit windows
+    // then share one bucket set and the Horner chain disappears
+    pl.fold = tab_c != 0;
+    if (pl.fold && nparts != 1) return set_error(ctx, B200ZK_ERR_ARG, "fixed-base tables take one input part");
+    pl.c = pl.fold ? tab_c : choose_window(pl.n);
+    // every other MSM splits its scalars (glv.cuh; G2: the same split, phi = (beta^2 x, y))
+    pl.Wh = (128 + pl.c - 1) / pl.c;                        // |k1|, |k2| < 2^127: Wh * c >= 128 leaves the carry room
+    pl.W = pl.fold ? msm_table_windows(pl.c) : 2 * pl.Wh;   // digit windows
+    pl.WB = pl.fold ? 1 : pl.W;                             // bucket sets
+    if ((uint64_t)pl.W * pl.n >= (pl.fold ? (1ull << 31) : (1ull << 32)))
+        return set_error(ctx, B200ZK_ERR_ARG, "MSM too large for 32-bit bucket offsets / entry indices (W * n)");
+    pl.B = 1u << (pl.c - 1);
+    pl.nb = pl.WB * pl.B;
+    pl.seg_len = pl.B < 16 ? pl.B : 16;
+    // Small bucket sets (<= 8192 16-bucket segments in all: a 30 k-point MSM, the small windows of a 2^16 one) are reduced by one
+    // QUAD per segment (k_msm_reduce_segments_quad) and, being pure latency chains, in 8-bucket segments whatever the caller's
+    // `seg`: 16 + ~16 dependent point operations per segment instead of 64 + ~15 with the 32-bucket segments a 2^20 proof prefers.
+    pl.quad_reduce = (uint64_t)pl.WB * (pl.B / pl.seg_len) <= 8192;
+    if (pl.quad_reduce) pl.seg_len = pl.B < 8 ? pl.B : 8;
+    else if (seg && seg <= pl.B) pl.seg_len = seg;
+    pl.nseg = pl.B / pl.seg_len;
+    // fold (one bucket set): the segment partials are summed by `wsplit` blocks whose results the Horner kernel adds up
+    pl.wsplit = pl.fold ? (pl.nseg >= 16 * 256 ? 16 : (pl.nseg >= 1024 ? 4 : 1)) : 1;
+
+    // window groups: consecutive bucket sets (whole windows, i.e. both GLV halves).  Measured on an earlier GPU:
+    // at 2^20 the extra launches, the drain bubble at the end of every bucket kernel and the slowdown of the latency-bound
+    // tail kernels when they share SMs with a bucket kernel cost more than the hidden tail saves (1 group beats 2 and 4);
+    // from 2^22 up four groups win; uneven groups lose.  Fixed-base tables have one bucket set;
+    // several input parts already cut the bucket work into pieces.
+    const unsigned unit_sets = pl.fold ? 1 : 2;
+    const unsigned units = pl.fold ? 1 : pl.Wh;             // windows
+    pl.ngroups = 1;
+    if (!pl.fold && nparts == 1 && pl.n >= (1u << 22)) pl.ngroups = units < 4 ? units : 4;
+    pl.rmw = nparts > 1 ? 1u : 0u;
+
+    // task length: 128 unless the average bucket is already that long (n >> 2^c: every bucket would be cut in two);
+    // then the next power of two above 3x the average -- only outliers are split -- as long as that leaves enough
+    // tasks (>= 2^19) to fill the machine
+    pl.total_max = (size_t)pl.W * pl.n_max;
+    pl.task_len = TASK_LEN;
+    while (pl.task_len < MAX_TASK_LEN && (uint64_t)pl.task_len * pl.nb < 3 * (uint64_t)pl.total_max &&
+           pl.total_max / (2 * pl.task_len) + pl.nb >= (1u << 19))
+        pl.task_len *= 2;
+    // Small inputs cannot fill the machine with 128-entry tasks, and a real witness (29 821 of the 29 823 entries of the
+    // reference's sha256 witness are 0 or 1, groth16/examples/sha256.rs:182-185) puts thousands of entries into ONE bucket:
+    // 118 serial chains of 128 additions for a 30 k-point MSM.  Shorter tasks turn that bucket into ~900 parallel
+    // chains of 16 plus a block-level tree (k_msm_merge_tasks); buckets that stay below 16 entries are unaffected.
+    if (pl.n_max <= (1u << 16))
+        while (pl.task_len > 16 && pl.total_max / pl.task_len < (1u << 17)) pl.task_len /= 2;
+    pl.max_tasks = pl.total_max / pl.task_len + pl.nb + pl.ngroups;
+
+    size_t tb = 0, lb = 2 * (size_t)pl.ngroups;
+    for (unsigned g = 0; g < pl.ngroups; ++g) {
+        MsmPlan::Group& G = pl.group[g];
+        const unsigned u0 = (unsigned)(((uint64_t)units * g) / pl.ngroups), u1 = (unsigned)(((uint64_t)units * (g + 1)) / pl.ngroups);
+        G.set0 = u0 * unit_sets; G.nsets = (u1 - u0) * unit_sets;
+        G.b0 = G.set0 * pl.B; G.nbk = G.nsets * pl.B;
+        const size_t gtotal = pl.fold ? pl.total_max : (size_t)G.nsets * pl.n_max;
+        G.task_cap = gtotal / pl.task_len + G.nbk + 1;
+        G.task_base = tb; tb += G.task_cap;
+        G.list_cap = (uint32_t)(gtotal / pl.task_len + 1);
+        G.list_base = lb; lb += G.list_cap;
+    }
+    return B200ZK_OK;
+}
+
+// Typed views of one MSM's workspace (the slot's ws_msm), 256-byte aligned: the sort and task arrays once per part, the bucket
+// set and the reduction buffers once.  Group g of a part uses ntasks / task_off from G.b0 + g (nbk + 1 entries), the task arrays
+// from G.task_base, multi from G.list_base (its big / small counts at [2 g], [2 g + 1]) and hist from g * (MAX_TASK_LEN + 1).
+template <class F>
+struct MsmWorkspace {
+    struct Part {
+        uint32_t *keys, *ranks, *entries, *counts, *offsets, *ntasks, *task_off, *task_bucket, *multi, *hist, *task_rank, *order;
+        xyzz_t<F>* task_sums;
+    };
+    std::vector<Part> part;
+    uint32_t* sums;
+    xyzz_t<F> *buckets, *partials, *wsum, *hstate;
+};
+
+template <class F>
+static int msm_workspace(b200zk_ctx* ctx, DevBuf& buf, const MsmPlan& pl, const MsmPart* parts, MsmWorkspace<F>& ws) {
+    ws.part.resize(pl.nparts);
+    // one carve-up, run twice: from address 0 it sizes the buffer, from the buffer's address it sets the pointers
+    auto layout = [&](uintptr_t base) {
+        size_t o = 0;
+        auto carve = [&](auto*& ptr, size_t count) {
+            using T = std::remove_reference_t<decltype(*ptr)>;
+            ptr = reinterpret_cast<T*>(base + o);
+            o += (count * sizeof(T) + 255) & ~(size_t)255;
+        };
+        for (unsigned p = 0; p < pl.nparts; ++p) {
+            typename MsmWorkspace<F>::Part& w = ws.part[p];
+            const size_t total = (size_t)pl.W * parts[p].n;
+            carve(w.keys, total); carve(w.ranks, total); carve(w.entries, total);
+            carve(w.counts, (size_t)pl.nb + 1); carve(w.offsets, (size_t)pl.nb + 1);
+            carve(w.ntasks, (size_t)pl.nb + pl.ngroups); carve(w.task_off, (size_t)pl.nb + pl.ngroups);
+            carve(w.task_bucket, pl.max_tasks);
+            carve(w.multi, pl.total_max / pl.task_len + 4 * pl.ngroups + 4);
+            carve(w.hist, (size_t)pl.ngroups * (MAX_TASK_LEN + 1));
+            carve(w.task_rank, pl.max_tasks); carve(w.order, pl.max_tasks);
+            carve(w.task_sums, pl.max_tasks);
+        }
+        carve(ws.sums, (size_t)pl.nb / SCAN_TILE + 2);
+        carve(ws.buckets, pl.nb);
+        carve(ws.partials, (size_t)pl.WB * pl.nseg);
+        carve(ws.wsum, (size_t)pl.WB * pl.wsplit);
+        carve(ws.hstate, 2);
+        return o;
+    };
+    B2_CUDA_OK(ctx, buf.reserve(layout(0)));
+    layout(reinterpret_cast<uintptr_t>(buf.p));
+    return B200ZK_OK;
+}
+
 // The window-group pipeline (one MSM, no host round trips):
 //   seq : digits, scan | prep(0) | prep(1) .. prep(G-1) | wait A0: tail(0) | wait A1: tail(1) | ...
 //   acc :                 wait P0: accumulate(0) -> A0 | wait P1: accumulate(1) -> A1 | ...
 // prep(g) = task tables + scatter of group g's bucket sets, tail(g) = merge + bucket reduction + window sums + Horner
 // step.  Groups hold consecutive bucket sets in Horner order (top windows first), so tail(g) -- a chain of dependent
 // point operations that used to follow the bucket kernel (a quarter of a 2^20 MSM) -- overlaps accumulate(g + 1); only
-// the last group's tail is exposed.  `seq` has the higher stream priority: its short kernels get the SM slots that
-// the running bucket kernel frees, instead of queueing behind it.
+// the last group's tail is exposed.  `seq` is the slot's high-priority side stream (common.cuh, msm_side): its short kernels
+// get the SM slots that the running bucket kernel frees, instead of queueing behind it.  `acc` is the slot's stream, which
+// the inputs and the result are ordered on.
 //
 // Several input PARTS (host-staged MSMs, api.cu): the pairs arrive over PCIe in `nparts` pieces.  Every part is sorted on
 // its own (digits / scan / task tables / scatter on seq as soon as its scalars are there) and its bucket kernel ADDS into
@@ -558,285 +690,167 @@ struct MsmPart {
 // part p + 1 hides behind the bucket kernel of part p and the reduction / Horner tail runs once.  (Two complete MSMs
 // on two streams instead -- two bucket sets, two tails -- were slower.)
 template <class F>
-static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, const MsmPart* parts, unsigned nparts,
-                        void* d_out, const char* acc_name, unsigned tab_c = 0) {
-    const int ch = ms.channel;
-    size_t nev = 0;
-    auto next_event = [&]() { return msm_event(ctx, ch, nev++); };
-    size_t n = 0, n_max = 0;                                 // all parts together / the largest part
-    for (unsigned p = 0; p < nparts; ++p) { n += parts[p].n; n_max = parts[p].n > n_max ? parts[p].n : n_max; }
+static int msm_dev_impl(b200zk_ctx* ctx, Slot& sl, const MsmPart* parts, unsigned nparts, unsigned tab_c, unsigned seg, void* d_out) {
+    MsmPlan pl;
+    B2_TRY(msm_plan(ctx, parts, nparts, tab_c, seg, pl));
     xyzz_t<F>* out = reinterpret_cast<xyzz_t<F>*>(d_out);
-    if (n == 0) return launch(ctx, ms.acc, "msm_small", k_set_identity<F>, 1, 32, 0, out);
-    if (n >= (1ull << 31)) return set_error(ctx, B200ZK_ERR_ARG, "MSM length must be < 2^31");
-    // tab_c != 0: the bases are a fixed-base table of msm_table_windows(tab_c) x n points (section 7); all digit windows
-    // then share one bucket set and the Horner chain disappears
-    const bool fold = tab_c != 0;
-    if (fold && nparts != 1) return set_error(ctx, B200ZK_ERR_ARG, "fixed-base tables take one input part");
-    const unsigned c = fold ? tab_c : choose_window(n);
-    // every other MSM splits its scalars (glv.cuh; G2: the same split, phi = (beta^2 x, y))
-    const unsigned Wh = (128 + c - 1) / c;                   // |k1|, |k2| < 2^127: Wh * c >= 128 leaves the carry room
-    const unsigned W = fold ? msm_table_windows(c) : 2 * Wh; // digit windows
-    const unsigned WB = fold ? 1 : W;                        // bucket sets
-    if ((uint64_t)W * n >= (fold ? (1ull << 31) : (1ull << 32)))
-        return set_error(ctx, B200ZK_ERR_ARG, "MSM too large for 32-bit bucket offsets / entry indices (W * n)");
-    const uint32_t B = 1u << (c - 1);
-    const uint32_t nb = WB * B;
-    uint32_t seg_len = B < 16 ? B : 16;
-    // Small bucket sets (<= 8192 16-bucket segments in all: a 30 k-point MSM, the small windows of a 2^16 one) are reduced by one
-    // QUAD per segment (k_msm_reduce_segments_quad) and, being pure latency chains, in 8-bucket segments whatever the caller's
-    // hint: 16 + ~16 dependent point operations per segment instead of 64 + ~15 with the 32-bucket segments a 2^20 proof prefers.
-    const bool quad_reduce = (uint64_t)WB * (B / seg_len) <= 8192;
-    if (quad_reduce) seg_len = B < 8 ? B : 8;
-    else if (ctx->msm_seg_hint && ctx->msm_seg_hint <= B) seg_len = ctx->msm_seg_hint;
-    const uint32_t nseg = B / seg_len;
-    // fold (one bucket set): the segment partials are summed by `wsplit` blocks whose results the Horner kernel adds up
-    const uint32_t wsplit = fold ? (nseg >= 16 * 256 ? 16 : (nseg >= 1024 ? 4 : 1)) : 1;
-
-    // window groups: consecutive bucket sets (whole windows, i.e. both GLV halves).  Measured on an earlier GPU:
-    // at 2^20 the extra launches, the drain bubble at the end of every bucket kernel and the slowdown of the latency-bound
-    // tail kernels when they share SMs with a bucket kernel cost more than the hidden tail saves (1 group beats 2 and 4);
-    // from 2^22 up four groups win; uneven groups lose.  Fixed-base tables have one bucket set;
-    // several input parts already cut the bucket work into pieces.
-    const unsigned unit_sets = fold ? 1 : 2;
-    const unsigned units = fold ? 1 : Wh;                    // windows
-    unsigned ngroups = 1;
-    if (!fold && nparts == 1 && n >= (1u << 22)) ngroups = units < 4 ? units : 4;
-    auto group_first_unit = [&](unsigned g) { return (unsigned)(((uint64_t)units * g) / ngroups); };   // balanced split
-    const uint32_t rmw = nparts > 1 ? 1u : 0u;               // bucket kernels add into the shared buckets
+    const cudaStream_t ast = sl.stream;
+    if (pl.n == 0) return launch(ctx, ast, "msm_small", k_set_identity<F>, 1, 32, 0, out);
 
     // Streams.  One group and one part (every MSM of a proof, the 2^20 benchmark point): nothing to overlap inside the MSM, so
     // everything runs in order on the caller's stream -- a high-priority side stream would only let this MSM's
     // reductions take SM time from the bucket kernels of the proof's other MSMs (measured: a slower 2^20 proof).
     // Otherwise `seq` (the side stream) runs sort + tail and `acc` the bucket kernels.
-    const bool split_streams = ngroups > 1 || nparts > 1;
-    const cudaStream_t st = split_streams ? ms.seq : ms.acc, ast = ms.acc;
-    if (split_streams) {                  // inputs were produced in `acc`-stream order
-        cudaEvent_t e = next_event();
-        if (!e) return set_error(ctx, B200ZK_ERR_CUDA, "cudaEventCreate failed");
-        B2_CUDA_OK(ctx, cudaEventRecord(e, ast));
-        B2_CUDA_OK(ctx, cudaStreamWaitEvent(st, e, 0));
-    }
-    auto finish = [&]() -> int {          // the result (written on seq) becomes visible in `acc`-stream order
-        if (split_streams) {
-            cudaEvent_t e = next_event();
-            if (!e) return set_error(ctx, B200ZK_ERR_CUDA, "cudaEventCreate failed");
-            B2_CUDA_OK(ctx, cudaEventRecord(e, st));
-            B2_CUDA_OK(ctx, cudaStreamWaitEvent(ast, e, 0));
+    const int ch = (int)(&sl - ctx->slots);
+    const bool split_streams = pl.ngroups > 1 || nparts > 1;
+    const cudaStream_t st = split_streams ? ctx->msm_side[ch] : ast;
+    // e = the next event of the slot's pool (grown on demand, only touched under the slot's mutex), recorded on `from`
+    size_t nev = 0;
+    auto record = [&](cudaStream_t from, cudaEvent_t& e) -> int {
+        std::vector<cudaEvent_t>& pool = ctx->msm_events[ch];
+        if (nev == pool.size()) {
+            cudaEvent_t fresh = nullptr;
+            if (cudaEventCreateWithFlags(&fresh, cudaEventDisableTiming) != cudaSuccess)
+                return set_error(ctx, B200ZK_ERR_CUDA, "cudaEventCreate failed");
+            pool.push_back(fresh);
         }
+        e = pool[nev++];
+        B2_CUDA_OK(ctx, cudaEventRecord(e, from));
         return B200ZK_OK;
     };
-
-    // workspace carve-up (256-byte aligned): the sort arrays once per part, the bucket set and the reduction buffers once
-    auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-    // task length: 128 unless the average bucket is already that long (n >> 2^c: every bucket would be cut in two);
-    // then the next power of two above 3x the average -- only outliers are split -- as long as that leaves enough
-    // tasks (>= 2^19) to fill the machine
-    const size_t total_max = (size_t)W * n_max;
-    uint32_t task_len = TASK_LEN;
-    while (task_len < MAX_TASK_LEN && (uint64_t)task_len * nb < 3 * (uint64_t)total_max &&
-           total_max / (2 * task_len) + nb >= (1u << 19))
-        task_len *= 2;
-    // Small inputs cannot fill the machine with 128-entry tasks, and a real witness (29 821 of the 29 823 entries of the
-    // reference's sha256 witness are 0 or 1, groth16/examples/sha256.rs:182-185) puts thousands of entries into ONE bucket:
-    // 118 serial chains of 128 additions for a 30 k-point MSM.  Shorter tasks turn that bucket into ~900 parallel
-    // chains of 16 plus a block-level tree (k_msm_merge_tasks); buckets that stay below 16 entries are unaffected.
-    if (n_max <= (1u << 16))
-        while (task_len > 16 && total_max / task_len < (1u << 17)) task_len /= 2;
-    const size_t max_tasks = total_max / task_len + nb + ngroups;             // per part, all groups together
-    size_t o = 0;
-    auto carve = [&](size_t bytes) { size_t r = o; o += al(bytes); return r; };
-    struct PartWs { size_t keys, ranks, entries, counts, offsets, ntasks, taskoff, taskbucket, multi, hist, rank, order, tasksums; };
-    std::vector<PartWs> pw(nparts);
-    for (unsigned p = 0; p < nparts; ++p) {
-        const size_t total = (size_t)W * parts[p].n;
-        pw[p].keys = carve(total * 4); pw[p].ranks = carve(total * 4); pw[p].entries = carve(total * 4);
-        pw[p].counts = carve(((size_t)nb + 1) * 4); pw[p].offsets = carve(((size_t)nb + 1) * 4);
-        pw[p].ntasks = carve(((size_t)nb + ngroups) * 4); pw[p].taskoff = carve(((size_t)nb + ngroups) * 4);
-        pw[p].taskbucket = carve(max_tasks * 4);
-        pw[p].multi = carve((total_max / task_len + 4 * ngroups + 4) * 4);
-        pw[p].hist = carve((size_t)ngroups * (MAX_TASK_LEN + 1) * 4);
-        pw[p].rank = carve(max_tasks * 4); pw[p].order = carve(max_tasks * 4);
-        pw[p].tasksums = carve(max_tasks * sizeof(xyzz_t<F>));
-    }
-    const size_t o_sums = carve(((size_t)nb / SCAN_TILE + 2) * 4);
-    const size_t o_buckets = carve((size_t)nb * sizeof(xyzz_t<F>));
-    const size_t o_partials = carve((size_t)WB * nseg * sizeof(xyzz_t<F>));
-    const size_t o_wsum = carve((size_t)WB * wsplit * sizeof(xyzz_t<F>));
-    const size_t o_state = carve(2 * sizeof(xyzz_t<F>));
-    B2_CUDA_OK(ctx, ws_buf.reserve(o));
-    char* ws = reinterpret_cast<char*>(ws_buf.p);
-    uint32_t* sums = reinterpret_cast<uint32_t*>(ws + o_sums);
-    xyzz_t<F>* buckets = reinterpret_cast<xyzz_t<F>*>(ws + o_buckets);
-    xyzz_t<F>* partials = reinterpret_cast<xyzz_t<F>*>(ws + o_partials);
-    xyzz_t<F>* wsum = reinterpret_cast<xyzz_t<F>*>(ws + o_wsum);
-    xyzz_t<F>* hstate = reinterpret_cast<xyzz_t<F>*>(ws + o_state);
-    B2_CUDA_OK(ctx, cudaMemsetAsync(buckets, 0, (size_t)nb * sizeof(xyzz_t<F>), st));   // all-zero XYZZ = identity
-    cudaEvent_t buckets_clear = nullptr;
-    if (rmw) {                                               // the first bucket kernel reads the buckets it adds into
-        buckets_clear = next_event();
-        if (!buckets_clear) return set_error(ctx, B200ZK_ERR_CUDA, "cudaEventCreate failed");
-        B2_CUDA_OK(ctx, cudaEventRecord(buckets_clear, st));
-        B2_CUDA_OK(ctx, cudaStreamWaitEvent(ast, buckets_clear, 0));
+    cudaEvent_t e;
+    if (split_streams) {                  // inputs were produced in `acc`-stream order
+        B2_TRY(record(ast, e));
+        B2_CUDA_OK(ctx, cudaStreamWaitEvent(st, e, 0));
     }
 
-    // per-group views of the task tables (same geometry for every part)
-    struct Group {
-        uint32_t set0, nsets, b0, nbk;          // bucket sets [set0, set0 + nsets), buckets [b0, b0 + nbk)
-        size_t task_cap, task_base;             // task arrays: [task_base, task_base + task_cap)
-        uint32_t list_cap; size_t list_base;    // multi-task bucket list
-    };
-    std::vector<Group> groups(ngroups);
-    {
-        size_t tb = 0, lb = 2 * (size_t)ngroups;
-        for (unsigned g = 0; g < ngroups; ++g) {
-            Group& G = groups[g];
-            const unsigned u0 = group_first_unit(g), u1 = group_first_unit(g + 1);
-            G.set0 = u0 * unit_sets; G.nsets = (u1 - u0) * unit_sets;
-            G.b0 = G.set0 * B; G.nbk = G.nsets * B;
-            const size_t gtotal = fold ? total_max : (size_t)G.nsets * n_max;
-            G.task_cap = gtotal / task_len + G.nbk + 1;
-            G.task_base = tb; tb += G.task_cap;
-            G.list_cap = (uint32_t)(gtotal / task_len + 1);
-            G.list_base = lb; lb += G.list_cap;
-        }
+    MsmWorkspace<F> ws;
+    B2_TRY(msm_workspace(ctx, sl.ws_msm, pl, parts, ws));
+    B2_CUDA_OK(ctx, cudaMemsetAsync(ws.buckets, 0, (size_t)pl.nb * sizeof(xyzz_t<F>), st));   // all-zero XYZZ = identity
+    if (pl.rmw) {                         // the first bucket kernel reads the buckets it adds into
+        B2_TRY(record(st, e));
+        B2_CUDA_OK(ctx, cudaStreamWaitEvent(ast, e, 0));
     }
-    std::vector<cudaEvent_t> prepped((size_t)nparts * ngroups), accumulated((size_t)nparts * ngroups);
-    for (auto& e : prepped) if (!(e = next_event())) return set_error(ctx, B200ZK_ERR_CUDA, "cudaEventCreate failed");
-    for (auto& e : accumulated) if (!(e = next_event())) return set_error(ctx, B200ZK_ERR_CUDA, "cudaEventCreate failed");
 
+    const unsigned ngroups = pl.ngroups;
+    std::vector<cudaEvent_t> accumulated((size_t)nparts * ngroups);     // [p * ngroups + g]: accumulate(g) of part p is done
+    const char* acc_name = sizeof(F) > 32 ? "msm_accumulate_g2" : "msm_accumulate_g1";
+    const uint32_t wave = (uint32_t)ctx->sm_count * (sizeof(F) > 32 ? ACC_MINBLOCKS_G2 : ACC_MINBLOCKS);
     for (unsigned p = 0; p < nparts; ++p) {
         const MsmPart& P = parts[p];
-        const size_t np = P.n, total = (size_t)W * np;
-        uint32_t* keys = reinterpret_cast<uint32_t*>(ws + pw[p].keys);
-        uint32_t* ranks = reinterpret_cast<uint32_t*>(ws + pw[p].ranks);
-        uint32_t* entries = reinterpret_cast<uint32_t*>(ws + pw[p].entries);
-        uint32_t* counts = reinterpret_cast<uint32_t*>(ws + pw[p].counts);
-        uint32_t* offsets = reinterpret_cast<uint32_t*>(ws + pw[p].offsets);
-        uint32_t* ntasks_all = reinterpret_cast<uint32_t*>(ws + pw[p].ntasks);
-        uint32_t* task_off_all = reinterpret_cast<uint32_t*>(ws + pw[p].taskoff);
-        uint32_t* task_bucket_all = reinterpret_cast<uint32_t*>(ws + pw[p].taskbucket);
-        uint32_t* multi_all = reinterpret_cast<uint32_t*>(ws + pw[p].multi);
-        uint32_t* hist_all = reinterpret_cast<uint32_t*>(ws + pw[p].hist);
-        uint32_t* task_rank_all = reinterpret_cast<uint32_t*>(ws + pw[p].rank);
-        uint32_t* order_all = reinterpret_cast<uint32_t*>(ws + pw[p].order);
-        xyzz_t<F>* task_sums_all = reinterpret_cast<xyzz_t<F>*>(ws + pw[p].tasksums);
+        const typename MsmWorkspace<F>::Part& w = ws.part[p];
+        const size_t np = P.n, total = (size_t)pl.W * np;
         if (np == 0) {                                           // nothing to add: keep the event chain intact
-            for (unsigned g = 0; g < ngroups; ++g) {
-                B2_CUDA_OK(ctx, cudaEventRecord(prepped[(size_t)p * ngroups + g], st));
-                B2_CUDA_OK(ctx, cudaEventRecord(accumulated[(size_t)p * ngroups + g], ast));
-            }
+            for (unsigned g = 0; g < ngroups; ++g) B2_TRY(record(ast, accumulated[(size_t)p * ngroups + g]));
             continue;
         }
         // ---- digits + scan of part p on seq (its scalars may still be arriving) ----------------------------------------------
         if (P.scalars_ready) B2_CUDA_OK(ctx, cudaStreamWaitEvent(st, P.scalars_ready, 0));
-        B2_CUDA_OK(ctx, cudaMemsetAsync(counts, 0, ((size_t)nb + 1) * 4, st));
-        B2_TRY(launch(ctx, st, "msm_digits", fold ? k_msm_digits : k_msm_digits_glv, (unsigned)((np + 255) / 256), 256, 0,
-                      reinterpret_cast<const Fr*>(P.scalars), (uint32_t)np, c, fold ? W : Wh, keys, ranks, counts));
-        B2_TRY(exclusive_scan(ctx, st, counts, offsets, sums, nb + 1));
-        B2_CUDA_OK(ctx, cudaMemsetAsync(multi_all, 0, (size_t)ngroups * 8, st));          // [2 g], [2 g + 1] = big / small counts
-        B2_CUDA_OK(ctx, cudaMemsetAsync(hist_all, 0, (size_t)ngroups * (MAX_TASK_LEN + 1) * 4, st));
+        B2_CUDA_OK(ctx, cudaMemsetAsync(w.counts, 0, ((size_t)pl.nb + 1) * 4, st));
+        B2_TRY(launch(ctx, st, "msm_digits", pl.fold ? k_msm_digits : k_msm_digits_glv, (unsigned)((np + 255) / 256), 256, 0,
+                      reinterpret_cast<const Fr*>(P.scalars), (uint32_t)np, pl.c, pl.fold ? pl.W : pl.Wh, w.keys, w.ranks, w.counts));
+        B2_TRY(exclusive_scan(ctx, st, w.counts, w.offsets, ws.sums, pl.nb + 1));
+        B2_CUDA_OK(ctx, cudaMemsetAsync(w.multi, 0, (size_t)ngroups * 8, st));             // [2 g], [2 g + 1] = big / small counts
+        B2_CUDA_OK(ctx, cudaMemsetAsync(w.hist, 0, (size_t)ngroups * (MAX_TASK_LEN + 1) * 4, st));
 
         // ---- prep(g): task tables (counting sort of the <= task_len-entry tasks by length) + scatter, on seq ----------------
+        cudaEvent_t prepped[4];
         for (unsigned g = 0; g < ngroups; ++g) {
-            const Group& G = groups[g];
-            uint32_t* ntasks = ntasks_all + G.b0 + g;               // nbk + 1 entries per group
-            uint32_t* task_off = task_off_all + G.b0 + g;
-            uint32_t* task_bucket = task_bucket_all + G.task_base;
-            uint32_t* task_rank = task_rank_all + G.task_base;
-            uint32_t* order = order_all + G.task_base;
-            uint32_t* hist = hist_all + (size_t)g * (MAX_TASK_LEN + 1);
+            const MsmPlan::Group& G = pl.group[g];
+            uint32_t* ntasks = w.ntasks + G.b0 + g;
+            uint32_t* task_off = w.task_off + G.b0 + g;
+            uint32_t* task_bucket = w.task_bucket + G.task_base;
+            uint32_t* task_rank = w.task_rank + G.task_base;
+            uint32_t* order = w.order + G.task_base;
+            uint32_t* hist = w.hist + (size_t)g * (MAX_TASK_LEN + 1);
             const unsigned task_grid = (unsigned)((G.task_cap + 255) / 256);
-            B2_TRY(launch(ctx, st, "msm_tasks", k_msm_task_counts, (G.nbk + 1 + 255) / 256, 256, 0, offsets + G.b0, G.nbk, task_len, ntasks));
-            B2_TRY(exclusive_scan(ctx, st, ntasks, task_off, sums, G.nbk + 1));
+            B2_TRY(launch(ctx, st, "msm_tasks", k_msm_task_counts, (G.nbk + 1 + 255) / 256, 256, 0, w.offsets + G.b0, G.nbk, pl.task_len,
+                          ntasks));
+            B2_TRY(exclusive_scan(ctx, st, ntasks, task_off, ws.sums, G.nbk + 1));
             B2_TRY(launch(ctx, st, "msm_tasks", k_msm_fill_tasks, (G.nbk + 255) / 256, 256, 0, task_off, G.nbk, task_bucket,
-                          multi_all + G.list_base, G.list_cap, multi_all + 2 * g));
-            B2_TRY(launch(ctx, st, "msm_tasks", k_msm_task_hist, task_grid, 256, 0, offsets + G.b0, task_off, task_bucket, G.nbk, task_len,
-                          hist, task_rank));
-            B2_TRY(launch(ctx, st, "msm_tasks", k_msm_task_hist_scan, 1, 1, 0, hist, task_len));
-            B2_TRY(launch(ctx, st, "msm_tasks", k_msm_task_order, task_grid, 256, 0, offsets + G.b0, task_off, task_bucket, G.nbk, task_len,
-                          hist, task_rank, order));
-            const size_t t0 = fold ? 0 : (size_t)G.set0 * np, cnt = fold ? total : (size_t)G.nsets * np;
-            B2_TRY(launch(ctx, st, "msm_scatter", k_msm_scatter, (unsigned)((cnt + 255) / 256), 256, 0, keys, ranks, offsets, (uint32_t)np, t0,
-                          cnt, fold ? 1u : 0u, entries));
-            B2_CUDA_OK(ctx, cudaEventRecord(prepped[(size_t)p * ngroups + g], st));
+                          w.multi + G.list_base, G.list_cap, w.multi + 2 * g));
+            B2_TRY(launch(ctx, st, "msm_tasks", k_msm_task_hist, task_grid, 256, 0, w.offsets + G.b0, task_off, task_bucket, G.nbk,
+                          pl.task_len, hist, task_rank));
+            B2_TRY(launch(ctx, st, "msm_tasks", k_msm_task_hist_scan, 1, 1, 0, hist, pl.task_len));
+            B2_TRY(launch(ctx, st, "msm_tasks", k_msm_task_order, task_grid, 256, 0, w.offsets + G.b0, task_off, task_bucket, G.nbk,
+                          pl.task_len, hist, task_rank, order));
+            const size_t t0 = pl.fold ? 0 : (size_t)G.set0 * np, cnt = pl.fold ? total : (size_t)G.nsets * np;
+            B2_TRY(launch(ctx, st, "msm_scatter", k_msm_scatter, (unsigned)((cnt + 255) / 256), 256, 0, w.keys, w.ranks, w.offsets,
+                          (uint32_t)np, t0, cnt, pl.fold ? 1u : 0u, w.entries));
+            B2_TRY(record(st, prepped[g]));
         }
 
         // ---- accumulate(g) of part p on acc: the sort phases above only read the scalars, the (2-4x larger) base array of a
         //      host-staged part may still be on its way and signals its arrival here ------------------------------------------------
         if (P.bases_ready) B2_CUDA_OK(ctx, cudaStreamWaitEvent(ast, P.bases_ready, 0));
         for (unsigned g = 0; g < ngroups; ++g) {
-            const Group& G = groups[g];
-            B2_CUDA_OK(ctx, cudaStreamWaitEvent(ast, prepped[(size_t)p * ngroups + g], 0));
-            const uint32_t wave = (uint32_t)ctx->sm_count * (sizeof(F) > 32 ? ACC_MINBLOCKS_G2 : ACC_MINBLOCKS);
-            B2_TRY(launch(ctx, ast, acc_name, rmw ? k_msm_accumulate<F, true> : k_msm_accumulate<F, false>,
-                          (unsigned)((G.task_cap + 127) / 128), 128, 0, reinterpret_cast<const affine_t<F>*>(P.bases), entries,
-                          offsets + G.b0, task_off_all + G.b0 + g, task_bucket_all + G.task_base, order_all + G.task_base, G.nbk,
-                          task_len, wave, buckets + G.b0, task_sums_all + G.task_base));
-            if (rmw) {
+            const MsmPlan::Group& G = pl.group[g];
+            B2_CUDA_OK(ctx, cudaStreamWaitEvent(ast, prepped[g], 0));
+            B2_TRY(launch(ctx, ast, acc_name, pl.rmw ? k_msm_accumulate<F, true> : k_msm_accumulate<F, false>,
+                          (unsigned)((G.task_cap + 127) / 128), 128, 0, reinterpret_cast<const affine_t<F>*>(P.bases), w.entries,
+                          w.offsets + G.b0, w.task_off + G.b0 + g, w.task_bucket + G.task_base, w.order + G.task_base, G.nbk,
+                          pl.task_len, wave, ws.buckets + G.b0, w.task_sums + G.task_base));
+            if (pl.rmw) {
                 // several parts: the next part's bucket kernel reads what this part's merges write, so they stay on `acc`
-                B2_TRY(launch(ctx, ast, "msm_merge", k_msm_merge_tasks<F>, 2 * ctx->sm_count, 128, 0, multi_all + G.list_base, multi_all + 2 * g,
-                              task_off_all + G.b0 + g, task_sums_all + G.task_base, rmw, buckets + G.b0));
-                B2_TRY(launch(ctx, ast, "msm_merge", k_msm_merge_small<F>, 4 * ctx->sm_count, 128, 0, multi_all + G.list_base, G.list_cap,
-                              multi_all + 2 * g + 1, task_off_all + G.b0 + g, task_sums_all + G.task_base, rmw, buckets + G.b0));
+                B2_TRY(launch(ctx, ast, "msm_merge", k_msm_merge_tasks<F>, 2 * ctx->sm_count, 128, 0, w.multi + G.list_base,
+                              w.multi + 2 * g, w.task_off + G.b0 + g, w.task_sums + G.task_base, pl.rmw, ws.buckets + G.b0));
+                B2_TRY(launch(ctx, ast, "msm_merge", k_msm_merge_small<F>, 4 * ctx->sm_count, 128, 0, w.multi + G.list_base, G.list_cap,
+                              w.multi + 2 * g + 1, w.task_off + G.b0 + g, w.task_sums + G.task_base, pl.rmw, ws.buckets + G.b0));
             }
-            B2_CUDA_OK(ctx, cudaEventRecord(accumulated[(size_t)p * ngroups + g], ast));
+            B2_TRY(record(ast, accumulated[(size_t)p * ngroups + g]));
         }
     }
+
     // ---- tail(g) on seq: merge, bucket reduction, window sums, Horner step ----------------------------------------------
     for (unsigned g = 0; g < ngroups; ++g) {
-        const Group& G = groups[g];
+        const MsmPlan::Group& G = pl.group[g];
         for (unsigned p = 0; p < nparts; ++p) B2_CUDA_OK(ctx, cudaStreamWaitEvent(st, accumulated[(size_t)p * ngroups + g], 0));
-        if (!rmw) {
-            uint32_t* multi_all = reinterpret_cast<uint32_t*>(ws + pw[0].multi);
-            uint32_t* task_off = reinterpret_cast<uint32_t*>(ws + pw[0].taskoff) + G.b0 + g;
-            xyzz_t<F>* task_sums = reinterpret_cast<xyzz_t<F>*>(ws + pw[0].tasksums) + G.task_base;
-            B2_TRY(launch(ctx, st, "msm_merge", k_msm_merge_tasks<F>, 2 * ctx->sm_count, 128, 0, multi_all + G.list_base, multi_all + 2 * g,
-                          task_off, task_sums, 0u, buckets + G.b0));
-            B2_TRY(launch(ctx, st, "msm_merge", k_msm_merge_small<F>, 4 * ctx->sm_count, 128, 0, multi_all + G.list_base, G.list_cap,
-                          multi_all + 2 * g + 1, task_off, task_sums, 0u, buckets + G.b0));
+        if (!pl.rmw) {
+            const typename MsmWorkspace<F>::Part& w = ws.part[0];
+            B2_TRY(launch(ctx, st, "msm_merge", k_msm_merge_tasks<F>, 2 * ctx->sm_count, 128, 0, w.multi + G.list_base, w.multi + 2 * g,
+                          w.task_off + G.b0 + g, w.task_sums + G.task_base, 0u, ws.buckets + G.b0));
+            B2_TRY(launch(ctx, st, "msm_merge", k_msm_merge_small<F>, 4 * ctx->sm_count, 128, 0, w.multi + G.list_base, G.list_cap,
+                          w.multi + 2 * g + 1, w.task_off + G.b0 + g, w.task_sums + G.task_base, 0u, ws.buckets + G.b0));
         }
-        xyzz_t<F>* group_partials = partials + (size_t)G.set0 * nseg;
-        if (quad_reduce)                                           // latency-bound: fewer segments than the machine has warps
-            B2_TRY(launch(ctx, st, "msm_reduce", k_msm_reduce_segments_quad<F>, (G.nsets * nseg * 4 + 127) / 128, 128, 0, buckets + G.b0,
-                          G.nsets, B, seg_len, group_partials));
+        xyzz_t<F>* group_partials = ws.partials + (size_t)G.set0 * pl.nseg;
+        if (pl.quad_reduce)                                        // latency-bound: fewer segments than the machine has warps
+            B2_TRY(launch(ctx, st, "msm_reduce", k_msm_reduce_segments_quad<F>, (G.nsets * pl.nseg * 4 + 127) / 128, 128, 0,
+                          ws.buckets + G.b0, G.nsets, pl.B, pl.seg_len, group_partials));
         else
-            B2_TRY(launch(ctx, st, "msm_reduce", k_msm_reduce_segments<F>, (G.nsets * nseg + 127) / 128, 128, 0, buckets + G.b0, G.nsets, B,
-                          seg_len, group_partials));
+            B2_TRY(launch(ctx, st, "msm_reduce", k_msm_reduce_segments<F>, (G.nsets * pl.nseg + 127) / 128, 128, 0, ws.buckets + G.b0,
+                          G.nsets, pl.B, pl.seg_len, group_partials));
         // fold: the single bucket set's partials are summed by `wsplit` blocks, then added up by the Horner kernel with zero
         // doublings per step
         constexpr int T = sizeof(F) > 32 ? 128 : 256;
-        B2_TRY(launch(ctx, st, "msm_window_sum", k_msm_window_sum<F, T>, G.nsets * wsplit, T, 0, group_partials, nseg / wsplit,
-                      wsum + (size_t)G.set0 * wsplit));
+        B2_TRY(launch(ctx, st, "msm_window_sum", k_msm_window_sum<F, T>, G.nsets * pl.wsplit, T, 0, group_partials, pl.nseg / pl.wsplit,
+                      ws.wsum + (size_t)G.set0 * pl.wsplit));
         const uint32_t first = g == 0, last = g + 1 == ngroups;
-        if (fold) B2_TRY(launch(ctx, st, "msm_combine", k_msm_horner<F>, 1, 32, 0, wsum, wsplit, 0u, first, last, hstate, out));
-        else B2_TRY(launch(ctx, st, "msm_combine", k_msm_horner_glv<F>, 1, 32, 0, wsum + G.set0, G.nsets / 2, c, first, last, hstate, out));
+        if (pl.fold)
+            B2_TRY(launch(ctx, st, "msm_combine", k_msm_horner<F>, 1, 32, 0, ws.wsum, pl.wsplit, 0u, first, last, ws.hstate, out));
+        else
+            B2_TRY(launch(ctx, st, "msm_combine", k_msm_horner_glv<F>, 1, 32, 0, ws.wsum + G.set0, G.nsets / 2, pl.c, first, last,
+                          ws.hstate, out));
     }
-    return finish();
+    if (split_streams) {                  // the result (written on seq) becomes visible in `acc`-stream order
+        B2_TRY(record(st, e));
+        B2_CUDA_OK(ctx, cudaStreamWaitEvent(ast, e, 0));
+    }
+    return B200ZK_OK;
 }
 
 // single-part convenience wrapper
 template <class F>
-static int msm_dev_impl(b200zk_ctx* ctx, const MsmStreams& ms, DevBuf& ws_buf, const void* d_bases, const void* d_scalars, size_t n,
-                        void* d_out, const char* acc_name, cudaEvent_t bases_ready, cudaEvent_t scalars_ready = nullptr,
-                        unsigned tab_c = 0) {
-    const MsmPart part{d_bases, d_scalars, n, bases_ready, scalars_ready};
-    return msm_dev_impl<F>(ctx, ms, ws_buf, &part, 1, d_out, acc_name, tab_c);
+static int msm_dev_impl(b200zk_ctx* ctx, Slot& sl, const void* d_bases, const void* d_scalars, size_t n, unsigned tab_c, unsigned seg,
+                        void* d_out) {
+    const MsmPart part{d_bases, d_scalars, n, nullptr, nullptr};
+    return msm_dev_impl<F>(ctx, sl, &part, 1, tab_c, seg, d_out);
 }
 
-static MsmStreams slot_streams(b200zk_ctx* ctx, Slot& sl, int aux) {
-    const int ch = 2 * (int)(&sl - ctx->slots) + (aux ? 1 : 0);
-    return MsmStreams{ctx->msm_side[ch], aux ? sl.aux_stream : sl.stream, ch};
+int msm_g1_dev(b200zk_ctx* ctx, Slot& sl, const void* d_bases, const void* d_scalars, size_t n, void* d_out, unsigned seg) {
+    return msm_dev_impl<Fq>(ctx, sl, d_bases, d_scalars, n, 0, seg, d_out);
 }
-
-int msm_g1_dev(b200zk_ctx* ctx, Slot& sl, const void* d_bases, const void* d_scalars, size_t n, void* d_out,
-               cudaEvent_t bases_ready, int aux) {
-    return msm_dev_impl<Fq>(ctx, slot_streams(ctx, sl, aux), aux ? sl.ws_msm_aux : sl.ws_msm, d_bases, d_scalars, n, d_out,
-                            "msm_accumulate_g1", bases_ready);
-}
-int msm_g2_dev(b200zk_ctx* ctx, Slot& sl, const void* d_bases, const void* d_scalars, size_t n, void* d_out,
-               cudaEvent_t bases_ready, int aux) {
-    return msm_dev_impl<Fq2>(ctx, slot_streams(ctx, sl, aux), aux ? sl.ws_msm_aux : sl.ws_msm, d_bases, d_scalars, n, d_out,
-                             "msm_accumulate_g2", bases_ready);
+int msm_g2_dev(b200zk_ctx* ctx, Slot& sl, const void* d_bases, const void* d_scalars, size_t n, void* d_out, unsigned seg) {
+    return msm_dev_impl<Fq2>(ctx, sl, d_bases, d_scalars, n, 0, seg, d_out);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -892,12 +906,9 @@ int msm_table_build_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_bases, 
               : table_build_impl<Fq>(ctx, sl.stream, d_bases, n, c, d_table);
 }
 int msm_table_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_table, const void* d_scalars, size_t n, unsigned c,
-                  void* d_out, int aux) {
+                  void* d_out, unsigned seg) {
     if (c < 2 || c > 24) return set_error(ctx, B200ZK_ERR_ARG, "table window must be in [2, 24]");
-    const MsmStreams st = slot_streams(ctx, sl, aux);
-    DevBuf& ws = aux ? sl.ws_msm_aux : sl.ws_msm;
-    return g2 ? msm_dev_impl<Fq2>(ctx, st, ws, d_table, d_scalars, n, d_out, "msm_accumulate_g2", nullptr, nullptr, c)
-              : msm_dev_impl<Fq>(ctx, st, ws, d_table, d_scalars, n, d_out, "msm_accumulate_g1", nullptr, nullptr, c);
+    return g2 ? msm_dev_impl<Fq2>(ctx, sl, d_table, d_scalars, n, c, seg, d_out) : msm_dev_impl<Fq>(ctx, sl, d_table, d_scalars, n, c, seg, d_out);
 }
 
 // Host-staged MSM in `nparts` pieces (api.cu): d_bases / d_scalars are the device staging buffers the caller is filling on its copy
@@ -914,8 +925,7 @@ int msm_parts_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_bases, const 
                            ev_bases ? ev_bases[p] : nullptr, ev_scalars ? ev_scalars[p] : nullptr};
         lo += cnt[p];
     }
-    return g2 ? msm_dev_impl<Fq2>(ctx, slot_streams(ctx, sl, 0), sl.ws_msm, parts, nparts, d_out, "msm_accumulate_g2")
-              : msm_dev_impl<Fq>(ctx, slot_streams(ctx, sl, 0), sl.ws_msm, parts, nparts, d_out, "msm_accumulate_g1");
+    return g2 ? msm_dev_impl<Fq2>(ctx, sl, parts, nparts, 0, 0, d_out) : msm_dev_impl<Fq>(ctx, sl, parts, nparts, 0, 0, d_out);
 }
 
 // out = sum of `count` XYZZ points at pts[i * stride] (no normalisation): combines gathered per-rank partials

@@ -151,9 +151,9 @@ int pk_tables_build(b200zk_ctx* ctx, Slot& sl, const void* const src[5], const s
 }
 
 int query_msm(b200zk_ctx* ctx, Slot& sl, int k, const void* query, void* const tab[5], const unsigned tab_c[5], const Fr* scalars,
-              size_t n, void* out) {
-    if (tab_c[k]) return msm_table_dev(ctx, sl, k == 2, tab[k], scalars, n, tab_c[k], out);
-    return k == 2 ? msm_g2_dev(ctx, sl, query, scalars, n, out) : msm_g1_dev(ctx, sl, query, scalars, n, out);
+              size_t n, void* out, unsigned seg) {
+    if (tab_c[k]) return msm_table_dev(ctx, sl, k == 2, tab[k], scalars, n, tab_c[k], out, seg);
+    return k == 2 ? msm_g2_dev(ctx, sl, query, scalars, n, out, seg) : msm_g1_dev(ctx, sl, query, scalars, n, out, seg);
 }
 
 // c = 0: msm_table_auto_window(n) per query (B200ZK_PK_TABLE_WINDOW overrides)
@@ -234,19 +234,18 @@ int prove_dev(b200zk_ctx* ctx, const b200zk_pk* pk, const Fr* d_z, const Fr* d_a
     // One stream pair per MSM with bucket kernels at the lowest priority and the h pipeline at the highest was measured
     // and lost at 2^20: it removes the idle stretches of this schedule, but the proof is bound by total multiplier work
     // and the reductions then compete with the bucket kernels (tools/prove_timeline.py).
-    ctx->msm_seg_hint = 32;            // bucket reduction in 32-bucket segments: 21% fewer group operations than 16, and
+    const unsigned seg = 32;           // bucket reduction in 32-bucket segments: 21% fewer group operations than 16, and
                                        // its longer dependency chains are hidden by the concurrent MSMs
-    int rc = query_msm(ctx, s1, 2, b2q + 128, pk->tab, pk->tab_c, d_z + 1, n1, sm + o_b2);
-    if (!rc) rc = query_msm(ctx, s2, 0, aq + 64, pk->tab, pk->tab_c, d_z + 1, n1, sm + o_a);
-    if (!rc) rc = query_msm(ctx, s2, 3, pk->l_query, pk->tab, pk->tab_c, d_z + pk->n_inputs, n_aux, sm + o_l);
-    if (!rc && need_b1) rc = query_msm(ctx, s2, 1, b1q + 64, pk->tab, pk->tab_c, d_z + 1, n1, sm + o_b1);
+    int rc = query_msm(ctx, s1, 2, b2q + 128, pk->tab, pk->tab_c, d_z + 1, n1, sm + o_b2, seg);
+    if (!rc) rc = query_msm(ctx, s2, 0, aq + 64, pk->tab, pk->tab_c, d_z + 1, n1, sm + o_a, seg);
+    if (!rc) rc = query_msm(ctx, s2, 3, pk->l_query, pk->tab, pk->tab_c, d_z + pk->n_inputs, n_aux, sm + o_l, seg);
+    if (!rc && need_b1) rc = query_msm(ctx, s2, 1, b1q + 64, pk->tab, pk->tab_c, d_z + 1, n1, sm + o_b1, seg);
     if (!rc) rc = h_circom_dev(ctx, s0, d_a, d_b, d_c, log_m, d_h);
-    if (!rc) rc = query_msm(ctx, s0, 4, pk->h_query, pk->tab, pk->tab_c, d_h, m, sm + o_h);
+    if (!rc) rc = query_msm(ctx, s0, 4, pk->h_query, pk->tab, pk->tab_c, d_h, m, sm + o_h, seg);
     cudaEventRecord(ev1, s1.stream);
     cudaEventRecord(ev2, s2.stream);
     cudaStreamWaitEvent(st, ev1, 0);
     cudaStreamWaitEvent(st, ev2, 0);
-    ctx->msm_seg_hint = 0;
     if (!rc) rc = finalize_dev(ctx, s0, pk, sm + o_a, sm + o_b2, sm + o_l, sm + o_h, need_b1 ? sm + o_b1 : nullptr, 1, proof_out);
     if (rc) cudaStreamSynchronize(st);
     cudaEventDestroy(ev_in); cudaEventDestroy(ev1); cudaEventDestroy(ev2);

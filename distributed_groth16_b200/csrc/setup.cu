@@ -149,8 +149,8 @@ static int points_spmv_impl(b200zk_ctx* ctx, Slot& sl, const uint32_t* d_ptr, co
             const size_t b = ptr[r], len = ptr[r + 1] - ptr[r];
             B2_TRY(launch(ctx, st, "points_gather", k_points_gather<F>, (unsigned)((len + 255) / 256), 256, 0, d_idx + b, d_points, len,
                           gathered));
-            B2_TRY(sizeof(F) > 32 ? msm_g2_dev(ctx, sl, gathered, d_val + b, len, msm_out)
-                                  : msm_g1_dev(ctx, sl, gathered, d_val + b, len, msm_out));
+            B2_TRY(sizeof(F) > 32 ? msm_g2_dev(ctx, sl, gathered, d_val + b, len, msm_out, 0)
+                                  : msm_g1_dev(ctx, sl, gathered, d_val + b, len, msm_out, 0));
             B2_TRY(launch(ctx, st, "xyzz_to_affine", k_xyzz_to_affine_one<F>, 1, 32, 0, reinterpret_cast<const xyzz_t<F>*>(msm_out),
                           d_out + r));
         }
