@@ -129,6 +129,11 @@ SIGNATURES = {
     "b200zk_group_pk_free": (None, [c_vp, c_vp]),
     "b200zk_group_pk_table_bytes": (ctypes.c_size_t, [c_vp]),
     "b200zk_group_groth16_prove": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b200zk_group_r1cs_upload": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, ctypes.c_size_t, ctypes.c_size_t,
+                                                ctypes.c_size_t, ctypes.c_uint, ctypes.c_int, ctypes.POINTER(c_vp)]),
+    "b200zk_group_r1cs_free": (None, [c_vp, c_vp]),
+    "b200zk_group_r1cs_local_row_ptr": (ctypes.c_int, [c_vp, ctypes.c_size_t, ctypes.c_uint, ctypes.c_int, ctypes.c_int, c_vp]),
+    "b200zk_group_groth16_prove_r1cs_dev": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b200zk_fr_op": (ctypes.c_int, [c_vp, ctypes.c_int, c_vp, c_vp, c_vp, ctypes.c_size_t]),
     "b200zk_test_field_op": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, c_vp, c_vp, ctypes.c_size_t]),
     "b200zk_test_arith": (ctypes.c_int, [c_vp, ctypes.c_int, c_vp, ctypes.c_size_t, c_vp]),

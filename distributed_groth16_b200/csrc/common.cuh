@@ -214,6 +214,12 @@ int fr_convert_dev(b200zk_ctx* ctx, Slot& sl, const void* d_in, void* d_out, siz
 int qap_dev(b200zk_ctx* ctx, Slot& sl, const void* a_ptr, const void* a_col, const void* a_val, const void* b_ptr,
             const void* b_col, const void* b_val, size_t nc, size_t n_inputs, const void* d_z, unsigned log_m, void* d_a,
             void* d_b, void* d_c);
+// The same mat-vec over n_slots output slots of a column-layout slice (qap.cu, QapSlots): slot j holds global row
+// (j mod 2^log_rows) 2^log_cols + c0 + j div 2^log_rows, the matrices' CSR row j holds that row's terms.  The caller checks
+// the domain.
+int qap_slots_dev(b200zk_ctx* ctx, Slot& sl, const void* a_ptr, const void* a_col, const void* a_val, const void* b_ptr,
+                  const void* b_col, const void* b_val, size_t nc, size_t n_inputs, const void* d_z, unsigned log_rows,
+                  unsigned log_cols, size_t c0, size_t n_slots, void* d_a, void* d_b, void* d_c);
 int r1cs_check_dev(b200zk_ctx* ctx, Slot& sl, const void* const ptr[3], const void* const col[3], const void* const val[3], size_t nc,
                    const void* d_w, uint64_t* n_failed, uint64_t* first_failed);
 // setup.cu

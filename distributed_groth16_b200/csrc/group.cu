@@ -9,6 +9,8 @@
 //                                                          the all-to-all -- then row NTTs)
 //   ext_wit::h      groth16/src/ext_wit.rs:16-101         -> b200zk_group_h_circom      (3 inverse + 3 forward sharded transforms)
 //   prove::{A,B,C}  groth16/src/prove.rs:21-136 + sha256.rs:208-212 -> b200zk_group_groth16_prove (BASELINE config 5)
+//   qap::qap + prove  groth16/src/qap.rs:44-91 + the above       -> b200zk_group_groth16_prove_r1cs_dev (the R1CS sharded by
+//                                                          output slot: each GPU computes its column-layout slice of a, b, c)
 // It is the C++ port of distributed_groth16_b200/parallel.py (the torch.distributed orchestration used by bench.py under
 // torchrun): same layouts, same kernels (ntt.cu / msm.cu / prove.cu entry points), the NCCL collectives replaced by peer
 // stores and cross-device events because everything lives in one address space.  The host thread only enqueues: all
@@ -48,6 +50,20 @@ struct b200zk_group_pk {
     std::vector<Shard> shard;
     b200zk_pk* pk0 = nullptr;         // device 0: vk points for the final assembly
     size_t table_bytes = 0;
+    const b200zk_group* owner = nullptr;
+};
+
+struct b200zk_group_r1cs {
+    const b200zk_group* owner = nullptr;
+    size_t nc = 0, n_inputs = 0, n_vars = 0, m = 0;
+    unsigned log_m = 0;
+    // per device: A and B (k = 0, 1) in CSR form over the m / P output slots of its column-layout slice, Montgomery values
+    struct Shard {
+        void* ptr[2] = {};
+        void* col[2] = {};
+        void* val[2] = {};
+    };
+    std::vector<Shard> shard;
 };
 
 namespace {
@@ -284,6 +300,88 @@ int sharded_h(b200zk_group* grp, Fr* const* a, Fr* const* b, Fr* const* c, Fr* c
     return B200ZK_OK;
 }
 
+// Slot j of GPU g's column-layout slice holds global row (j mod rows) cols + g cols / P + j div rows (local[c rows + r] =
+// x[r cols + g cg + c]); qap.cu's global_row is the device twin
+size_t slot_row(size_t j, unsigned log_rows, unsigned log_cols, int P, int g) {
+    return ((j & (((size_t)1 << log_rows) - 1)) << log_cols) + (size_t)g * (((size_t)1 << log_cols) / P) + (j >> log_rows);
+}
+
+// The m / P + 1 entries of GPU g's slice CSR row_ptr from the global one (num_constraints + 1 entries; global rows >=
+// num_constraints have no terms).  Host only.
+void fill_local_row_ptr(const uint32_t* row_ptr, size_t nc, unsigned log_rows, unsigned log_cols, int P, int g, uint32_t* lptr) {
+    const size_t n = ((size_t)1 << (log_rows + log_cols)) / P;
+    lptr[0] = 0;
+    for (size_t j = 0; j < n; ++j) {
+        const size_t i = slot_row(j, log_rows, log_cols, P, g);
+        lptr[j + 1] = lptr[j] + (i < nc ? row_ptr[i + 1] - row_ptr[i] : 0);
+    }
+}
+
+// A CSR matrix from outside the program: row_ptr starts at 0 and never decreases, every column is < n_vars (the QAP kernel
+// gathers z[col] unchecked)
+int check_csr(b200zk_group* grp, const char* name, const uint32_t* row_ptr, const uint32_t* col, const uint64_t* val, size_t nc,
+              size_t n_vars) {
+    if (row_ptr[0] != 0) return gerr(grp, B200ZK_ERR_ARG, std::string("matrix ") + name + ": row_ptr[0] is " + std::to_string(row_ptr[0]) + ", not 0");
+    for (size_t i = 0; i < nc; ++i)
+        if (row_ptr[i + 1] < row_ptr[i])
+            return gerr(grp, B200ZK_ERR_ARG, std::string("matrix ") + name + ": row_ptr decreases at constraint " + std::to_string(i));
+    const size_t nnz = row_ptr[nc];
+    if (nnz && (!col || !val)) return gerr(grp, B200ZK_ERR_ARG, std::string("matrix ") + name + ": null col or val with terms");
+    for (size_t i = 0; i < nc; ++i)
+        for (size_t k = row_ptr[i]; k < row_ptr[i + 1]; ++k)
+            if (col[k] >= n_vars)
+                return gerr(grp, B200ZK_ERR_ARG, std::string("matrix ") + name + ": term " + std::to_string(k) + " (constraint " + std::to_string(i) +
+                                                     ") has column " + std::to_string(col[k]) + " >= n_vars " + std::to_string(n_vars));
+    return B200ZK_OK;
+}
+
+// The prover from a, b, c already in the column layout on the devices (a, b, c, t1, t2: loc Fr each per device; t2 ends up
+// holding h): sharded h, five partial MSMs per device, peer copies of the partials to device 0, sums and assembly there.
+// zq[g] = z[v0, v1) and zl[g] = z[n_inputs + l0, n_inputs + l1) of device g's key shard.  The caller holds the slot locks and
+// has reserved every device's small buffer (4 KB).
+int prove_columns(b200zk_group* grp, const b200zk_group_pk* pk, Fr* const* va, Fr* const* vb, Fr* const* vc, Fr* const* t1, Fr* const* t2,
+                  const Fr* const* zq, const Fr* const* zl, const uint64_t r[4], const uint64_t s[4], uint8_t proof_out[128]) {
+    const int P = grp->n;
+    const bool need_b1 = (r[0] | r[1] | r[2] | r[3]) != 0;
+    int rc = sharded_h(grp, va, vb, vc, t1, t2, pk->log_m, t2);
+    if (rc) return rc;
+    // partial MSMs: small[0..16) A, [16..32) L, [32..48) H, [48..64) B1 (u64 words), [64..96) B2
+    for (int g = 0; g < P; ++g) {
+        b200zk_ctx* ctx = grp->ctx[g];
+        Slot& sl = ctx->slots[0];
+        const b200zk_group_pk::Shard& S = pk->shard[g];
+        G_CUDA_OK(grp, cudaSetDevice(ctx->device));
+        char* sm = reinterpret_cast<char*>(sl.small.p);
+        auto msm = [&](int k, const Fr* scalars, size_t n, void* out) {
+            return query_msm(ctx, sl, k, S.q[k], S.tab, S.tab_c, scalars, n, out, 0);
+        };
+        G_TRY(grp, g, msm(2, zq[g], S.v1 - S.v0, sm + 512));                    // the G2 MSM first: the longest
+        G_TRY(grp, g, msm(0, zq[g], S.v1 - S.v0, sm + 0));
+        G_TRY(grp, g, msm(3, zl[g], S.l1 - S.l0, sm + 128));
+        G_TRY(grp, g, msm(4, t2[g], S.hn, sm + 256));
+        if (need_b1) G_TRY(grp, g, msm(1, zq[g], S.v1 - S.v0, sm + 384));
+        else G_CUDA_OK(grp, cudaMemsetAsync(sm + 384, 0, 128, sl.stream));
+        G_CUDA_OK(grp, cudaEventRecord(grp->ev_done[g], sl.stream));
+    }
+    // gather on device 0, add up, assemble (the sharded MSMs ran over index 0 too: z[0] = 1 makes a_query[0] z[0] the term the
+    // reference's driver adds, sha256.rs:208-212 -> include_zero_terms = 0)
+    b200zk_ctx* c0 = grp->ctx[0];
+    Slot& s0 = c0->slots[0];
+    G_CUDA_OK(grp, cudaSetDevice(c0->device));
+    G_CUDA_OK(grp, s0.io_b.reserve((size_t)(P + 1) * 768));
+    char* gathered = reinterpret_cast<char*>(s0.io_b.p);
+    char* tot = gathered + (size_t)P * 768;
+    for (int g = 0; g < P; ++g) {
+        if (g) G_CUDA_OK(grp, cudaStreamWaitEvent(s0.stream, grp->ev_done[g], 0));
+        G_CUDA_OK(grp, cudaMemcpyPeerAsync(gathered + (size_t)g * 768, c0->device, grp->ctx[g]->slots[0].small.p, grp->ctx[g]->device, 768, s0.stream));
+    }
+    for (int k = 0; k < 4; ++k) G_TRY(grp, 0, xyzz_sum_dev(c0, s0, 0, gathered + k * 128, P, 6, tot + k * 128));      // stride: 768 B = 6 G1 XYZZ
+    G_TRY(grp, 0, xyzz_sum_dev(c0, s0, 1, gathered + 512, P, 3, tot + 512));                                          // 3 G2 XYZZ
+    rc = gfrom(grp, 0, assemble_dev(c0, s0, pk->pk0, tot, tot + 512, tot + 128, tot + 256, need_b1 ? tot + 384 : nullptr, r, s, 0, proof_out));
+    if (rc) return rc;
+    return sync_all(grp);
+}
+
 }  // namespace
 
 extern "C" {
@@ -439,7 +537,7 @@ int b200zk_group_pk_upload(b200zk_group* grp, const uint64_t* a_query, const uin
     if (cols < (size_t)P) return gerr(grp, B200ZK_ERR_ARG, "domain too small for this many GPUs");
     SlotLocks locks(grp);
     b200zk_group_pk* pk = new b200zk_group_pk();
-    pk->n = P; pk->n_vars = n_vars; pk->n_inputs = n_inputs; pk->m = m; pk->log_m = log_m;
+    pk->n = P; pk->n_vars = n_vars; pk->n_inputs = n_inputs; pk->m = m; pk->log_m = log_m; pk->owner = grp;
     pk->shard.resize(P);
     const size_t n_aux = n_vars - n_inputs;
     const bool want_tables = pk_tables_enabled();
@@ -506,10 +604,10 @@ int b200zk_group_groth16_prove(b200zk_group* grp, const b200zk_group_pk* pk, con
     unsigned log_rows, log_cols;
     split_log(log_m, &log_rows, &log_cols);
     const size_t rows = (size_t)1 << log_rows, cols = (size_t)1 << log_cols, m = pk->m, loc = m / P;
-    const bool need_b1 = (r[0] | r[1] | r[2] | r[3]) != 0;
     SlotLocks locks(grp);
     // staging per device: a, b, c (column layout) + 2 temporaries (t2 ends up holding h), then this device's rows of z
-    std::vector<void*> va(P), vb(P), vc(P), t1(P), t2(P), vz(P);
+    std::vector<void*> va(P), vb(P), vc(P), t1(P), t2(P);
+    std::vector<const Fr*> zq(P), zl(P);
     for (int g = 0; g < P; ++g) {
         b200zk_ctx* ctx = grp->ctx[g];
         const b200zk_group_pk::Shard& S = pk->shard[g];
@@ -518,10 +616,11 @@ int b200zk_group_groth16_prove(b200zk_group* grp, const b200zk_group_pk* pk, con
         G_CUDA_OK(grp, ctx->slots[0].io_a.reserve((5 * loc + (S.v1 - S.v0) + (S.l1 - S.l0) + zrows) * sizeof(Fr)));
         G_CUDA_OK(grp, ctx->slots[0].small.reserve(4096));
         Fr* p = reinterpret_cast<Fr*>(ctx->slots[0].io_a.p);
-        va[g] = p; vb[g] = p + loc; vc[g] = p + 2 * loc; t1[g] = p + 3 * loc; t2[g] = p + 4 * loc; vz[g] = p + 5 * loc;
+        va[g] = p; vb[g] = p + loc; vc[g] = p + 2 * loc; t1[g] = p + 3 * loc; t2[g] = p + 4 * loc;
         cudaStream_t st = ctx->slots[0].stream;
-        Fr* dz = reinterpret_cast<Fr*>(vz[g]);
+        Fr* dz = p + 5 * loc;
         Fr* dzaux = dz + (S.v1 - S.v0);
+        zq[g] = dz; zl[g] = dzaux;
         G_CUDA_OK(grp, cudaMemcpyAsync(dz, reinterpret_cast<const char*>(z) + S.v0 * 32, (S.v1 - S.v0) * 32, cudaMemcpyHostToDevice, st));
         G_CUDA_OK(grp, cudaMemcpyAsync(dzaux, reinterpret_cast<const char*>(z) + (pk->n_inputs + S.l0) * 32, (S.l1 - S.l0) * 32, cudaMemcpyHostToDevice, st));
     }
@@ -529,46 +628,150 @@ int b200zk_group_groth16_prove(b200zk_group* grp, const b200zk_group_pk* pk, con
     if (!rc) rc = scatter_columns<Blob32>(grp, b, rows, cols, t1.data(), vb.data());
     if (!rc) rc = scatter_columns<Blob32>(grp, c, rows, cols, t1.data(), vc.data());
     if (rc) return rc;
-    rc = sharded_h(grp, reinterpret_cast<Fr* const*>(va.data()), reinterpret_cast<Fr* const*>(vb.data()), reinterpret_cast<Fr* const*>(vc.data()),
-                   reinterpret_cast<Fr* const*>(t1.data()), reinterpret_cast<Fr* const*>(t2.data()), log_m, reinterpret_cast<Fr* const*>(t2.data()));
-    if (rc) return rc;
-    // partial MSMs: small[0..16) A, [16..32) L, [32..48) H, [48..64) B1 (u64 words), [64..96) B2
+    auto fr = [](std::vector<void*>& v) { return reinterpret_cast<Fr* const*>(v.data()); };
+    return prove_columns(grp, pk, fr(va), fr(vb), fr(vc), fr(t1), fr(t2), zq.data(), zl.data(), r, s, proof_out);
+}
+
+// ---- R1CS sharded by output slot + prove from the witness on device 0 ---------------------------------------------------------
+int b200zk_group_r1cs_local_row_ptr(const uint32_t* row_ptr, size_t num_constraints, unsigned log_m, int n_gpus, int rank,
+                                    uint32_t* local_row_ptr) {
+    if (!row_ptr || !local_row_ptr || n_gpus < 1 || n_gpus > 8 || (n_gpus & (n_gpus - 1)) || rank < 0 || rank >= n_gpus) return B200ZK_ERR_ARG;
+    if (log_m > 27 || num_constraints > ((size_t)1 << log_m)) return B200ZK_ERR_DOMAIN;
+    unsigned log_rows, log_cols;
+    split_log(log_m, &log_rows, &log_cols);
+    if (((size_t)1 << log_cols) < (size_t)n_gpus) return B200ZK_ERR_ARG;
+    fill_local_row_ptr(row_ptr, num_constraints, log_rows, log_cols, n_gpus, rank, local_row_ptr);
+    return B200ZK_OK;
+}
+void b200zk_group_r1cs_free(b200zk_group* grp, b200zk_group_r1cs* q) {
+    DeviceGuard dev_guard;
+    if (!q) return;
+    for (size_t g = 0; g < q->shard.size(); ++g) {
+        if (grp && g < grp->ctx.size()) cudaSetDevice(grp->ctx[g]->device);
+        for (int k = 0; k < 2; ++k) {
+            if (q->shard[g].ptr[k]) cudaFree(q->shard[g].ptr[k]);
+            if (q->shard[g].col[k]) cudaFree(q->shard[g].col[k]);
+            if (q->shard[g].val[k]) cudaFree(q->shard[g].val[k]);
+        }
+    }
+    delete q;
+}
+
+int b200zk_group_r1cs_upload(b200zk_group* grp, const uint32_t* a_row_ptr, const uint32_t* a_col, const uint64_t* a_val,
+                             const uint32_t* b_row_ptr, const uint32_t* b_col, const uint64_t* b_val, size_t num_constraints,
+                             size_t num_inputs, size_t n_vars, unsigned log_m, int values_montgomery_depth, b200zk_group_r1cs** out) {
+    DeviceGuard dev_guard;
+    if (!grp || !out || !a_row_ptr || !b_row_ptr) return B200ZK_ERR_ARG;
+    *out = nullptr;
+    if (log_m > 27) return gerr(grp, B200ZK_ERR_DOMAIN, "log_m > 27: 2m exceeds the 2^28 subgroup (PolynomialDegreeTooLarge)");
+    const size_t m = (size_t)1 << log_m, nc = num_constraints;
+    if (nc + num_inputs > m) return gerr(grp, B200ZK_ERR_DOMAIN, "num_constraints + num_inputs exceeds the domain size");
+    if (num_inputs == 0 || num_inputs > n_vars) return gerr(grp, B200ZK_ERR_ARG, "need 1 <= num_inputs <= n_vars");
+    const int P = grp->n;
+    unsigned log_rows, log_cols;
+    split_log(log_m, &log_rows, &log_cols);
+    if (((size_t)1 << log_cols) < (size_t)P) return gerr(grp, B200ZK_ERR_ARG, "domain too small for this many GPUs");
+    const uint32_t* row_ptr[2] = {a_row_ptr, b_row_ptr};
+    const uint32_t* col[2] = {a_col, b_col};
+    const uint64_t* val[2] = {a_val, b_val};
+    for (int k = 0; k < 2; ++k) {
+        int rc = check_csr(grp, k ? "B" : "A", row_ptr[k], col[k], val[k], nc, n_vars);
+        if (rc) return rc;
+    }
+    SlotLocks locks(grp);
+    b200zk_group_r1cs* q = new b200zk_group_r1cs();
+    q->owner = grp; q->nc = nc; q->n_inputs = num_inputs; q->n_vars = n_vars; q->m = m; q->log_m = log_m;
+    q->shard.resize(P);
+    auto fail = [&](int rc) { b200zk_group_r1cs_free(grp, q); return rc; };
+    const size_t loc = m / P;
+    std::vector<uint32_t> lptr(loc + 1), lcol;
+    std::vector<uint64_t> lval;
+    for (int g = 0; g < P; ++g) {
+        b200zk_ctx* ctx = grp->ctx[g];
+        Slot& sl = ctx->slots[0];
+        if (cudaSetDevice(ctx->device) != cudaSuccess) return fail(gerr(grp, B200ZK_ERR_CUDA, "cudaSetDevice failed"));
+        b200zk_group_r1cs::Shard& S = q->shard[g];
+        for (int k = 0; k < 2; ++k) {
+            // the slice's rows in slot order, gathered once on the host (index and word copies only)
+            fill_local_row_ptr(row_ptr[k], nc, log_rows, log_cols, P, g, lptr.data());
+            const size_t nnz = lptr[loc];
+            lcol.resize(nnz);
+            lval.resize(nnz * 4);
+            for (size_t j = 0; j < loc; ++j) {
+                const size_t i = slot_row(j, log_rows, log_cols, P, g);
+                if (i >= nc || row_ptr[k][i + 1] == row_ptr[k][i]) continue;
+                const size_t lo = row_ptr[k][i], n = row_ptr[k][i + 1] - lo;
+                memcpy(lcol.data() + lptr[j], col[k] + lo, n * sizeof(uint32_t));
+                memcpy(lval.data() + (size_t)lptr[j] * 4, val[k] + lo * 4, n * 32);
+            }
+            if (cudaMalloc(&S.ptr[k], (loc + 1) * sizeof(uint32_t)) != cudaSuccess || cudaMalloc(&S.col[k], nnz * sizeof(uint32_t) + 16) != cudaSuccess ||
+                cudaMalloc(&S.val[k], nnz * 32 + 16) != cudaSuccess)
+                return fail(gerr(grp, B200ZK_ERR_OOM, "constraint-matrix shard allocation failed"));
+            // pageable sources: each copy has consumed its source when the call returns, so the host vectors can be refilled
+            if (cudaMemcpyAsync(S.ptr[k], lptr.data(), (loc + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, sl.stream) != cudaSuccess ||
+                (nnz && cudaMemcpyAsync(S.col[k], lcol.data(), nnz * sizeof(uint32_t), cudaMemcpyHostToDevice, sl.stream) != cudaSuccess) ||
+                (nnz && cudaMemcpyAsync(S.val[k], lval.data(), nnz * 32, cudaMemcpyHostToDevice, sl.stream) != cudaSuccess))
+                return fail(gerr(grp, B200ZK_ERR_CUDA, "constraint-matrix upload failed"));
+            if (values_montgomery_depth != 0) {
+                const int to_mont = values_montgomery_depth < 0, times = to_mont ? -values_montgomery_depth : values_montgomery_depth;
+                int rc = gfrom(grp, g, fr_convert_dev(ctx, sl, S.val[k], S.val[k], nnz, to_mont, times));
+                if (rc) return fail(rc);
+            }
+        }
+    }
+    int rc = sync_all(grp);
+    if (rc) return fail(rc);
+    *out = q;
+    return B200ZK_OK;
+}
+
+int b200zk_group_groth16_prove_r1cs_dev(b200zk_group* grp, const b200zk_group_pk* pk, const b200zk_group_r1cs* q, const void* d_z,
+                                        const uint64_t r[4], const uint64_t s[4], uint8_t proof_out[128]) {
+    DeviceGuard dev_guard;
+    if (!grp || !pk || !q || !d_z || !r || !s || !proof_out) return B200ZK_ERR_ARG;
+    if (pk->owner != grp) return gerr(grp, B200ZK_ERR_ARG, "proving key was uploaded to a different group");
+    if (q->owner != grp) return gerr(grp, B200ZK_ERR_ARG, "constraint matrices were uploaded to a different group");
+    if (q->m != pk->m)
+        return gerr(grp, B200ZK_ERR_DOMAIN, "constraint matrices of domain " + std::to_string(q->m) + ", proving key of domain " + std::to_string(pk->m));
+    if (q->n_inputs != pk->n_inputs)
+        return gerr(grp, B200ZK_ERR_ARG, "constraint matrices with " + std::to_string(q->n_inputs) + " inputs, proving key with " + std::to_string(pk->n_inputs));
+    if (q->n_vars != pk->n_vars)
+        return gerr(grp, B200ZK_ERR_ARG, "constraint matrices over " + std::to_string(q->n_vars) + " variables, proving key over " + std::to_string(pk->n_vars));
+    const int P = grp->n;
+    unsigned log_rows, log_cols;
+    split_log(pk->log_m, &log_rows, &log_cols);
+    const size_t cg = ((size_t)1 << log_cols) / P, loc = pk->m / P, zbytes = pk->n_vars * sizeof(Fr);
+    SlotLocks locks(grp);
+    // the caller wrote z on device 0's slot-0 stream: every other device's copy of it waits for that point
+    b200zk_ctx* c0 = grp->ctx[0];
+    G_CUDA_OK(grp, cudaSetDevice(c0->device));
+    G_CUDA_OK(grp, cudaEventRecord(grp->ev_done[0], c0->slots[0].stream));
+    // per device: a, b, c (column layout, written by the mat-vec) + 2 temporaries (t2 ends up holding h), then (devices >= 1) z
+    std::vector<void*> va(P), vb(P), vc(P), t1(P), t2(P);
+    std::vector<const Fr*> zq(P), zl(P);
     for (int g = 0; g < P; ++g) {
         b200zk_ctx* ctx = grp->ctx[g];
         Slot& sl = ctx->slots[0];
         const b200zk_group_pk::Shard& S = pk->shard[g];
+        const b200zk_group_r1cs::Shard& Q = q->shard[g];
         G_CUDA_OK(grp, cudaSetDevice(ctx->device));
-        char* sm = reinterpret_cast<char*>(sl.small.p);
-        const Fr* dz = reinterpret_cast<const Fr*>(vz[g]);
-        const Fr* dzaux = dz + (S.v1 - S.v0);
-        auto msm = [&](int k, const Fr* scalars, size_t n, void* out) {
-            return query_msm(ctx, sl, k, S.q[k], S.tab, S.tab_c, scalars, n, out, 0);
-        };
-        G_TRY(grp, g, msm(2, dz, S.v1 - S.v0, sm + 512));                       // the G2 MSM first: the longest
-        G_TRY(grp, g, msm(0, dz, S.v1 - S.v0, sm + 0));
-        G_TRY(grp, g, msm(3, dzaux, S.l1 - S.l0, sm + 128));
-        G_TRY(grp, g, msm(4, reinterpret_cast<const Fr*>(t2[g]), S.hn, sm + 256));
-        if (need_b1) G_TRY(grp, g, msm(1, dz, S.v1 - S.v0, sm + 384));
-        else G_CUDA_OK(grp, cudaMemsetAsync(sm + 384, 0, 128, sl.stream));
-        G_CUDA_OK(grp, cudaEventRecord(grp->ev_done[g], sl.stream));
+        G_CUDA_OK(grp, sl.io_a.reserve(5 * loc * sizeof(Fr) + (g ? zbytes : 0)));
+        G_CUDA_OK(grp, sl.small.reserve(4096));
+        Fr* p = reinterpret_cast<Fr*>(sl.io_a.p);
+        va[g] = p; vb[g] = p + loc; vc[g] = p + 2 * loc; t1[g] = p + 3 * loc; t2[g] = p + 4 * loc;
+        const Fr* z = reinterpret_cast<const Fr*>(d_z);
+        if (g) {
+            G_CUDA_OK(grp, cudaStreamWaitEvent(sl.stream, grp->ev_done[0], 0));
+            G_CUDA_OK(grp, cudaMemcpyPeerAsync(p + 5 * loc, ctx->device, d_z, c0->device, zbytes, sl.stream));
+            z = p + 5 * loc;
+        }
+        zq[g] = z + S.v0;
+        zl[g] = z + pk->n_inputs + S.l0;
+        G_TRY(grp, g, qap_slots_dev(ctx, sl, Q.ptr[0], Q.col[0], Q.val[0], Q.ptr[1], Q.col[1], Q.val[1], q->nc, q->n_inputs, z, log_rows, log_cols,
+                                    (size_t)g * cg, loc, va[g], vb[g], vc[g]));
     }
-    // gather on device 0, add up, assemble (the sharded MSMs ran over index 0 too: z[0] = 1 makes a_query[0] z[0] the term the
-    // reference's driver adds, sha256.rs:208-212 -> include_zero_terms = 0)
-    b200zk_ctx* c0 = grp->ctx[0];
-    Slot& s0 = c0->slots[0];
-    G_CUDA_OK(grp, cudaSetDevice(c0->device));
-    G_CUDA_OK(grp, s0.io_b.reserve((size_t)(P + 1) * 768));
-    char* gathered = reinterpret_cast<char*>(s0.io_b.p);
-    char* tot = gathered + (size_t)P * 768;
-    for (int g = 0; g < P; ++g) {
-        if (g) G_CUDA_OK(grp, cudaStreamWaitEvent(s0.stream, grp->ev_done[g], 0));
-        G_CUDA_OK(grp, cudaMemcpyPeerAsync(gathered + (size_t)g * 768, c0->device, grp->ctx[g]->slots[0].small.p, grp->ctx[g]->device, 768, s0.stream));
-    }
-    for (int k = 0; k < 4; ++k) G_TRY(grp, 0, xyzz_sum_dev(c0, s0, 0, gathered + k * 128, P, 6, tot + k * 128));      // stride: 768 B = 6 G1 XYZZ
-    G_TRY(grp, 0, xyzz_sum_dev(c0, s0, 1, gathered + 512, P, 3, tot + 512));                                          // 3 G2 XYZZ
-    rc = gfrom(grp, 0, assemble_dev(c0, s0, pk->pk0, tot, tot + 512, tot + 128, tot + 256, need_b1 ? tot + 384 : nullptr, r, s, 0, proof_out));
-    if (rc) return rc;
-    return sync_all(grp);
+    auto fr = [](std::vector<void*>& v) { return reinterpret_cast<Fr* const*>(v.data()); };
+    return prove_columns(grp, pk, fr(va), fr(vb), fr(vc), fr(t1), fr(t2), zq.data(), zl.data(), r, s, proof_out);
 }
 
 }  // extern "C"

@@ -25,19 +25,31 @@ __device__ __forceinline__ Fr row_dot(const uint32_t* ptr, const uint32_t* col, 
     return acc;
 }
 
+// The output slots of one mat-vec launch: slot j holds global row i = (j mod 2^log_rows) 2^log_cols + c0 + j div 2^log_rows, and
+// the matrices hold, at CSR row j, the terms of that global row.  The one-GPU QAP writes the whole domain in natural order
+// (log_rows = log m, log_cols = 0, c0 = 0: i = j); GPU g of a group writes its slice of the column layout of group.cu
+// (log_rows, log_cols = the four-step split of the domain, c0 = g cols / P, n = m / P).
+struct QapSlots {
+    uint32_t n, log_rows, log_cols, c0;
+};
+__device__ __forceinline__ uint32_t global_row(const QapSlots& s, uint32_t j) {
+    return ((j & ((1u << s.log_rows) - 1)) << s.log_cols) + s.c0 + (j >> s.log_rows);
+}
+
 __global__ void k_qap(const uint32_t* a_ptr, const uint32_t* a_col, const Fr* a_val, const uint32_t* b_ptr, const uint32_t* b_col,
-                      const Fr* b_val, const Fr* z, uint32_t nc, uint32_t n_inputs, uint32_t m, Fr* a, Fr* b, Fr* c) {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m) return;
+                      const Fr* b_val, const Fr* z, uint32_t nc, uint32_t n_inputs, QapSlots s, Fr* a, Fr* b, Fr* c) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= s.n) return;
+    const uint32_t i = global_row(s, j);
     Fr va = Fr::zero(), vb = Fr::zero(), vc = Fr::zero();
     if (i < nc) {
-        va = row_dot(a_ptr, a_col, a_val, z, i);
-        vb = row_dot(b_ptr, b_col, b_val, z, i);
+        va = row_dot(a_ptr, a_col, a_val, z, j);
+        vb = row_dot(b_ptr, b_col, b_val, z, j);
         vc = Fr::mul(va, vb);
     } else if (i < nc + n_inputs) {
         va = ld16(z + (i - nc));
     }
-    st16(a + i, va); st16(b + i, vb); st16(c + i, vc);
+    st16(a + j, va); st16(b + j, vb); st16(c + j, vc);
 }
 
 // One warp per row: the lanes stride over the row's non-zeros and the partial sums meet in a shuffle tree.  Small circuits have
@@ -60,18 +72,19 @@ __device__ __forceinline__ Fr row_dot_warp(const uint32_t* ptr, const uint32_t* 
 }
 __global__ void __launch_bounds__(256) k_qap_warp(const uint32_t* a_ptr, const uint32_t* a_col, const Fr* a_val, const uint32_t* b_ptr,
                                                   const uint32_t* b_col, const Fr* b_val, const Fr* z, uint32_t nc, uint32_t n_inputs,
-                                                  uint32_t m, Fr* a, Fr* b, Fr* c) {
-    const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (i >= m) return;
+                                                  QapSlots s, Fr* a, Fr* b, Fr* c) {
+    const uint32_t j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (j >= s.n) return;
+    const uint32_t i = global_row(s, j);
     Fr va = Fr::zero(), vb = Fr::zero(), vc = Fr::zero();
     if (i < nc) {
-        va = row_dot_warp(a_ptr, a_col, a_val, z, i, lane);
-        vb = row_dot_warp(b_ptr, b_col, b_val, z, i, lane);
+        va = row_dot_warp(a_ptr, a_col, a_val, z, j, lane);
+        vb = row_dot_warp(b_ptr, b_col, b_val, z, j, lane);
         vc = Fr::mul(va, vb);
     } else if (i < nc + n_inputs) {
         va = ld16(z + (i - nc));
     }
-    if (lane == 0) { st16(a + i, va); st16(b + i, vb); st16(c + i, vc); }
+    if (lane == 0) { st16(a + j, va); st16(b + j, vb); st16(c + j, vc); }
 }
 
 int fr_convert_dev(b200zk_ctx* ctx, Slot& sl, const void* d_in, void* d_out, size_t n, int to_mont, int times) {
@@ -80,17 +93,25 @@ int fr_convert_dev(b200zk_ctx* ctx, Slot& sl, const void* d_in, void* d_out, siz
                   times);
 }
 
+int qap_slots_dev(b200zk_ctx* ctx, Slot& sl, const void* a_ptr, const void* a_col, const void* a_val, const void* b_ptr,
+                  const void* b_col, const void* b_val, size_t nc, size_t n_inputs, const void* d_z, unsigned log_rows,
+                  unsigned log_cols, size_t c0, size_t n_slots, void* d_a, void* d_b, void* d_c) {
+    if (n_slots == 0) return B200ZK_OK;
+    const uint32_t *ap = (const uint32_t*)a_ptr, *ac = (const uint32_t*)a_col, *bp = (const uint32_t*)b_ptr, *bc = (const uint32_t*)b_col;
+    const QapSlots s{(uint32_t)n_slots, log_rows, log_cols, (uint32_t)c0};
+    const bool warp = n_slots <= ((size_t)1 << 18);     // warp per row while rows x 32 lanes still fit a few waves
+    return launch(ctx, sl.stream, "qap_matvec", warp ? k_qap_warp : k_qap,
+                  (unsigned)(warp ? (n_slots * 32 + 255) / 256 : (n_slots + 127) / 128), warp ? 256 : 128, 0, ap, ac, (const Fr*)a_val,
+                  bp, bc, (const Fr*)b_val, (const Fr*)d_z, (uint32_t)nc, (uint32_t)n_inputs, s, (Fr*)d_a, (Fr*)d_b, (Fr*)d_c);
+}
+
 int qap_dev(b200zk_ctx* ctx, Slot& sl, const void* a_ptr, const void* a_col, const void* a_val, const void* b_ptr,
             const void* b_col, const void* b_val, size_t nc, size_t n_inputs, const void* d_z, unsigned log_m, void* d_a,
             void* d_b, void* d_c) {
     if (log_m > 28) return set_error(ctx, B200ZK_ERR_DOMAIN, "domain too large (PolynomialDegreeTooLarge)");
     size_t m = (size_t)1 << log_m;
     if (nc + n_inputs > m) return set_error(ctx, B200ZK_ERR_DOMAIN, "num_constraints + num_inputs exceeds the domain size");
-    const uint32_t *ap = (const uint32_t*)a_ptr, *ac = (const uint32_t*)a_col, *bp = (const uint32_t*)b_ptr, *bc = (const uint32_t*)b_col;
-    const bool warp = m <= ((size_t)1 << 18);          // warp per row while rows x 32 lanes still fit a few waves
-    return launch(ctx, sl.stream, "qap_matvec", warp ? k_qap_warp : k_qap, (unsigned)(warp ? (m * 32 + 255) / 256 : (m + 127) / 128),
-                  warp ? 256 : 128, 0, ap, ac, (const Fr*)a_val, bp, bc, (const Fr*)b_val, (const Fr*)d_z, (uint32_t)nc,
-                  (uint32_t)n_inputs, (uint32_t)m, (Fr*)d_a, (Fr*)d_b, (Fr*)d_c);
+    return qap_slots_dev(ctx, sl, a_ptr, a_col, a_val, b_ptr, b_col, b_val, nc, n_inputs, d_z, log_m, 0, 0, m, d_a, d_b, d_c);
 }
 
 // R1CS satisfaction (snarkjs `wtns check`): constraint i holds iff <A_i, w> <B_i, w> = <C_i, w>.  The same mat-vec as k_qap

@@ -17,12 +17,19 @@ def load_zkey(net: Net, zkey_bytes: bytes):
     zk = formats.read_zkey(zkey_bytes)
     pk = ProvingKey(net, zk.a_query, zk.b_g1_query, zk.b_g2_query, zk.l_query, zk.h_query, zk.n_inputs, zk.alpha_g1,
                     zk.beta_g1, zk.delta_g1, zk.beta_g2, zk.delta_g2)
+    a_coo, b_coo = zkey_matrices_coo(zk)
+    mats = ConstraintMatrices(net, zk.n_inputs, zk.num_constraints, a_coo, b_coo, values_montgomery_depth=1)
+    return pk, mats, zk
+
+
+def zkey_matrices_coo(zk: formats.ZKey):
+    """-> (A, B) of the zkey's coefficient section as (rows, cols, values x R^2) COO triplets; the constructors of the
+    constraint matrices keep rows < zk.num_constraints, which drops the public-input rows snarkjs appends."""
     coo = []
     for mi in (0, 1):
         sel = zk.coef_matrix == mi
         coo.append((zk.coef_row[sel], zk.coef_col[sel], zk.coef_val_r2[sel]))
-    mats = ConstraintMatrices(net, zk.n_inputs, zk.num_constraints, coo[0], coo[1], values_montgomery_depth=1)
-    return pk, mats, zk
+    return coo[0], coo[1]
 
 
 def ptau_prepare_phase2(net: Net, src_path: str, dst_path: str) -> None:
@@ -240,6 +247,35 @@ def prove_zkey_wtns(net: Net, zkey_bytes: bytes, wtns_bytes: bytes, r=None, s=No
     proof = prove_from_matrices(pk, mats, z, r, s)
     pk.free()
     return proof, w[1:1 + zk.n_public].copy()
+
+
+def prove_zkey_wtns_group(group, zkey_bytes: bytes, wtns_bytes: bytes, r=None, s=None):
+    """prove_zkey_wtns on every GPU of a group.Group: the key and the constraint matrices sharded over the GPUs, the witness
+    converted on device 0 and the QAP computed on each GPU in its column layout.  -> (proof bytes, public inputs as canonical
+    limbs (n_public, 4)), the same as prove_zkey_wtns gives on one GPU."""
+    from .. import group as grp
+    w = formats.read_wtns(wtns_bytes)
+    gpk, mats, zk = grp.load_zkey(group, zkey_bytes)
+    try:
+        if w.shape[0] != zk.n_vars:
+            raise formats.FormatError("witness has %d entries, the key expects %d" % (w.shape[0], zk.n_vars))
+        proof = gpk.create_proof_r1cs(mats, group.witness_to_device(w), r, s)
+    finally:
+        mats.free()
+        gpk.free()
+    return proof, w[1:1 + zk.n_public].copy()
+
+
+def groth16_prove_group(group, zkey_bytes: bytes, wtns_bytes: bytes, r=None, s=None):
+    """snarkjs `groth16 prove` on every GPU of a group.Group (prove_zkey_wtns_group; r, s as groth16_prove takes them).  ->
+    (text of proof.json, text of public.json), the texts groth16_prove writes on one GPU."""
+    from . import snarkjs
+    proof, public = prove_zkey_wtns_group(group, zkey_bytes, wtns_bytes, r, s)
+    net = Net(group.devices[0])
+    try:
+        return snarkjs.proof_to_json(net, proof), snarkjs.public_to_json(public)
+    finally:
+        net.close()
 
 
 def wtns_check(net: Net, r1cs_bytes: bytes, wtns_bytes: bytes):

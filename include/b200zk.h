@@ -31,6 +31,7 @@ typedef struct b200zk_ctx b200zk_ctx;
 typedef struct b200zk_pk b200zk_pk;
 typedef struct b200zk_group b200zk_group;         /* several GPUs of one box, one host process (csrc/group.cu) */
 typedef struct b200zk_group_pk b200zk_group_pk;   /* a proving key sharded over a group */
+typedef struct b200zk_group_r1cs b200zk_group_r1cs;   /* a circuit's A and B sharded over a group by QAP output slot */
 
 enum {
     B200ZK_OK = 0,
@@ -370,6 +371,31 @@ size_t b200zk_group_pk_table_bytes(const b200zk_group_pk* pk);
 int b200zk_group_groth16_prove(b200zk_group* group, const b200zk_group_pk* pk, const uint64_t* z, const uint64_t* a,
                                const uint64_t* b, const uint64_t* c, const uint64_t r[4], const uint64_t s[4],
                                uint8_t proof_out[128]);
+/* A and B of the circuit in CSR form (conventions of b200zk_qap_dev: row_ptr num_constraints + 1 x u32, col nnz x u32,
+ * val nnz x 4 limbs), for a key of domain 2^log_m (log_m <= 27) and n_vars variables.  values_montgomery_depth as
+ * groth16.qap.ConstraintMatrices: 1 = zkey words (value R^2), 0 = Montgomery, -1 = canonical; the conversion runs on each
+ * GPU after upload.  GPU g keeps the rows of its column-layout slice of the domain (rows = 2^ceil(log_m / 2),
+ * cols = 2^floor(log_m / 2), cg = cols / P: local slot c rows + r is global row r cols + g cg + c), reordered on the host once.
+ * Refused before any launch: num_constraints + num_inputs > 2^log_m or log_m > 27 (B200ZK_ERR_DOMAIN); cols < P, a column
+ * index >= n_vars (the message names the matrix and the term), a row_ptr that does not start at 0 or decreases, or
+ * num_inputs outside 1..n_vars (B200ZK_ERR_ARG). */
+int  b200zk_group_r1cs_upload(b200zk_group* group, const uint32_t* a_row_ptr, const uint32_t* a_col, const uint64_t* a_val,
+                              const uint32_t* b_row_ptr, const uint32_t* b_col, const uint64_t* b_val, size_t num_constraints,
+                              size_t num_inputs, size_t n_vars, unsigned log_m, int values_montgomery_depth,
+                              b200zk_group_r1cs** out);
+void b200zk_group_r1cs_free(b200zk_group* group, b200zk_group_r1cs* matrices);
+/* Host only (no device is touched): the 2^log_m / n_gpus + 1 entries of the CSR row_ptr that GPU `rank` of b200zk_group_r1cs_upload
+ * keeps, from the global row_ptr (num_constraints + 1 entries).  B200ZK_ERR_DOMAIN / B200ZK_ERR_ARG as the upload. */
+int  b200zk_group_r1cs_local_row_ptr(const uint32_t* row_ptr, size_t num_constraints, unsigned log_m, int n_gpus, int rank,
+                                     uint32_t* local_row_ptr);
+/* b200zk_group_groth16_prove from the witness: d_z is the full assignment (n_vars x 4 limbs, Montgomery) resident on the
+ * group's device 0 and written on the slot-0 stream of b200zk_group_ctx(group, 0).  The call copies it to every other GPU
+ * (peer copies), runs the sharded QAP (each GPU computes its column-layout slice of a, b, c), then exactly the rest of
+ * b200zk_group_groth16_prove; the host waits only for the proof bytes.  Refused before any launch: a key or matrices uploaded
+ * to another group, n_inputs or n_vars differing between key and matrices (B200ZK_ERR_ARG), different domain sizes
+ * (B200ZK_ERR_DOMAIN). */
+int  b200zk_group_groth16_prove_r1cs_dev(b200zk_group* group, const b200zk_group_pk* pk, const b200zk_group_r1cs* matrices,
+                                         const void* d_z, const uint64_t r[4], const uint64_t s[4], uint8_t proof_out[128]);
 
 /* ---- the parties' local share arithmetic (n-party compatibility mirrors, SURVEY 8f4) ----------------------------------
  * Element-wise Fr operation on host buffers of n x 4 Montgomery limbs: op 0 = a * b (share-wise product of two sharings,
