@@ -43,7 +43,8 @@ int b200zk_ctx_create(int device, b200zk_ctx** out) {
         }
         ctx->slots[i].owns_stream = true;
         bool ok = cudaStreamCreateWithFlags(&ctx->slots[i].copy_stream, cudaStreamNonBlocking) == cudaSuccess &&
-                  cudaEventCreateWithFlags(&ctx->slots[i].copy_done, cudaEventDisableTiming) == cudaSuccess;
+                  cudaEventCreateWithFlags(&ctx->slots[i].copy_done, cudaEventDisableTiming) == cudaSuccess &&
+                  cudaEventCreateWithFlags(&ctx->slots[i].rebind, cudaEventDisableTiming) == cudaSuccess;
         for (int k = 0; ok && k < 32; ++k) ok = cudaEventCreateWithFlags(&ctx->slots[i].stage_ev[k], cudaEventDisableTiming) == cudaSuccess;
         if (!ok) {
             delete ctx;
@@ -74,6 +75,7 @@ void b200zk_ctx_destroy(b200zk_ctx* ctx) {
         if (s.owns_stream && s.stream) cudaStreamDestroy(s.stream);
         if (s.copy_stream) cudaStreamDestroy(s.copy_stream);
         if (s.copy_done) cudaEventDestroy(s.copy_done);
+        if (s.rebind) cudaEventDestroy(s.rebind);
         for (int k = 0; k < 32; ++k) if (s.stage_ev[k]) cudaEventDestroy(s.stage_ev[k]);
     }
     for (int k = 0; k < 3; ++k) if (ctx->msm_side[k]) cudaStreamDestroy(ctx->msm_side[k]);
@@ -88,8 +90,23 @@ int b200zk_ctx_set_stream(b200zk_ctx* ctx, int stream, void* cuda_stream) {
     if (!ctx || !valid_slot(stream)) return B200ZK_ERR_ARG;
     Slot& s = ctx->slots[stream];
     std::lock_guard<std::mutex> g(s.mu);
-    if (s.owns_stream && s.stream) { cudaStreamSynchronize(s.stream); cudaStreamDestroy(s.stream); }
-    s.stream = reinterpret_cast<cudaStream_t>(cuda_stream);
+    cudaStream_t next = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (s.owns_stream && s.stream) {
+        cudaStreamSynchronize(s.stream);
+        cudaStreamDestroy(s.stream);
+    } else if (s.stream != next) {
+        // work already queued through this slot on the old stream still uses the slot's buffers (workspaces, staging): the
+        // new stream waits for it, without blocking the host.  The caller's current device is restored (Group._t0 calls
+        // this with another device current).
+        int prev = -1;
+        if (cudaGetDevice(&prev) != cudaSuccess) prev = -1;
+        cudaError_t e = cudaSetDevice(ctx->device);
+        if (e == cudaSuccess) e = cudaEventRecord(s.rebind, s.stream);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(next, s.rebind, 0);
+        if (prev >= 0) cudaSetDevice(prev);
+        B2_CUDA_OK(ctx, e);
+    }
+    s.stream = next;
     s.owns_stream = false;
     return B200ZK_OK;
 }
@@ -198,6 +215,9 @@ int msm_staged_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* bases, const v
     const char* hb = reinterpret_cast<const char*>(bases);
     const char* hs = reinterpret_cast<const char*>(scalars);
     cudaStream_t cs = sl.copy_stream;
+    // io_a may still be read by kernels queued on the slot's stream (the previous staged MSM of this slot): the copies wait
+    B2_CUDA_OK(ctx, cudaEventRecord(sl.copy_done, sl.stream));
+    B2_CUDA_OK(ctx, cudaStreamWaitEvent(cs, sl.copy_done, 0));
     size_t cnt[5];
     cudaEvent_t ev_s[5], ev_b[5];
     size_t lo = 0;

@@ -50,7 +50,8 @@ struct Slot {                 // one per MultiplexedStreamID
     DevBuf io_a, io_b;        // staging for host-buffer entry points
     DevBuf small;             // results
     cudaStream_t copy_stream = nullptr;   // second stream for overlapped H2D staging (host-buffer entry points)
-    cudaEvent_t copy_done = nullptr;
+    cudaEvent_t copy_done = nullptr;      // host-staged MSM: earlier work on `stream` is done with io_a (the copy stream waits)
+    cudaEvent_t rebind = nullptr;         // b200zk_ctx_set_stream: work queued on the old stream, waited on by the new one
     cudaEvent_t stage_ev[32] = {};        // host-staged MSM: arrival of part p's scalars [2 p] / bases [2 p + 1]
 };
 

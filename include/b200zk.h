@@ -47,7 +47,9 @@ int b200zk_ctx_create(int device, b200zk_ctx** out);
 void b200zk_ctx_destroy(b200zk_ctx* ctx);
 const char* b200zk_last_error(const b200zk_ctx* ctx);
 const char* b200zk_version(void);
-/* Make slot `stream` (0..2) launch on a caller-provided cudaStream_t (e.g. torch's current stream). */
+/* Make slot `stream` (0..2) launch on a caller-provided cudaStream_t (e.g. torch's current stream).  Work already queued
+ * through the slot is ordered before work on the new stream (an event wait, no host synchronisation), so the old stream
+ * must still exist when the slot is re-bound. */
 int b200zk_ctx_set_stream(b200zk_ctx* ctx, int stream, void* cuda_stream);
 int b200zk_ctx_sync(b200zk_ctx* ctx, int stream);
 /* Per-kernel CUDA-event profiling (used by bench.py for the roofline numbers). */
@@ -66,8 +68,8 @@ int b200zk_msm_g2(b200zk_ctx* ctx, int stream, const uint64_t* bases, size_t n_b
                   const uint64_t* scalars, size_t n_scalars, uint64_t out_affine[16], int* out_is_inf);
 /* Host buffers in, this GPU's partial sum out (XYZZ, device memory, ordered on slot `stream`): the input travels over PCIe in
  * parts whose bucket kernels add into one bucket set, so the transfer hides behind the compute.  The multi-GPU callers use it
- * for their index range and combine the partials (b200zk_msm_exchange_sum_dev, b200zk_group_msm_*).  Returns once the host
- * buffers may be reused. */
+ * for their index range and combine the partials (b200zk_msm_exchange_sum_dev, b200zk_group_msm_*).  The staging copies
+ * wait for earlier work on the slot's stream.  Returns once the host buffers may be reused. */
 int b200zk_msm_staged_dev(b200zk_ctx* ctx, int stream, int g2, const uint64_t* bases, size_t n_bases, const uint64_t* scalars,
                           size_t n_scalars, void* d_out_xyzz);
 /* Device buffers (inputs already resident in HBM).  `d_out_xyzz` receives the un-normalised
