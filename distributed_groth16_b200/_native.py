@@ -10,8 +10,8 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200zk.so")
 
-OK, ERR_LENGTH, ERR_DOMAIN, ERR_CUDA, ERR_ARG, ERR_OOM = range(6)
-_ERR_NAMES = {1: "BAD_LENGTH", 2: "BAD_DOMAIN", 3: "CUDA", 4: "BAD_ARG", 5: "OOM"}
+OK, ERR_LENGTH, ERR_DOMAIN, ERR_CUDA, ERR_ARG, ERR_OOM, ERR_SHORT_BUFFER = range(7)
+_ERR_NAMES = {1: "BAD_LENGTH", 2: "BAD_DOMAIN", 3: "CUDA", 4: "BAD_ARG", 5: "OOM", 6: "SHORT_BUFFER"}
 
 
 class B200zkError(RuntimeError):
@@ -94,6 +94,11 @@ SIGNATURES = {
     "b200zk_points_compress_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, ctypes.c_size_t, c_vp]),
     "b200zk_points_decompress_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, ctypes.c_size_t, ctypes.c_int, c_vp,
                                                     ctypes.POINTER(ctypes.c_size_t)]),
+    "b200zk_zkey_load": (ctypes.c_int, [c_vp, c_vp, ctypes.c_size_t, ctypes.c_uint, ctypes.POINTER(c_vp)]),
+    "b200zk_zkey_free": (None, [c_vp, c_vp]),
+    "b200zk_zkey_info": (ctypes.c_int, [c_vp] + [ctypes.POINTER(ctypes.c_size_t)] * 4),
+    "b200zk_zkey_prove": (ctypes.c_int, [c_vp, c_vp, c_vp, ctypes.c_size_t, c_vp, c_vp, c_vp, ctypes.c_char_p,
+                                         ctypes.POINTER(ctypes.c_size_t), ctypes.c_char_p, ctypes.POINTER(ctypes.c_size_t)]),
     "b200zk_xyzz_sum_dev": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, ctypes.c_size_t, ctypes.c_size_t, c_vp]),
     "b200zk_groth16_assemble_dev": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, ctypes.c_int, c_vp]),
     "b200zk_fixed_base_mul_dev": (ctypes.c_int, [c_vp, ctypes.c_int, c_vp, ctypes.c_size_t, c_vp]),

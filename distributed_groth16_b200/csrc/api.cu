@@ -3,6 +3,7 @@
 
 #include "blake2b.cuh"
 #include "common.cuh"
+#include "snarkjs_files.h"
 
 using namespace b200zk;
 
@@ -511,7 +512,7 @@ static int upload(b200zk_ctx* ctx, void** dst, const void* src, size_t bytes, cu
 
 static int pk_build(b200zk_ctx* ctx, const void* a_query, const void* b_g1_query, const void* b_g2_query, const void* l_query,
                     const void* h_query, size_t n_vars, size_t n_inputs, size_t m, const uint64_t* vk_points,
-                    cudaMemcpyKind kind, b200zk_pk** out) {
+                    cudaMemcpyKind kind, unsigned table_window, b200zk_pk** out) {
     if (!ctx || !out || !a_query || !b_g1_query || !b_g2_query || !h_query || !vk_points) return B200ZK_ERR_ARG;
     if (n_vars == 0 || n_inputs == 0 || n_inputs > n_vars) return set_error(ctx, B200ZK_ERR_ARG, "need 1 <= n_inputs <= n_vars");
     if (m == 0 || (m & (m - 1))) return set_error(ctx, B200ZK_ERR_DOMAIN, "h_query length must be a power of two");
@@ -526,8 +527,9 @@ static int pk_build(b200zk_ctx* ctx, const void* a_query, const void* b_g1_query
     if (!rc) rc = upload(ctx, &pk->vk, vk_points, 56 * 8);
     if (!rc && cudaStreamSynchronize(ctx->slots[0].stream) != cudaSuccess) rc = set_error(ctx, B200ZK_ERR_CUDA, "proving-key upload failed");
     if (rc) { b200zk_pk_free(ctx, pk); return rc; }
-    if (pk_tables_enabled()) {
-        rc = with_slot(ctx, 0, [&](Slot&) { return pk_precompute_dev(ctx, pk, 0); });
+    // table_window as b200zk_pk_precompute's c; 0 is the automatic policy, which B200ZK_PK_TABLES=0 turns off
+    if (table_window != 0xFFFFFFFFu && (table_window != 0 || pk_tables_enabled())) {
+        rc = with_slot(ctx, 0, [&](Slot&) { return pk_precompute_dev(ctx, pk, table_window); });
         if (rc) { b200zk_pk_free(ctx, pk); return rc; }
     }
     *out = pk;
@@ -538,13 +540,13 @@ int b200zk_pk_upload(b200zk_ctx* ctx, const uint64_t* a_query, const uint64_t* b
                      const uint64_t* l_query, const uint64_t* h_query, size_t n_vars, size_t n_inputs, size_t m,
                      const uint64_t* vk_points, b200zk_pk** out) {
     return pk_build(ctx, a_query, b_g1_query, b_g2_query, l_query, h_query, n_vars, n_inputs, m, vk_points,
-                    cudaMemcpyHostToDevice, out);
+                    cudaMemcpyHostToDevice, 0, out);
 }
 int b200zk_pk_upload_dev(b200zk_ctx* ctx, const void* a_query, const void* b_g1_query, const void* b_g2_query,
                          const void* l_query, const void* h_query, size_t n_vars, size_t n_inputs, size_t m,
                          const uint64_t* vk_points, b200zk_pk** out) {
     return pk_build(ctx, a_query, b_g1_query, b_g2_query, l_query, h_query, n_vars, n_inputs, m, vk_points,
-                    cudaMemcpyDeviceToDevice, out);
+                    cudaMemcpyDeviceToDevice, 0, out);
 }
 
 void b200zk_pk_free(b200zk_ctx* ctx, b200zk_pk* pk) {
@@ -586,6 +588,73 @@ int b200zk_groth16_prove_dev(b200zk_ctx* ctx, const b200zk_pk* pk, const void* d
     if (!ctx || !pk || !d_z || !d_a || !d_b || !d_c || !r || !s || !proof_out) return B200ZK_ERR_ARG;
     return with_slot(ctx, 0, [&](Slot&) {
         return prove_dev(ctx, pk, (const Fr*)d_z, (const Fr*)d_a, (const Fr*)d_b, (const Fr*)d_c, r, s, mirror_bg1, proof_out);
+    });
+}
+
+// ---- a snarkjs zkey resident in HBM (zkey.cu) ------------------------------------------------------------------------------
+void b200zk_zkey_free(b200zk_ctx* ctx, b200zk_zkey* zk) {
+    if (!zk) return;
+    if (ctx) cudaSetDevice(ctx->device);
+    if (zk->csr) cudaFree(zk->csr);
+    b200zk_pk_free(ctx, zk->pk);
+    delete zk;
+}
+
+int b200zk_zkey_load(b200zk_ctx* ctx, const void* zkey, size_t zkey_len, unsigned table_window, b200zk_zkey** out) {
+    if (!ctx) return B200ZK_ERR_ARG;
+    if (!zkey || !out) return set_error(ctx, B200ZK_ERR_ARG, "zkey_load: null pointer");
+    *out = nullptr;
+    const uint8_t* file = reinterpret_cast<const uint8_t*>(zkey);
+    sjf::Zkey h;
+    std::string err;
+    if (!sjf::parse_zkey(file, zkey_len, &h, &err)) return set_error(ctx, B200ZK_ERR_ARG, err);
+    if (h.domain_size > (1u << 27)) {
+        return set_error(ctx, B200ZK_ERR_DOMAIN, "zkey domain size " + std::to_string(h.domain_size) +
+                                                     " exceeds 2^27: the h step needs twice the domain within Fr's 2^28 subgroup");
+    }
+    b200zk_zkey* zk = new b200zk_zkey();
+    zk->n_vars = h.n_vars;
+    zk->n_public = h.n_public;
+    zk->domain_size = h.domain_size;
+    int rc = with_slot(ctx, 0, [&](Slot& sl) { return zkey_matrices_dev(ctx, sl, file, h, zk); });
+    if (!rc) {
+        // vk points in b200zk_pk_upload's order from the header's alpha_1 beta_1 beta_2 gamma_2 delta_1 delta_2; the queries go
+        // from the caller's bytes, which are already the device layout
+        const uint8_t* hp = file + h.hdr_points;
+        uint64_t vk[56];
+        memcpy(vk, hp, 128);                    // alpha_1, beta_1
+        memcpy(vk + 16, hp + 384, 64);          // delta_1
+        memcpy(vk + 24, hp + 128, 128);         // beta_2
+        memcpy(vk + 40, hp + 448, 128);         // delta_2
+        rc = pk_build(ctx, file + h.a, file + h.b1, file + h.b2, file + h.l, file + h.h, h.n_vars, (size_t)h.n_public + 1, h.domain_size,
+                      vk, cudaMemcpyHostToDevice, table_window, &zk->pk);
+    }
+    if (rc) {
+        b200zk_zkey_free(ctx, zk);
+        return rc;
+    }
+    *out = zk;
+    return B200ZK_OK;
+}
+
+int b200zk_zkey_info(const b200zk_zkey* zk, size_t* n_vars, size_t* n_public, size_t* domain_size, size_t* num_constraints) {
+    if (!zk) return B200ZK_ERR_ARG;
+    if (n_vars) *n_vars = zk->n_vars;
+    if (n_public) *n_public = zk->n_public;
+    if (domain_size) *domain_size = zk->domain_size;
+    if (num_constraints) *num_constraints = zk->num_constraints;
+    return B200ZK_OK;
+}
+
+int b200zk_zkey_prove(b200zk_ctx* ctx, const b200zk_zkey* zk, const void* wtns, size_t wtns_len, const uint64_t r[4],
+                      const uint64_t s[4], uint8_t proof_out[128], char* proof_json, size_t* proof_json_len, char* public_json,
+                      size_t* public_json_len) {
+    if (!ctx) return B200ZK_ERR_ARG;
+    if (!zk || !wtns || (proof_json && !proof_json_len) || (public_json && !public_json_len))
+        return set_error(ctx, B200ZK_ERR_ARG, "zkey_prove: null key or witness, or a JSON buffer without its length");
+    return with_slot(ctx, 0, [&](Slot& sl) {
+        return zkey_prove_dev(ctx, sl, zk, reinterpret_cast<const uint8_t*>(wtns), wtns_len, r, s, proof_out, proof_json, proof_json_len,
+                              public_json, public_json_len);
     });
 }
 

@@ -94,6 +94,18 @@ struct b200zk_pk {
     size_t tab_bytes = 0;
 };
 
+// A snarkjs Groth16 zkey resident in HBM (zkey.cu): the proving key and A, B in CSR form.  row_ptr holds 2 nc + 1 entries, A's
+// row i at entry i and B's row i at entry nc + i, both indexing col / val (val Montgomery), so b200zk_qap_dev runs on
+// (row_ptr, col, val) and (row_ptr + nc, col, val).
+struct b200zk_zkey {
+    b200zk_pk* pk = nullptr;
+    size_t n_vars = 0, n_public = 0, domain_size = 0, num_constraints = 0;
+    void* csr = nullptr;                  // one allocation behind row_ptr, val and col
+    uint32_t* row_ptr = nullptr;
+    uint32_t* col = nullptr;
+    b200zk::Fr* val = nullptr;
+};
+
 namespace b200zk {
 
 inline int set_error(b200zk_ctx* ctx, int code, const std::string& msg) {
@@ -199,6 +211,8 @@ int msm_parts_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_bases, const 
 int msm_staged_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* bases, const void* scalars, size_t n, void* d_out, bool wait_copies);
 unsigned msm_table_windows(unsigned c);
 unsigned msm_table_auto_window(size_t n);
+// exclusive prefix sum of n u32 (n < 2^32); sums: scratch of ceil(n / 2048) u32
+int exclusive_scan(b200zk_ctx* ctx, cudaStream_t st, const uint32_t* in, uint32_t* out, uint32_t* sums, uint32_t n);
 int msm_table_build_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_bases, size_t n, unsigned c, void* d_table);
 int msm_table_dev(b200zk_ctx* ctx, Slot& sl, int g2, const void* d_table, const void* d_scalars, size_t n, unsigned c,
                   void* d_out_xyzz, unsigned seg);
@@ -272,5 +286,11 @@ int query_msm(b200zk_ctx* ctx, Slot& sl, int k, const void* query, void* const t
               size_t n, void* out, unsigned seg);
 int prove_dev(b200zk_ctx* ctx, const b200zk_pk* pk, const Fr* d_z, const Fr* d_a, const Fr* d_b, const Fr* d_c,
               const uint64_t r[4], const uint64_t s[4], int mirror_bg1, uint8_t proof_out[128]);
+// zkey.cu (the header fields come from snarkjs_files.h's parse_zkey)
+namespace sjf { struct Zkey; }
+int zkey_matrices_dev(b200zk_ctx* ctx, Slot& sl, const uint8_t* file, const sjf::Zkey& h, b200zk_zkey* zk);
+int zkey_prove_dev(b200zk_ctx* ctx, Slot& sl, const b200zk_zkey* zk, const uint8_t* wtns, size_t wtns_len, const uint64_t* r,
+                   const uint64_t* s, uint8_t* proof_out, char* proof_json, size_t* proof_json_len, char* public_json,
+                   size_t* public_json_len);
 
 }  // namespace b200zk

@@ -515,7 +515,7 @@ static unsigned choose_window(size_t n) {
     return (unsigned)c;
 }
 
-static int exclusive_scan(b200zk_ctx* ctx, cudaStream_t st, const uint32_t* in, uint32_t* out, uint32_t* sums, uint32_t n) {
+int exclusive_scan(b200zk_ctx* ctx, cudaStream_t st, const uint32_t* in, uint32_t* out, uint32_t* sums, uint32_t n) {
     uint32_t nblk = (n + SCAN_TILE - 1) / SCAN_TILE;
     B2_TRY(launch(ctx, st, "msm_scan", k_scan_local, nblk, SCAN_THREADS, 0, in, out, sums, n));
     B2_TRY(launch(ctx, st, "msm_scan", k_scan_sums, 1, SCAN_THREADS, 0, sums, nblk));

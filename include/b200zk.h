@@ -32,6 +32,7 @@ typedef struct b200zk_pk b200zk_pk;
 typedef struct b200zk_group b200zk_group;         /* several GPUs of one box, one host process (csrc/group.cu) */
 typedef struct b200zk_group_pk b200zk_group_pk;   /* a proving key sharded over a group */
 typedef struct b200zk_group_r1cs b200zk_group_r1cs;   /* a circuit's A and B sharded over a group by QAP output slot */
+typedef struct b200zk_zkey b200zk_zkey;   /* a snarkjs Groth16 .zkey resident in HBM: b200zk_pk + A, B in CSR */
 
 enum {
     B200ZK_OK = 0,
@@ -39,7 +40,8 @@ enum {
     B200ZK_ERR_DOMAIN = 2,  /* log_n > 28 (Fr two-adicity) / size mismatch: `D::new` -> None, ext_wit.rs:31-32 */
     B200ZK_ERR_CUDA = 3,
     B200ZK_ERR_ARG = 4,
-    B200ZK_ERR_OOM = 5
+    B200ZK_ERR_OOM = 5,
+    B200ZK_ERR_SHORT_BUFFER = 6   /* an output buffer is too small: the *_len arguments say what is needed */
 };
 
 /* ---- context (one per GPU; the reference's per-party `Net` handle plays this role) ---------- */
@@ -244,6 +246,42 @@ int b200zk_groth16_prove(b200zk_ctx* ctx, const b200zk_pk* pk, const uint64_t* z
 int b200zk_groth16_prove_dev(b200zk_ctx* ctx, const b200zk_pk* pk, const void* d_z, const void* d_a, const void* d_b,
                              const void* d_c, const uint64_t r[4], const uint64_t s[4], int mirror_bg1,
                              uint8_t proof_out[128]);
+
+/* ---- snarkjs `groth16 prove <zkey> <wtns> <proof.json> <public.json>` from the files' bytes (csrc/zkey.cu) ---------------
+ * b200zk_zkey_load: parse a Groth16 .zkey (zkey_len bytes; the caller may unmap it on return) and keep it in HBM: the point
+ * sections go to the device as they are (Montgomery, little-endian, infinity all-zero), and the coefficient section is sorted
+ * into A and B in CSR form on the device, dropping the public-input rows snarkjs appends; num_constraints = the largest
+ * constraint index - n_public.  table_window as b200zk_pk_precompute's c: 0 = the automatic table policy of
+ * b200zk_pk_upload (B200ZK_PK_TABLES, B200ZK_PK_TABLE_MAX_GB), 0xFFFFFFFF = no fixed-base tables (a caller that proves once:
+ * the tables cost more to build than one proof saves).  Refused before any launch (B200ZK_ERR_ARG, the message of
+ * formats.read_zkey): a bad magic, a section past zkey_len, a missing or short section, a protocol other than Groth16 (1),
+ * a field other than BN254, n_public + 1 > n_vars, a domain size that is not a power of two; a domain above 2^27:
+ * B200ZK_ERR_DOMAIN.  A coefficient record with matrix > 1, signal >= n_vars or constraint >= domain size: B200ZK_ERR_ARG
+ * with the count and the first index.  Peak device memory while loading: 80 bytes per coefficient record + 16 bytes per
+ * constraint, then the proving key and its tables; held afterwards: the key, its tables, 36 bytes per record + 8 per
+ * constraint. */
+int  b200zk_zkey_load(b200zk_ctx* ctx, const void* zkey, size_t zkey_len, unsigned table_window, b200zk_zkey** out);
+void b200zk_zkey_free(b200zk_ctx* ctx, b200zk_zkey* zk);
+int  b200zk_zkey_info(const b200zk_zkey* zk, size_t* n_vars, size_t* n_public, size_t* domain_size, size_t* num_constraints);
+/* The longest proof.json plus its NUL: every coordinate below q has at most 77 digits.  The longest public.json of n public
+ * signals plus its NUL: "[", n lines of up to 77 digits in quotes, n - 1 commas, "\n]" (n = 0: "[]"). */
+#define B200ZK_PROOF_JSON_MAX 810
+#define B200ZK_PUBLIC_JSON_MAX(n_public) (3 + 82 * (size_t)(n_public))
+/* Prove from a .wtns (n8 = 32, prime = r, n_vars entries, each < r) with the key: the proof of circom.groth16_prove.
+ * r, s: 4 Montgomery limbs each (as b200zk_groth16_prove); NULL draws the value uniformly mod r from getrandom, so that the
+ * proof is zero-knowledge.  proof_out (128 bytes, ark-serialize Compress::Yes), proof_json and public_json may each be NULL.
+ * The JSON is snarkjs's text (one-space indent, no trailing newline, infinity ["0","1","0"] / [["0","0"],["1","0"],["0","0"]]),
+ * NUL-terminated; public.json holds w[1..n_public] of the witness.  *proof_json_len / *public_json_len: in, the buffer sizes;
+ * out, the text lengths without the NUL.  Buffers of B200ZK_PROOF_JSON_MAX / B200ZK_PUBLIC_JSON_MAX(n_public) bytes always
+ * suffice.  A buffer under B200ZK_PROOF_JSON_MAX / the exact public.json size + 1 is refused
+ * before any launch with B200ZK_ERR_SHORT_BUFFER, both lengths then set to the sizes needed.  Refused before any launch: a
+ * malformed wtns (B200ZK_ERR_ARG, formats.read_wtns's message), an entry count other than n_vars (B200ZK_ERR_LENGTH,
+ * "witness has N entries, the key expects M"); an entry >= r: B200ZK_ERR_ARG naming the count and the first index.  One key
+ * may prove any number of witnesses and several keys may be live on one context; calls are serialised as
+ * b200zk_groth16_prove's (slots 0, 1 and 2). */
+int  b200zk_zkey_prove(b200zk_ctx* ctx, const b200zk_zkey* zk, const void* wtns, size_t wtns_len, const uint64_t r[4],
+                       const uint64_t s[4], uint8_t proof_out[128], char* proof_json, size_t* proof_json_len, char* public_json,
+                       size_t* public_json_len);
 
 /* Multi-GPU prove building blocks: sum `count` XYZZ partials spaced `stride` points apart into one XYZZ point,
  * and run only the final assembly (prove.rs:36-44,75-83,128-134 + sha256.rs:208-212 + Compress::Yes) on MSM results
