@@ -12,8 +12,8 @@
 //   3 scatter    entries[offset[bucket] + rank] = point index | sign  (counting sort, no comparison sort)
 //   4 accumulate one thread per bucket task: gather affine points (the 2^20 x 64 B base array is larger
 //                than H100's 50 MB L2), mixed XYZZ additions
-//   5 reduce     per window sum_b b * bucket_b as segment running sums + small scalar multiples,
-//                tree-combined per window in shared memory
+//   5 reduce     per window sum_b b * bucket_b as segment running sums, the segment offsets summed per bit of the
+//                segment index, tree-combined per window in shared memory
 //   6 combine    Horner over windows (c doublings each)
 #include <type_traits>
 
@@ -347,11 +347,16 @@ __global__ void __launch_bounds__(128) k_msm_merge_small(const uint32_t* multi_l
 // ---------------------------------------------------------------------------------------------
 // 5. window reduction: S_w = sum_{k<B} (k+1) * bucket[w][k]
 // ---------------------------------------------------------------------------------------------
-// one thread per (window, segment).  (A quad-cooperative version of this kernel was measured slower at 2^20:
-// it is throughput- not latency-bound.)
+// With segments of L buckets, R_s = sum_{j<L} b_{sL+j} and A_s = sum_{j<L} (j+1) b_{sL+j}:
+//   S_w = sum_s A_s + L * sum_s s R_s = sum_s A_s + sum_b 2^(b + log2 L) C_b,   C_b = sum of R_s over the s with bit b set.
+// The segment kernel writes the pair (R_s, A_s) and multiplies nothing by its offset sL; the C_b are plain sums
+// (k_msm_window_bits), and each is doubled b + log2 L times once, by the block that sums it.
+//
+// One thread per (window, segment).  (A quad-cooperative version of this kernel was measured slower at 2^20:
+// it is throughput- not latency-bound.)  pairs[2 t] = R_s, pairs[2 t + 1] = A_s.
 template <class F>
 __global__ void __launch_bounds__(128) k_msm_reduce_segments(const xyzz_t<F>* buckets, uint32_t W, uint32_t B, uint32_t seg_len,
-                                      xyzz_t<F>* partials) {
+                                      xyzz_t<F>* pairs) {
     uint32_t nseg = B / seg_len;
     uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= W * nseg) return;
@@ -359,22 +364,53 @@ __global__ void __launch_bounds__(128) k_msm_reduce_segments(const xyzz_t<F>* bu
     uint32_t lo = seg * seg_len;
     const xyzz_t<F>* bw = buckets + (size_t)w * B;
     xyzz_t<F> run = xyzz_t<F>::identity(), acc = xyzz_t<F>::identity();
-    // G1: the group law is inlined here (add_sel / dbl_sel: an out-of-line call moves 3 x 128 B through local memory per
+    // G1: the group law is inlined here (add_sel: an out-of-line call moves 3 x 128 B through local memory per
     // operation, which dominated this latency-bound chain); G2 keeps the calls to bound code size.
     for (uint32_t k = lo + seg_len; k-- > lo;) {
         xyzz_t<F> bk = ld16(bw + k);
         run = add_sel<F>(run, bk);
         acc = add_sel<F>(acc, run);
     }
-    if (lo) {   // + lo * run
-        xyzz_t<F> m = xyzz_t<F>::identity();
-        for (int bit = 31 - __clz(lo); bit >= 0; --bit) {
-            m = dbl_sel<F>(m);
-            if ((lo >> bit) & 1) m = add_sel<F>(m, run);
+    st16(pairs + 2 * (size_t)t, run);
+    st16(pairs + 2 * (size_t)t + 1, acc);
+}
+
+// Block (set w, term b, part h) of the segment pairs of a set (nseg a power of two, nbits = log2 nseg): term b < nbits sums
+// part h of the nseg / 2 values R_s whose index s has bit b set and doubles the sum b + log2 L times; term nbits sums part
+// h of the A_s.  parts[blockIdx.x]; the (nbits + 1) * split parts of a set add up to S_w (k_msm_window_sum).  Every block
+// is a plain sum, as deep as the window sum of the quad reduction plus at most log2 B doublings.
+template <class F, int THREADS>
+__global__ void __launch_bounds__(THREADS, 2) k_msm_window_bits(const xyzz_t<F>* pairs, uint32_t nseg, uint32_t log2L, uint32_t split,
+                                                             xyzz_t<F>* parts) {
+    __shared__ xyzz_t<F> sh[THREADS];
+    const uint32_t nbits = 31 - __clz(nseg), per_set = (nbits + 1) * split;
+    const uint32_t w = blockIdx.x / per_set, r = blockIdx.x % per_set, b = r / split, h = r % split;
+    const xyzz_t<F>* pw = pairs + 2 * (size_t)w * nseg;
+    xyzz_t<F> acc = xyzz_t<F>::identity();
+    if (b == nbits) {
+        const uint32_t cnt = nseg / split, lo = h * cnt;
+        for (uint32_t k = lo + threadIdx.x; k < lo + cnt; k += THREADS) acc = add_sel<F>(acc, ld16(pw + 2 * (size_t)k + 1));
+    } else {
+        const uint32_t cnt = nseg / 2 / split, lo = h * cnt, low = (1u << b) - 1;
+        for (uint32_t k = lo + threadIdx.x; k < lo + cnt; k += THREADS) {
+            const uint32_t s = ((k & ~low) << 1) | (1u << b) | (k & low);     // the k-th index with bit b set
+            acc = add_sel<F>(acc, ld16(pw + 2 * (size_t)s));
         }
-        acc = add_sel<F>(acc, m);
     }
-    st16(partials + t, acc);
+    sh[threadIdx.x] = acc;
+    __syncthreads();
+    for (int s = THREADS / 2; s > 0; s >>= 1) {
+        if ((int)threadIdx.x < s) {
+            xyzz_t<F> x = sh[threadIdx.x], y = sh[threadIdx.x + s];
+            sh[threadIdx.x] = add_sel<F>(x, y);
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x != 0) return;
+    xyzz_t<F> v = sh[0];
+    if (b < nbits)
+        for (uint32_t j = 0; j < b + log2L; ++j) v = dbl_sel<F>(v);
+    st16(parts + blockIdx.x, v);
 }
 
 // The same reduction with one QUAD per (window, segment): the (up to 4) independent field products of every level of a point
@@ -410,7 +446,7 @@ __global__ void __launch_bounds__(128) k_msm_reduce_segments_quad(const xyzz_t<F
     if ((threadIdx.x & 3) == 0) st16(partials + t, acc);
 }
 
-// one block per window: sum nseg partials
+// one block per window: sum nseg partials (the quad reduction's segment partials, or the parts of k_msm_window_bits)
 template <class F, int THREADS>
 __global__ void __launch_bounds__(THREADS) k_msm_window_sum(const xyzz_t<F>* partials, uint32_t nseg, xyzz_t<F>* wsum) {
     __shared__ xyzz_t<F> sh[THREADS];
@@ -539,7 +575,8 @@ struct MsmPlan {
     unsigned c, Wh, W, WB;              // window bits, windows per GLV half, digit windows, bucket sets
     uint32_t B, nb;                     // buckets per set, in all
     bool quad_reduce;                   // one quad per reduction segment (k_msm_reduce_segments_quad)
-    uint32_t seg_len, nseg, wsplit;     // buckets per reduction segment, segments per set, window-sum blocks per set
+    uint32_t seg_len, nseg, wsplit;     // buckets per reduction segment, segments per set, window-sum blocks per set (quad)
+    uint32_t nterms, bsplit;            // thread reduction: k_msm_window_bits terms (log2 nseg + 1) and blocks per term
     uint32_t rmw;                       // several parts: the bucket kernels add into the shared buckets
     size_t total_max;                   // sort entries of the largest part
     uint32_t task_len;
@@ -577,11 +614,19 @@ static int msm_plan(b200zk_ctx* ctx, const MsmPart* parts, unsigned nparts, unsi
     // QUAD per segment (k_msm_reduce_segments_quad) and, being pure latency chains, in 8-bucket segments whatever the caller's
     // `seg`: 16 + ~16 dependent point operations per segment instead of 64 + ~15 with the 32-bucket segments a 2^20 proof prefers.
     pl.quad_reduce = (uint64_t)pl.WB * (pl.B / pl.seg_len) <= 8192;
+    // B200ZK_MSM_SEG (read on every call) overrides the caller's segment-length hint
+    const char* env_seg = getenv("B200ZK_MSM_SEG");
+    if (env_seg && atoi(env_seg) > 0) seg = (unsigned)atoi(env_seg);
     if (pl.quad_reduce) pl.seg_len = pl.B < 8 ? pl.B : 8;
-    else if (seg && seg <= pl.B) pl.seg_len = seg;
+    else if (seg && seg <= pl.B) pl.seg_len = 1u << (31 - __builtin_clz(seg));      // a power of two, like B
     pl.nseg = pl.B / pl.seg_len;
-    // fold (one bucket set): the segment partials are summed by `wsplit` blocks whose results the Horner kernel adds up
-    pl.wsplit = pl.fold ? (pl.nseg >= 16 * 256 ? 16 : (pl.nseg >= 1024 ? 4 : 1)) : 1;
+    // quad reduction, fold (one bucket set): the segment partials are summed by `wsplit` blocks whose results the Horner
+    // kernel adds up
+    pl.wsplit = pl.fold && pl.quad_reduce ? (pl.nseg >= 16 * 256 ? 16 : (pl.nseg >= 1024 ? 4 : 1)) : 1;
+    // thread reduction: log2 nseg + 1 plain sums per set, each cut into parts of <= 2048 segments (one block each)
+    pl.nterms = 32 - __builtin_clz(pl.nseg);
+    pl.bsplit = 1;
+    while (pl.nseg / 2 / pl.bsplit > 2048) pl.bsplit *= 2;
 
     // window groups: consecutive bucket sets (whole windows, i.e. both GLV halves).  Measured on an earlier GPU:
     // at 2^20 the extra launches, the drain bubble at the end of every bucket kernel and the slowdown of the latency-bound
@@ -636,7 +681,7 @@ struct MsmWorkspace {
     };
     std::vector<Part> part;
     uint32_t* sums;
-    xyzz_t<F> *buckets, *partials, *wsum, *hstate;
+    xyzz_t<F> *buckets, *partials, *parts, *wsum, *hstate;
 };
 
 template <class F>
@@ -664,7 +709,8 @@ static int msm_workspace(b200zk_ctx* ctx, DevBuf& buf, const MsmPlan& pl, const 
         }
         carve(ws.sums, (size_t)pl.nb / SCAN_TILE + 2);
         carve(ws.buckets, pl.nb);
-        carve(ws.partials, (size_t)pl.WB * pl.nseg);
+        carve(ws.partials, (size_t)pl.WB * pl.nseg * (pl.quad_reduce ? 1 : 2));     // quad: one partial per segment, else a pair
+        carve(ws.parts, pl.quad_reduce ? 0 : (size_t)pl.WB * pl.nterms * pl.bsplit);
         carve(ws.wsum, (size_t)pl.WB * pl.wsplit);
         carve(ws.hstate, 2);
         return o;
@@ -812,18 +858,25 @@ static int msm_dev_impl(b200zk_ctx* ctx, Slot& sl, const MsmPart* parts, unsigne
             B2_TRY(launch(ctx, st, "msm_merge", k_msm_merge_small<F>, 4 * ctx->sm_count, 128, 0, w.multi + G.list_base, G.list_cap,
                           w.multi + 2 * g + 1, w.task_off + G.b0 + g, w.task_sums + G.task_base, 0u, ws.buckets + G.b0));
         }
-        xyzz_t<F>* group_partials = ws.partials + (size_t)G.set0 * pl.nseg;
-        if (pl.quad_reduce)                                        // latency-bound: fewer segments than the machine has warps
+        xyzz_t<F>* wsum = ws.wsum + (size_t)G.set0 * pl.wsplit;
+        constexpr int T = sizeof(F) > 32 ? 128 : 256;
+        if (pl.quad_reduce) {                                      // latency-bound: fewer segments than the machine has warps
+            xyzz_t<F>* group_partials = ws.partials + (size_t)G.set0 * pl.nseg;
             B2_TRY(launch(ctx, st, "msm_reduce", k_msm_reduce_segments_quad<F>, (G.nsets * pl.nseg * 4 + 127) / 128, 128, 0,
                           ws.buckets + G.b0, G.nsets, pl.B, pl.seg_len, group_partials));
-        else
+            // fold: the single bucket set's partials are summed by `wsplit` blocks, then added up by the Horner kernel with zero
+            // doublings per step
+            B2_TRY(launch(ctx, st, "msm_window_sum", k_msm_window_sum<F, T>, G.nsets * pl.wsplit, T, 0, group_partials,
+                          pl.nseg / pl.wsplit, wsum));
+        } else {
+            xyzz_t<F>* pairs = ws.partials + 2 * (size_t)G.set0 * pl.nseg;
+            xyzz_t<F>* parts = ws.parts + (size_t)G.set0 * pl.nterms * pl.bsplit;
             B2_TRY(launch(ctx, st, "msm_reduce", k_msm_reduce_segments<F>, (G.nsets * pl.nseg + 127) / 128, 128, 0, ws.buckets + G.b0,
-                          G.nsets, pl.B, pl.seg_len, group_partials));
-        // fold: the single bucket set's partials are summed by `wsplit` blocks, then added up by the Horner kernel with zero
-        // doublings per step
-        constexpr int T = sizeof(F) > 32 ? 128 : 256;
-        B2_TRY(launch(ctx, st, "msm_window_sum", k_msm_window_sum<F, T>, G.nsets * pl.wsplit, T, 0, group_partials, pl.nseg / pl.wsplit,
-                      ws.wsum + (size_t)G.set0 * pl.wsplit));
+                          G.nsets, pl.B, pl.seg_len, pairs));
+            B2_TRY(launch(ctx, st, "msm_window_sum", k_msm_window_bits<F, T>, G.nsets * pl.nterms * pl.bsplit, T, 0, pairs, pl.nseg,
+                          31u - __builtin_clz(pl.seg_len), pl.bsplit, parts));
+            B2_TRY(launch(ctx, st, "msm_window_sum", k_msm_window_sum<F, T>, G.nsets, T, 0, parts, pl.nterms * pl.bsplit, wsum));
+        }
         const uint32_t first = g == 0, last = g + 1 == ngroups;
         if (pl.fold)
             B2_TRY(launch(ctx, st, "msm_combine", k_msm_horner<F>, 1, 32, 0, ws.wsum, pl.wsplit, 0u, first, last, ws.hstate, out));
