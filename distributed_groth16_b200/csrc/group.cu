@@ -83,20 +83,42 @@ int gfrom(b200zk_group* g, int rank, int rc) {
     if (rc != B200ZK_OK && g) g->last_error = "device " + std::to_string(g->ctx[rank]->device) + ": " + g->ctx[rank]->last_error;
     return rc;
 }
-#define G_CUDA_OK(grp, expr)                                                                                  \
-    do {                                                                                                      \
-        cudaError_t _e = (expr);                                                                              \
-        if (_e != cudaSuccess) {                                                                              \
-            char _b[512];                                                                                     \
-            snprintf(_b, sizeof(_b), "CUDA error %s at %s:%d (%s)", cudaGetErrorString(_e), __FILE__, __LINE__, #expr); \
-            return gerr((grp), _e == cudaErrorMemoryAllocation ? B200ZK_ERR_OOM : B200ZK_ERR_CUDA, _b);         \
-        }                                                                                                     \
-    } while (0)
-#define G_TRY(grp, rank, expr)                     \
-    do {                                           \
-        int _rc = gfrom((grp), (rank), (expr));    \
-        if (_rc != B200ZK_OK) return _rc;          \
-    } while (0)
+
+// The prologue of every b200zk_group_* entry that works on the devices: a null group is refused, the caller's current device
+// is restored on return, and slot 0 of every device is held for the whole call, taken in rank order (the same order
+// everywhere: no deadlock).
+template <class Body>
+int with_group(b200zk_group* grp, Body&& body) {
+    DeviceGuard dev_guard;
+    if (!grp) return B200ZK_ERR_ARG;
+    std::vector<std::unique_lock<std::mutex>> locks;
+    for (int g = 0; g < grp->n; ++g) locks.emplace_back(grp->ctx[g]->slots[0].mu);
+    return body();
+}
+
+// body(ctx, slot 0) of rank g with its device current.  body's errors are context errors (the message in ctx->last_error)
+// and reach the group as "device N: <message>".
+template <class Body>
+int on_device(b200zk_group* grp, int g, Body&& body) {
+    b200zk_ctx* ctx = grp->ctx[g];
+    const cudaError_t e = cudaSetDevice(ctx->device);
+    if (e != cudaSuccess) {
+        char b[512];
+        snprintf(b, sizeof(b), "CUDA error %s at %s:%d (cudaSetDevice(ctx->device))", cudaGetErrorString(e), __FILE__, __LINE__);
+        return gerr(grp, e == cudaErrorMemoryAllocation ? B200ZK_ERR_OOM : B200ZK_ERR_CUDA, b);
+    }
+    return gfrom(grp, g, body(ctx, ctx->slots[0]));
+}
+
+// body(g, ctx, slot 0) on every rank in order, up to the first failure
+template <class Body>
+int each_device(b200zk_group* grp, Body&& body) {
+    for (int g = 0; g < grp->n; ++g) {
+        const int rc = on_device(grp, g, [&](b200zk_ctx* ctx, Slot& sl) { return body(g, ctx, sl); });
+        if (rc) return rc;
+    }
+    return B200ZK_OK;
+}
 
 // out[c][r] = in[r][c] for an R x C matrix of T (Fr: 32 B, G1 point: 64 B, G2 point: 128 B)
 template <class T>
@@ -125,29 +147,30 @@ void split_log(unsigned log_n, unsigned* log_rows, unsigned* log_cols) {
 
 // every device's stream waits until all devices have passed `ev[g]` (recorded on their streams just before)
 int cross_barrier(b200zk_group* grp, std::vector<cudaEvent_t>& ev) {
-    for (int g = 0; g < grp->n; ++g) {
-        G_CUDA_OK(grp, cudaSetDevice(grp->ctx[g]->device));
-        G_CUDA_OK(grp, cudaEventRecord(ev[g], grp->ctx[g]->slots[0].stream));
-    }
-    for (int g = 0; g < grp->n; ++g) {
-        G_CUDA_OK(grp, cudaSetDevice(grp->ctx[g]->device));
+    int rc = each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) -> int {
+        B2_CUDA_OK(ctx, cudaEventRecord(ev[g], sl.stream));
+        return B200ZK_OK;
+    });
+    if (rc) return rc;
+    return each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) -> int {
         for (int o = 0; o < grp->n; ++o)
-            if (o != g) G_CUDA_OK(grp, cudaStreamWaitEvent(grp->ctx[g]->slots[0].stream, ev[o], 0));
-    }
-    return B200ZK_OK;
+            if (o != g) B2_CUDA_OK(ctx, cudaStreamWaitEvent(sl.stream, ev[o], 0));
+        return B200ZK_OK;
+    });
 }
 
 int ensure_recv(b200zk_group* grp, size_t bytes) {
     if (bytes <= grp->recv_bytes) return B200ZK_OK;
-    for (int g = 0; g < grp->n; ++g) {
-        G_CUDA_OK(grp, cudaSetDevice(grp->ctx[g]->device));
-        G_CUDA_OK(grp, cudaDeviceSynchronize());
+    int rc = each_device(grp, [&](int g, b200zk_ctx* ctx, Slot&) -> int {
+        B2_CUDA_OK(ctx, cudaDeviceSynchronize());
         for (int b = 0; b < 2; ++b) {
             if (grp->recv[b][g]) cudaFree(grp->recv[b][g]);
             grp->recv[b][g] = nullptr;
-            G_CUDA_OK(grp, cudaMalloc(&grp->recv[b][g], bytes));
+            B2_CUDA_OK(ctx, cudaMalloc(&grp->recv[b][g], bytes));
         }
-    }
+        return B200ZK_OK;
+    });
+    if (rc) return rc;
     grp->recv_bytes = bytes;
     return B200ZK_OK;
 }
@@ -163,69 +186,59 @@ int sharded_ntt(b200zk_group* grp, Fr* const* in, Fr* const* out, unsigned log_r
     if (rc) return rc;
     const int b = grp->turn;
     grp->turn ^= 1;
-    for (int g = 0; g < P; ++g) {
-        b200zk_ctx* ctx = grp->ctx[g];
-        G_CUDA_OK(grp, cudaSetDevice(ctx->device));
-        G_TRY(grp, g, fourstep_cols_p2p_dev(ctx, ctx->slots[0], in[g], grp->recv[b], (unsigned)P, log_rows, ceil_log2(cg), log_rows + log_cols,
-                                            (uint64_t)g * cg, inverse));
-    }
+    rc = each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) {
+        return fourstep_cols_p2p_dev(ctx, sl, in[g], grp->recv[b], (unsigned)P, log_rows, ceil_log2(cg), log_rows + log_cols, (uint64_t)g * cg,
+                                     inverse);
+    });
+    if (rc) return rc;
     rc = cross_barrier(grp, grp->ev_col);          // all column kernels (= all peer stores) are complete
     if (rc) return rc;
-    for (int g = 0; g < P; ++g) {
-        b200zk_ctx* ctx = grp->ctx[g];
-        G_CUDA_OK(grp, cudaSetDevice(ctx->device));
+    return each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) {
         const Fr* rows_in = reinterpret_cast<const Fr*>(grp->recv[b][g]);
-        if (!shift_log_m) G_TRY(grp, g, ntt_dev(ctx, ctx->slots[0], rows_in, out[g], log_cols, inverse, false, (unsigned)rl));
-        else G_TRY(grp, g, ntt_batched_post_dev(ctx, ctx->slots[0], rows_in, out[g], log_cols, (unsigned)rl, inverse, shift_log_m + 1, true,
-                                                 (uint64_t)g * rl, 0, 1, rows));
-    }
-    return B200ZK_OK;
+        if (!shift_log_m) return ntt_dev(ctx, sl, rows_in, out[g], log_cols, inverse, false, (unsigned)rl);
+        return ntt_batched_post_dev(ctx, sl, rows_in, out[g], log_cols, (unsigned)rl, inverse, shift_log_m + 1, true, (uint64_t)g * rl, 0, 1, rows);
+    });
 }
 
 // host vector (natural order, N = rows x cols row-major) -> column layout on the devices: a strided H2D copy of the
 // device's column slab (rows x cg) followed by an on-device transpose to cg x rows
-template <class T>
-int scatter_columns(b200zk_group* grp, const void* host, size_t rows, size_t cols, void* const* d_tmp, void* const* d_out) {
-    const int P = grp->n;
-    const size_t cg = cols / P;
-    for (int g = 0; g < P; ++g) {
-        b200zk_ctx* ctx = grp->ctx[g];
-        G_CUDA_OK(grp, cudaSetDevice(ctx->device));
-        cudaStream_t st = ctx->slots[0].stream;
-        G_CUDA_OK(grp, cudaMemcpy2DAsync(d_tmp[g], cg * sizeof(T), reinterpret_cast<const char*>(host) + g * cg * sizeof(T), cols * sizeof(T),
-                                         cg * sizeof(T), rows, cudaMemcpyHostToDevice, st));
-        G_TRY(grp, g, transpose_dev<T>(ctx, st, d_tmp[g], d_out[g], rows, cg));
-    }
-    return B200ZK_OK;
+int scatter_columns(b200zk_group* grp, const void* host, size_t rows, size_t cols, Fr* const* d_tmp, Fr* const* d_out) {
+    const size_t cg = cols / grp->n;
+    return each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) -> int {
+        B2_CUDA_OK(ctx, cudaMemcpy2DAsync(d_tmp[g], cg * sizeof(Fr), reinterpret_cast<const char*>(host) + g * cg * sizeof(Fr), cols * sizeof(Fr),
+                                          cg * sizeof(Fr), rows, cudaMemcpyHostToDevice, sl.stream));
+        return transpose_dev<Blob32>(ctx, sl.stream, d_tmp[g], d_out[g], rows, cg);
+    });
 }
 // column layout (cg x rows per device) -> host natural order
-template <class T>
-int gather_columns(b200zk_group* grp, void* host, size_t rows, size_t cols, void* const* d_in, void* const* d_tmp) {
-    const int P = grp->n;
-    const size_t cg = cols / P;
-    for (int g = 0; g < P; ++g) {
-        b200zk_ctx* ctx = grp->ctx[g];
-        G_CUDA_OK(grp, cudaSetDevice(ctx->device));
-        cudaStream_t st = ctx->slots[0].stream;
-        G_TRY(grp, g, transpose_dev<T>(ctx, st, d_in[g], d_tmp[g], cg, rows));
-        G_CUDA_OK(grp, cudaMemcpy2DAsync(reinterpret_cast<char*>(host) + g * cg * sizeof(T), cols * sizeof(T), d_tmp[g], cg * sizeof(T),
-                                         cg * sizeof(T), rows, cudaMemcpyDeviceToHost, st));
-    }
-    return B200ZK_OK;
+int gather_columns(b200zk_group* grp, void* host, size_t rows, size_t cols, Fr* const* d_in, Fr* const* d_tmp) {
+    const size_t cg = cols / grp->n;
+    return each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) -> int {
+        B2_TRY(transpose_dev<Blob32>(ctx, sl.stream, d_in[g], d_tmp[g], cg, rows));
+        B2_CUDA_OK(ctx, cudaMemcpy2DAsync(reinterpret_cast<char*>(host) + g * cg * sizeof(Fr), cols * sizeof(Fr), d_tmp[g], cg * sizeof(Fr),
+                                          cg * sizeof(Fr), rows, cudaMemcpyDeviceToHost, sl.stream));
+        return B200ZK_OK;
+    });
 }
 
 int sync_all(b200zk_group* grp) {
+    return each_device(grp, [&](int, b200zk_ctx* ctx, Slot& sl) -> int {
+        B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.stream));
+        return B200ZK_OK;
+    });
+}
+
+// Device 0's slot-0 stream copies the first `bytes` of every rank g's slot-0 result buffer (`small`) to dst + g * bytes,
+// behind ev_done[g], which rank g recorded once it wrote them.  Device 0 is current.
+int gather_on_device0(b200zk_group* grp, size_t bytes, char* dst) {
+    b200zk_ctx* c0 = grp->ctx[0];
+    cudaStream_t st = c0->slots[0].stream;
     for (int g = 0; g < grp->n; ++g) {
-        G_CUDA_OK(grp, cudaSetDevice(grp->ctx[g]->device));
-        G_CUDA_OK(grp, cudaStreamSynchronize(grp->ctx[g]->slots[0].stream));
+        if (g) B2_CUDA_OK(c0, cudaStreamWaitEvent(st, grp->ev_done[g], 0));
+        B2_CUDA_OK(c0, cudaMemcpyPeerAsync(dst + g * bytes, c0->device, grp->ctx[g]->slots[0].small.p, grp->ctx[g]->device, bytes, st));
     }
     return B200ZK_OK;
 }
-
-struct SlotLocks {           // slot 0 of every device, in rank order (same order everywhere: no deadlock)
-    std::vector<std::unique_lock<std::mutex>> l;
-    explicit SlotLocks(b200zk_group* grp) { for (int g = 0; g < grp->n; ++g) l.emplace_back(grp->ctx[g]->slots[0].mu); }
-};
 
 // balanced index-range split
 size_t cut(size_t n, int g, int P) { return (size_t)(((unsigned __int128)n * (unsigned)g) / (unsigned)P); }
@@ -233,71 +246,79 @@ size_t cut(size_t n, int g, int P) { return (size_t)(((unsigned __int128)n * (un
 template <int G2>
 int group_msm(b200zk_group* grp, const uint64_t* bases, size_t n_bases, const uint64_t* scalars, size_t n_scalars, uint64_t* out_affine,
               int* out_is_inf) {
-    DeviceGuard dev_guard;
-    if (!grp || !out_affine || !out_is_inf) return B200ZK_ERR_ARG;
-    if (n_bases != n_scalars) return gerr(grp, B200ZK_ERR_LENGTH, std::to_string(n_bases < n_scalars ? n_bases : n_scalars));
-    const size_t n = n_bases;
-    if (n && (!bases || !scalars)) return gerr(grp, B200ZK_ERR_ARG, "null input");
-    const size_t PB = G2 ? 128 : 64, XB = G2 ? 256 : 128;
-    const int P = grp->n;
-    SlotLocks locks(grp);
-    // every device: stage its slice (scalars on the compute stream, bases on the copy stream behind the sort phases), MSM
-    for (int g = 0; g < P; ++g) {
-        b200zk_ctx* ctx = grp->ctx[g];
-        Slot& sl = ctx->slots[0];
-        G_CUDA_OK(grp, cudaSetDevice(ctx->device));
-        const size_t lo = cut(n, g, P), cnt = cut(n, g + 1, P) - lo;
-        G_CUDA_OK(grp, sl.small.reserve(4096));
-        // this device's index range, staged in parts behind its own bucket kernels (api.cu, msm_staged_dev)
-        G_TRY(grp, g, msm_staged_dev(ctx, sl, G2, reinterpret_cast<const char*>(bases) + lo * PB, reinterpret_cast<const char*>(scalars) + lo * 32,
-                                     cnt, sl.small.p, false));
-        G_CUDA_OK(grp, cudaEventRecord(grp->ev_done[g], sl.stream));
-    }
-    // partials -> device 0 (peer copies), sum, normalise
-    b200zk_ctx* c0 = grp->ctx[0];
-    Slot& s0 = c0->slots[0];
-    G_CUDA_OK(grp, cudaSetDevice(c0->device));
-    char* sm = reinterpret_cast<char*>(s0.small.p);
-    char* gathered = sm + 1024;                               // P x XB <= 2 KB
-    for (int g = 0; g < P; ++g) {
-        if (g) G_CUDA_OK(grp, cudaStreamWaitEvent(s0.stream, grp->ev_done[g], 0));
-        G_CUDA_OK(grp, cudaMemcpyPeerAsync(gathered + g * XB, c0->device, grp->ctx[g]->slots[0].small.p, grp->ctx[g]->device, XB, s0.stream));
-    }
-    G_TRY(grp, 0, G2 ? g2_sum_dev(c0, s0, gathered, P, sm + 3584) : g1_sum_dev(c0, s0, gathered, P, sm + 3584));
-    uint64_t host[17];
-    G_CUDA_OK(grp, cudaMemcpyAsync(host, sm + 3584, PB + 8, cudaMemcpyDeviceToHost, s0.stream));
-    G_CUDA_OK(grp, cudaStreamSynchronize(s0.stream));
-    int rc = sync_all(grp);
-    for (int g = 0; g < P && !rc; ++g) {                      // the host buffers are free again once every copy stream drained
-        cudaSetDevice(grp->ctx[g]->device);
-        if (cudaStreamSynchronize(grp->ctx[g]->slots[0].copy_stream) != cudaSuccess) rc = gerr(grp, B200ZK_ERR_CUDA, "copy stream failed");
-    }
-    if (rc) return rc;
-    memcpy(out_affine, host, PB);
-    *out_is_inf = (int)host[PB / 8];
-    return B200ZK_OK;
+    return with_group(grp, [&]() -> int {
+        if (!out_affine || !out_is_inf) return B200ZK_ERR_ARG;
+        if (n_bases != n_scalars) return gerr(grp, B200ZK_ERR_LENGTH, std::to_string(n_bases < n_scalars ? n_bases : n_scalars));
+        const size_t n = n_bases;
+        if (n && (!bases || !scalars)) return gerr(grp, B200ZK_ERR_ARG, "null input");
+        const size_t PB = G2 ? 128 : 64, XB = G2 ? 256 : 128;
+        const int P = grp->n;
+        // every device: stage its slice (scalars on the compute stream, bases on the copy stream behind the sort phases), MSM
+        int rc = each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) -> int {
+            const size_t lo = cut(n, g, P), cnt = cut(n, g + 1, P) - lo;
+            B2_CUDA_OK(ctx, sl.small.reserve(4096));
+            // this device's index range, staged in parts behind its own bucket kernels (api.cu, msm_staged_dev)
+            B2_TRY(msm_staged_dev(ctx, sl, G2, reinterpret_cast<const char*>(bases) + lo * PB, reinterpret_cast<const char*>(scalars) + lo * 32,
+                                  cnt, sl.small.p, false));
+            B2_CUDA_OK(ctx, cudaEventRecord(grp->ev_done[g], sl.stream));
+            return B200ZK_OK;
+        });
+        if (rc) return rc;
+        // partials -> device 0 (peer copies), sum, normalise
+        uint64_t host[17];
+        rc = on_device(grp, 0, [&](b200zk_ctx* c0, Slot& s0) -> int {
+            char* sm = reinterpret_cast<char*>(s0.small.p);
+            char* gathered = sm + 1024;                               // P x XB <= 2 KB
+            B2_TRY(gather_on_device0(grp, XB, gathered));
+            B2_TRY(G2 ? g2_sum_dev(c0, s0, gathered, P, sm + 3584) : g1_sum_dev(c0, s0, gathered, P, sm + 3584));
+            B2_CUDA_OK(c0, cudaMemcpyAsync(host, sm + 3584, PB + 8, cudaMemcpyDeviceToHost, s0.stream));
+            B2_CUDA_OK(c0, cudaStreamSynchronize(s0.stream));
+            return B200ZK_OK;
+        });
+        if (!rc) rc = sync_all(grp);
+        // the host buffers are free again once every copy stream drained
+        if (!rc) rc = each_device(grp, [&](int, b200zk_ctx* ctx, Slot& sl) -> int {
+            B2_CUDA_OK(ctx, cudaStreamSynchronize(sl.copy_stream));
+            return B200ZK_OK;
+        });
+        if (rc) return rc;
+        memcpy(out_affine, host, PB);
+        *out_is_inf = (int)host[PB / 8];
+        return B200ZK_OK;
+    });
 }
 
-// the h pipeline on vectors already in the column layout: a, b, c, h: (cols / P) x rows per device
-int sharded_h(b200zk_group* grp, Fr* const* a, Fr* const* b, Fr* const* c, Fr* const* tmp1, Fr* const* tmp2, unsigned log_m, Fr* const* h) {
+// The column-layout workspace of an h or proof computation, carved from slot 0's io_a on every device g: a, b, c and the
+// temporaries t1, t2 (t2 ends up holding h), loc Fr each, then the caller's tail of z at z[g].
+struct Columns {
+    std::vector<Fr*> a, b, c, t1, t2, z;
+    explicit Columns(int P) : a(P), b(P), c(P), t1(P), t2(P), z(P) {}
+};
+
+// tail(g): the Fr that follow the five vectors on device g
+template <class Tail>
+int carve_columns(b200zk_group* grp, size_t loc, Tail&& tail, Columns& w) {
+    return each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) -> int {
+        B2_CUDA_OK(ctx, sl.io_a.reserve((5 * loc + tail(g)) * sizeof(Fr)));
+        Fr* p = reinterpret_cast<Fr*>(sl.io_a.p);
+        w.a[g] = p; w.b[g] = p + loc; w.c[g] = p + 2 * loc; w.t1[g] = p + 3 * loc; w.t2[g] = p + 4 * loc; w.z[g] = p + 5 * loc;
+        return B200ZK_OK;
+    });
+}
+
+// the h pipeline on w.a, w.b, w.c, already in the column layout ((cols / P) x rows per device); h lands in w.t2
+int sharded_h(b200zk_group* grp, const Columns& w, unsigned log_m) {
     unsigned log_rows, log_cols;
     split_log(log_m, &log_rows, &log_cols);
-    // a, b, c are transformed in place (through tmp1): coef = iNTT + shift, ev = NTT
-    Fr* const* vecs[3] = {a, b, c};
-    for (int k = 0; k < 3; ++k) {
-        int rc = sharded_ntt(grp, vecs[k], tmp1, log_rows, log_cols, true, log_m);
+    // a, b, c are transformed in place (through t1): coef = iNTT + shift, ev = NTT
+    for (const std::vector<Fr*>* v : {&w.a, &w.b, &w.c}) {
+        int rc = sharded_ntt(grp, v->data(), w.t1.data(), log_rows, log_cols, true, log_m);
         if (rc) return rc;
-        rc = sharded_ntt(grp, tmp1, vecs[k], log_cols, log_rows, false, 0);
+        rc = sharded_ntt(grp, w.t1.data(), v->data(), log_cols, log_rows, false, 0);
         if (rc) return rc;
     }
     const size_t local = ((size_t)1 << log_m) / grp->n;
-    for (int g = 0; g < grp->n; ++g) {
-        b200zk_ctx* ctx = grp->ctx[g];
-        G_CUDA_OK(grp, cudaSetDevice(ctx->device));
-        G_TRY(grp, g, mul_sub_dev(ctx, ctx->slots[0], a[g], b[g], c[g], h[g], local));
-    }
-    (void)tmp2;
-    return B200ZK_OK;
+    return each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) { return mul_sub_dev(ctx, sl, w.a[g], w.b[g], w.c[g], w.t2[g], local); });
 }
 
 // Slot j of GPU g's column-layout slice holds global row (j mod rows) cols + g cols / P + j div rows (local[c rows + r] =
@@ -335,49 +356,43 @@ int check_csr(b200zk_group* grp, const char* name, const uint32_t* row_ptr, cons
     return B200ZK_OK;
 }
 
-// The prover from a, b, c already in the column layout on the devices (a, b, c, t1, t2: loc Fr each per device; t2 ends up
-// holding h): sharded h, five partial MSMs per device, peer copies of the partials to device 0, sums and assembly there.
-// zq[g] = z[v0, v1) and zl[g] = z[n_inputs + l0, n_inputs + l1) of device g's key shard.  The caller holds the slot locks and
-// has reserved every device's small buffer (4 KB).
-int prove_columns(b200zk_group* grp, const b200zk_group_pk* pk, Fr* const* va, Fr* const* vb, Fr* const* vc, Fr* const* t1, Fr* const* t2,
-                  const Fr* const* zq, const Fr* const* zl, const uint64_t r[4], const uint64_t s[4], uint8_t proof_out[128]) {
+// The prover from a, b, c already in w's column layout on the devices: sharded h, five partial MSMs per device, peer copies
+// of the partials to device 0, sums and assembly there.  zq[g] = z[v0, v1) and zl[g] = z[n_inputs + l0, n_inputs + l1) of
+// device g's key shard.  The caller holds the slot locks and has reserved every device's small buffer (4 KB).
+int prove_columns(b200zk_group* grp, const b200zk_group_pk* pk, const Columns& w, const Fr* const* zq, const Fr* const* zl, const uint64_t r[4],
+                  const uint64_t s[4], uint8_t proof_out[128]) {
     const int P = grp->n;
     const bool need_b1 = (r[0] | r[1] | r[2] | r[3]) != 0;
-    int rc = sharded_h(grp, va, vb, vc, t1, t2, pk->log_m, t2);
+    int rc = sharded_h(grp, w, pk->log_m);
     if (rc) return rc;
     // partial MSMs: small[0..16) A, [16..32) L, [32..48) H, [48..64) B1 (u64 words), [64..96) B2
-    for (int g = 0; g < P; ++g) {
-        b200zk_ctx* ctx = grp->ctx[g];
-        Slot& sl = ctx->slots[0];
+    rc = each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) -> int {
         const b200zk_group_pk::Shard& S = pk->shard[g];
-        G_CUDA_OK(grp, cudaSetDevice(ctx->device));
         char* sm = reinterpret_cast<char*>(sl.small.p);
         auto msm = [&](int k, const Fr* scalars, size_t n, void* out) {
             return query_msm(ctx, sl, k, S.q[k], S.tab, S.tab_c, scalars, n, out, 0);
         };
-        G_TRY(grp, g, msm(2, zq[g], S.v1 - S.v0, sm + 512));                    // the G2 MSM first: the longest
-        G_TRY(grp, g, msm(0, zq[g], S.v1 - S.v0, sm + 0));
-        G_TRY(grp, g, msm(3, zl[g], S.l1 - S.l0, sm + 128));
-        G_TRY(grp, g, msm(4, t2[g], S.hn, sm + 256));
-        if (need_b1) G_TRY(grp, g, msm(1, zq[g], S.v1 - S.v0, sm + 384));
-        else G_CUDA_OK(grp, cudaMemsetAsync(sm + 384, 0, 128, sl.stream));
-        G_CUDA_OK(grp, cudaEventRecord(grp->ev_done[g], sl.stream));
-    }
+        B2_TRY(msm(2, zq[g], S.v1 - S.v0, sm + 512));                    // the G2 MSM first: the longest
+        B2_TRY(msm(0, zq[g], S.v1 - S.v0, sm + 0));
+        B2_TRY(msm(3, zl[g], S.l1 - S.l0, sm + 128));
+        B2_TRY(msm(4, w.t2[g], S.hn, sm + 256));
+        if (need_b1) B2_TRY(msm(1, zq[g], S.v1 - S.v0, sm + 384));
+        else B2_CUDA_OK(ctx, cudaMemsetAsync(sm + 384, 0, 128, sl.stream));
+        B2_CUDA_OK(ctx, cudaEventRecord(grp->ev_done[g], sl.stream));
+        return B200ZK_OK;
+    });
+    if (rc) return rc;
     // gather on device 0, add up, assemble (the sharded MSMs ran over index 0 too: z[0] = 1 makes a_query[0] z[0] the term the
     // reference's driver adds, sha256.rs:208-212 -> include_zero_terms = 0)
-    b200zk_ctx* c0 = grp->ctx[0];
-    Slot& s0 = c0->slots[0];
-    G_CUDA_OK(grp, cudaSetDevice(c0->device));
-    G_CUDA_OK(grp, s0.io_b.reserve((size_t)(P + 1) * 768));
-    char* gathered = reinterpret_cast<char*>(s0.io_b.p);
-    char* tot = gathered + (size_t)P * 768;
-    for (int g = 0; g < P; ++g) {
-        if (g) G_CUDA_OK(grp, cudaStreamWaitEvent(s0.stream, grp->ev_done[g], 0));
-        G_CUDA_OK(grp, cudaMemcpyPeerAsync(gathered + (size_t)g * 768, c0->device, grp->ctx[g]->slots[0].small.p, grp->ctx[g]->device, 768, s0.stream));
-    }
-    for (int k = 0; k < 4; ++k) G_TRY(grp, 0, xyzz_sum_dev(c0, s0, 0, gathered + k * 128, P, 6, tot + k * 128));      // stride: 768 B = 6 G1 XYZZ
-    G_TRY(grp, 0, xyzz_sum_dev(c0, s0, 1, gathered + 512, P, 3, tot + 512));                                          // 3 G2 XYZZ
-    rc = gfrom(grp, 0, assemble_dev(c0, s0, pk->pk0, tot, tot + 512, tot + 128, tot + 256, need_b1 ? tot + 384 : nullptr, r, s, 0, proof_out));
+    rc = on_device(grp, 0, [&](b200zk_ctx* c0, Slot& s0) -> int {
+        B2_CUDA_OK(c0, s0.io_b.reserve((size_t)(P + 1) * 768));
+        char* gathered = reinterpret_cast<char*>(s0.io_b.p);
+        char* tot = gathered + (size_t)P * 768;
+        B2_TRY(gather_on_device0(grp, 768, gathered));
+        for (int k = 0; k < 4; ++k) B2_TRY(xyzz_sum_dev(c0, s0, 0, gathered + k * 128, P, 6, tot + k * 128));      // stride: 768 B = 6 G1 XYZZ
+        B2_TRY(xyzz_sum_dev(c0, s0, 1, gathered + 512, P, 3, tot + 512));                                          // 3 G2 XYZZ
+        return assemble_dev(c0, s0, pk->pk0, tot, tot + 512, tot + 128, tot + 256, need_b1 ? tot + 384 : nullptr, r, s, 0, proof_out);
+    });
     if (rc) return rc;
     return sync_all(grp);
 }
@@ -448,63 +463,49 @@ int b200zk_group_msm_g2(b200zk_group* grp, const uint64_t* bases, size_t n_bases
 }
 
 int b200zk_group_ntt_fr(b200zk_group* grp, uint64_t* data, unsigned log_n, int inverse) {
-    DeviceGuard dev_guard;
-    if (!grp || !data) return B200ZK_ERR_ARG;
-    if (log_n > 28) return gerr(grp, B200ZK_ERR_DOMAIN, "log n > 28");
-    const int P = grp->n;
-    unsigned log_rows, log_cols;
-    split_log(log_n, &log_rows, &log_cols);
-    const size_t rows = (size_t)1 << log_rows, cols = (size_t)1 << log_cols, N = (size_t)1 << log_n;
-    if (cols < (size_t)P) return gerr(grp, B200ZK_ERR_ARG, "transform too small for this many GPUs");
-    SlotLocks locks(grp);
-    std::vector<void*> bufA(P), bufB(P);
-    for (int g = 0; g < P; ++g) {
-        b200zk_ctx* ctx = grp->ctx[g];
-        G_CUDA_OK(grp, cudaSetDevice(ctx->device));
-        G_CUDA_OK(grp, ctx->slots[0].io_a.reserve(2 * (N / P) * sizeof(Fr)));
-        bufA[g] = ctx->slots[0].io_a.p;
-        bufB[g] = reinterpret_cast<Fr*>(bufA[g]) + N / P;
-    }
-    int rc = scatter_columns<Blob32>(grp, data, rows, cols, bufB.data(), bufA.data());         // layout(cols) in A
-    if (rc) return rc;
-    std::vector<Fr*> in(P), out(P);
-    for (int g = 0; g < P; ++g) { in[g] = reinterpret_cast<Fr*>(bufA[g]); out[g] = reinterpret_cast<Fr*>(bufB[g]); }
-    rc = sharded_ntt(grp, in.data(), out.data(), log_rows, log_cols, inverse != 0, 0);          // layout(rows) in B: (rows / P) x cols
-    if (rc) return rc;
-    // X[k1 + rows k2] sits at out[g][k1 local][k2]: as a cols x rows row-major matrix X[k2][k1] the device owns columns k1
-    rc = gather_columns<Blob32>(grp, data, cols, rows, bufB.data(), bufA.data());
-    if (rc) return rc;
-    return sync_all(grp);
+    return with_group(grp, [&]() -> int {
+        if (!data) return B200ZK_ERR_ARG;
+        if (log_n > 28) return gerr(grp, B200ZK_ERR_DOMAIN, "log n > 28");
+        const int P = grp->n;
+        unsigned log_rows, log_cols;
+        split_log(log_n, &log_rows, &log_cols);
+        const size_t rows = (size_t)1 << log_rows, cols = (size_t)1 << log_cols, N = (size_t)1 << log_n;
+        if (cols < (size_t)P) return gerr(grp, B200ZK_ERR_ARG, "transform too small for this many GPUs");
+        std::vector<Fr*> bufA(P), bufB(P);
+        int rc = each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) -> int {
+            B2_CUDA_OK(ctx, sl.io_a.reserve(2 * (N / P) * sizeof(Fr)));
+            bufA[g] = reinterpret_cast<Fr*>(sl.io_a.p);
+            bufB[g] = bufA[g] + N / P;
+            return B200ZK_OK;
+        });
+        if (!rc) rc = scatter_columns(grp, data, rows, cols, bufB.data(), bufA.data());                    // layout(cols) in A
+        if (!rc) rc = sharded_ntt(grp, bufA.data(), bufB.data(), log_rows, log_cols, inverse != 0, 0);     // layout(rows) in B: (rows / P) x cols
+        // X[k1 + rows k2] sits at bufB[g][k1 local][k2]: as a cols x rows row-major matrix X[k2][k1] the device owns columns k1
+        if (!rc) rc = gather_columns(grp, data, cols, rows, bufB.data(), bufA.data());
+        if (rc) return rc;
+        return sync_all(grp);
+    });
 }
 
 int b200zk_group_h_circom(b200zk_group* grp, const uint64_t* a, const uint64_t* b, const uint64_t* c, unsigned log_m, uint64_t* h_out) {
-    DeviceGuard dev_guard;
-    if (!grp || !a || !b || !c || !h_out) return B200ZK_ERR_ARG;
-    if (log_m + 1 > 28) return gerr(grp, B200ZK_ERR_DOMAIN, "2m exceeds the 2^28 subgroup (PolynomialDegreeTooLarge)");
-    const int P = grp->n;
-    unsigned log_rows, log_cols;
-    split_log(log_m, &log_rows, &log_cols);
-    const size_t rows = (size_t)1 << log_rows, cols = (size_t)1 << log_cols, m = (size_t)1 << log_m, loc = m / P;
-    if (cols < (size_t)P) return gerr(grp, B200ZK_ERR_ARG, "domain too small for this many GPUs");
-    SlotLocks locks(grp);
-    std::vector<void*> va(P), vb(P), vc(P), t1(P), t2(P);
-    for (int g = 0; g < P; ++g) {
-        b200zk_ctx* ctx = grp->ctx[g];
-        G_CUDA_OK(grp, cudaSetDevice(ctx->device));
-        G_CUDA_OK(grp, ctx->slots[0].io_a.reserve(5 * loc * sizeof(Fr)));
-        Fr* p = reinterpret_cast<Fr*>(ctx->slots[0].io_a.p);
-        va[g] = p; vb[g] = p + loc; vc[g] = p + 2 * loc; t1[g] = p + 3 * loc; t2[g] = p + 4 * loc;
-    }
-    int rc = scatter_columns<Blob32>(grp, a, rows, cols, t1.data(), va.data());
-    if (!rc) rc = scatter_columns<Blob32>(grp, b, rows, cols, t1.data(), vb.data());
-    if (!rc) rc = scatter_columns<Blob32>(grp, c, rows, cols, t1.data(), vc.data());
-    if (rc) return rc;
-    rc = sharded_h(grp, reinterpret_cast<Fr* const*>(va.data()), reinterpret_cast<Fr* const*>(vb.data()), reinterpret_cast<Fr* const*>(vc.data()),
-                   reinterpret_cast<Fr* const*>(t1.data()), reinterpret_cast<Fr* const*>(t2.data()), log_m, reinterpret_cast<Fr* const*>(t2.data()));
-    if (rc) return rc;
-    rc = gather_columns<Blob32>(grp, h_out, rows, cols, t2.data(), t1.data());
-    if (rc) return rc;
-    return sync_all(grp);
+    return with_group(grp, [&]() -> int {
+        if (!a || !b || !c || !h_out) return B200ZK_ERR_ARG;
+        if (log_m + 1 > 28) return gerr(grp, B200ZK_ERR_DOMAIN, "2m exceeds the 2^28 subgroup (PolynomialDegreeTooLarge)");
+        const int P = grp->n;
+        unsigned log_rows, log_cols;
+        split_log(log_m, &log_rows, &log_cols);
+        const size_t rows = (size_t)1 << log_rows, cols = (size_t)1 << log_cols, m = (size_t)1 << log_m, loc = m / P;
+        if (cols < (size_t)P) return gerr(grp, B200ZK_ERR_ARG, "domain too small for this many GPUs");
+        Columns w(P);
+        int rc = carve_columns(grp, loc, [](int) { return (size_t)0; }, w);
+        if (!rc) rc = scatter_columns(grp, a, rows, cols, w.t1.data(), w.a.data());
+        if (!rc) rc = scatter_columns(grp, b, rows, cols, w.t1.data(), w.b.data());
+        if (!rc) rc = scatter_columns(grp, c, rows, cols, w.t1.data(), w.c.data());
+        if (!rc) rc = sharded_h(grp, w, log_m);
+        if (!rc) rc = gather_columns(grp, h_out, rows, cols, w.t2.data(), w.t1.data());
+        if (rc) return rc;
+        return sync_all(grp);
+    });
 }
 
 // ---- sharded proving key + prove (BASELINE config 5) ------------------------------------------------------------------------
@@ -525,111 +526,103 @@ void b200zk_group_pk_free(b200zk_group* grp, b200zk_group_pk* pk) {
 int b200zk_group_pk_upload(b200zk_group* grp, const uint64_t* a_query, const uint64_t* b_g1_query, const uint64_t* b_g2_query,
                            const uint64_t* l_query, const uint64_t* h_query, size_t n_vars, size_t n_inputs, size_t m,
                            const uint64_t* vk_points, b200zk_group_pk** out) {
-    DeviceGuard dev_guard;
-    if (!grp || !out || !a_query || !b_g1_query || !b_g2_query || !h_query || !vk_points) return B200ZK_ERR_ARG;
-    if (n_vars == 0 || n_inputs == 0 || n_inputs > n_vars) return gerr(grp, B200ZK_ERR_ARG, "need 1 <= n_inputs <= n_vars");
-    if (m == 0 || (m & (m - 1))) return gerr(grp, B200ZK_ERR_DOMAIN, "h_query length must be a power of two");
-    const int P = grp->n;
-    const unsigned log_m = ceil_log2(m);
-    unsigned log_rows, log_cols;
-    split_log(log_m, &log_rows, &log_cols);
-    const size_t rows = (size_t)1 << log_rows, cols = (size_t)1 << log_cols;
-    if (cols < (size_t)P) return gerr(grp, B200ZK_ERR_ARG, "domain too small for this many GPUs");
-    SlotLocks locks(grp);
-    b200zk_group_pk* pk = new b200zk_group_pk();
-    pk->n = P; pk->n_vars = n_vars; pk->n_inputs = n_inputs; pk->m = m; pk->log_m = log_m; pk->owner = grp;
-    pk->shard.resize(P);
-    const size_t n_aux = n_vars - n_inputs;
-    const bool want_tables = pk_tables_enabled();
-    auto fail = [&](int rc) { b200zk_group_pk_free(grp, pk); return rc; };
-    for (int g = 0; g < P; ++g) {
-        b200zk_ctx* ctx = grp->ctx[g];
-        Slot& sl = ctx->slots[0];
-        if (cudaSetDevice(ctx->device) != cudaSuccess) return fail(gerr(grp, B200ZK_ERR_CUDA, "cudaSetDevice failed"));
-        b200zk_group_pk::Shard& S = pk->shard[g];
-        S.v0 = cut(n_vars, g, P); S.v1 = cut(n_vars, g + 1, P);
-        S.l0 = cut(n_aux, g, P); S.l1 = cut(n_aux, g + 1, P);
-        S.hn = m / P;
-        const size_t cnt[5] = {S.v1 - S.v0, S.v1 - S.v0, S.v1 - S.v0, S.l1 - S.l0, S.hn};
-        const size_t psz[5] = {64, 64, 128, 64, 64};
-        const void* src[4] = {reinterpret_cast<const char*>(a_query) + S.v0 * 64, reinterpret_cast<const char*>(b_g1_query) + S.v0 * 64,
-                              reinterpret_cast<const char*>(b_g2_query) + S.v0 * 128,
-                              l_query ? reinterpret_cast<const char*>(l_query) + S.l0 * 64 : nullptr};
-        for (int k = 0; k < 5; ++k) {
-            if (cudaMalloc(&S.q[k], cnt[k] * psz[k] + 16) != cudaSuccess) return fail(gerr(grp, B200ZK_ERR_OOM, "proving-key shard allocation failed"));
-            if (k < 4 && cnt[k] && cudaMemcpyAsync(S.q[k], src[k], cnt[k] * psz[k], cudaMemcpyHostToDevice, sl.stream) != cudaSuccess)
-                return fail(gerr(grp, B200ZK_ERR_CUDA, "proving-key upload failed"));
+    return with_group(grp, [&]() -> int {
+        if (!out || !a_query || !b_g1_query || !b_g2_query || !h_query || !vk_points) return B200ZK_ERR_ARG;
+        if (n_vars == 0 || n_inputs == 0 || n_inputs > n_vars) return gerr(grp, B200ZK_ERR_ARG, "need 1 <= n_inputs <= n_vars");
+        if (m == 0 || (m & (m - 1))) return gerr(grp, B200ZK_ERR_DOMAIN, "h_query length must be a power of two");
+        const int P = grp->n;
+        const unsigned log_m = ceil_log2(m);
+        unsigned log_rows, log_cols;
+        split_log(log_m, &log_rows, &log_cols);
+        const size_t rows = (size_t)1 << log_rows, cols = (size_t)1 << log_cols;
+        if (cols < (size_t)P) return gerr(grp, B200ZK_ERR_ARG, "domain too small for this many GPUs");
+        b200zk_group_pk* pk = new b200zk_group_pk();
+        pk->n = P; pk->n_vars = n_vars; pk->n_inputs = n_inputs; pk->m = m; pk->log_m = log_m; pk->owner = grp;
+        pk->shard.resize(P);
+        const size_t n_aux = n_vars - n_inputs;
+        const bool want_tables = pk_tables_enabled();
+        int rc = each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) -> int {
+            b200zk_group_pk::Shard& S = pk->shard[g];
+            S.v0 = cut(n_vars, g, P); S.v1 = cut(n_vars, g + 1, P);
+            S.l0 = cut(n_aux, g, P); S.l1 = cut(n_aux, g + 1, P);
+            S.hn = m / P;
+            const size_t cnt[5] = {S.v1 - S.v0, S.v1 - S.v0, S.v1 - S.v0, S.l1 - S.l0, S.hn};
+            const size_t psz[5] = {64, 64, 128, 64, 64};
+            const void* src[4] = {reinterpret_cast<const char*>(a_query) + S.v0 * 64, reinterpret_cast<const char*>(b_g1_query) + S.v0 * 64,
+                                  reinterpret_cast<const char*>(b_g2_query) + S.v0 * 128,
+                                  l_query ? reinterpret_cast<const char*>(l_query) + S.l0 * 64 : nullptr};
+            for (int k = 0; k < 5; ++k) {
+                if (cudaMalloc(&S.q[k], cnt[k] * psz[k] + 16) != cudaSuccess) return set_error(ctx, B200ZK_ERR_OOM, "proving-key shard allocation failed");
+                if (k < 4 && cnt[k] && cudaMemcpyAsync(S.q[k], src[k], cnt[k] * psz[k], cudaMemcpyHostToDevice, sl.stream) != cudaSuccess)
+                    return set_error(ctx, B200ZK_ERR_CUDA, "proving-key upload failed");
+            }
+            {   // h_query in the column layout of the h this device will compute: local[c][r] = h_query[r cols + g cg + c]
+                const size_t cg = cols / P;
+                if (sl.io_a.reserve(S.hn * 64) != cudaSuccess) return set_error(ctx, B200ZK_ERR_OOM, "staging allocation failed");
+                if (cudaMemcpy2DAsync(sl.io_a.p, cg * 64, reinterpret_cast<const char*>(h_query) + g * cg * 64, cols * 64, cg * 64, rows,
+                                      cudaMemcpyHostToDevice, sl.stream) != cudaSuccess)
+                    return set_error(ctx, B200ZK_ERR_CUDA, "h_query upload failed");
+                B2_TRY(transpose_dev<Blob64>(ctx, sl.stream, sl.io_a.p, S.q[4], rows, cg));
+            }
+            if (want_tables) {          // automatic windows only: B200ZK_PK_TABLE_WINDOW is not read here
+                size_t bytes = 0;
+                B2_TRY(pk_tables_build(ctx, sl, S.q, cnt, 0, S.tab, S.tab_c, &bytes));
+                pk->table_bytes += bytes;
+            }
+            return B200ZK_OK;
+        });
+        // device 0 keeps the vk points for the final assembly (queries of the tiny pk object are never read: include_zero_terms = 0)
+        if (!rc) rc = on_device(grp, 0, [&](b200zk_ctx* c0, Slot& s0) -> int {
+            pk->pk0 = new b200zk_pk();
+            pk->pk0->n_vars = n_vars; pk->pk0->n_inputs = n_inputs; pk->pk0->m = m;
+            if (cudaMalloc(&pk->pk0->vk, 56 * 8) != cudaSuccess || cudaMemcpyAsync(pk->pk0->vk, vk_points, 56 * 8, cudaMemcpyHostToDevice, s0.stream) != cudaSuccess)
+                return set_error(c0, B200ZK_ERR_CUDA, "vk upload failed");
+            return B200ZK_OK;
+        });
+        if (!rc) rc = sync_all(grp);
+        if (rc) {
+            b200zk_group_pk_free(grp, pk);
+            return rc;
         }
-        {   // h_query in the column layout of the h this device will compute: local[c][r] = h_query[r cols + g cg + c]
-            const size_t cg = cols / P;
-            if (sl.io_a.reserve(S.hn * 64) != cudaSuccess) return fail(gerr(grp, B200ZK_ERR_OOM, "staging allocation failed"));
-            if (cudaMemcpy2DAsync(sl.io_a.p, cg * 64, reinterpret_cast<const char*>(h_query) + g * cg * 64, cols * 64, cg * 64, rows,
-                                  cudaMemcpyHostToDevice, sl.stream) != cudaSuccess)
-                return fail(gerr(grp, B200ZK_ERR_CUDA, "h_query upload failed"));
-            int rc = gfrom(grp, g, transpose_dev<Blob64>(ctx, sl.stream, sl.io_a.p, S.q[4], rows, cg));
-            if (rc) return fail(rc);
-        }
-        if (want_tables) {          // automatic windows only: B200ZK_PK_TABLE_WINDOW is not read here
-            size_t bytes = 0;
-            int rc = gfrom(grp, g, pk_tables_build(ctx, sl, S.q, cnt, 0, S.tab, S.tab_c, &bytes));
-            if (rc) return fail(rc);
-            pk->table_bytes += bytes;
-        }
-    }
-    // device 0 keeps the vk points for the final assembly (queries of the tiny pk object are never read: include_zero_terms = 0)
-    {
-        b200zk_ctx* c0 = grp->ctx[0];
-        cudaSetDevice(c0->device);
-        pk->pk0 = new b200zk_pk();
-        pk->pk0->n_vars = n_vars; pk->pk0->n_inputs = n_inputs; pk->pk0->m = m;
-        if (cudaMalloc(&pk->pk0->vk, 56 * 8) != cudaSuccess ||
-            cudaMemcpyAsync(pk->pk0->vk, vk_points, 56 * 8, cudaMemcpyHostToDevice, c0->slots[0].stream) != cudaSuccess)
-            return fail(gerr(grp, B200ZK_ERR_CUDA, "vk upload failed"));
-    }
-    int rc = sync_all(grp);
-    if (rc) return fail(rc);
-    *out = pk;
-    return B200ZK_OK;
+        *out = pk;
+        return B200ZK_OK;
+    });
 }
 
 size_t b200zk_group_pk_table_bytes(const b200zk_group_pk* pk) { return pk ? pk->table_bytes : 0; }
 
 int b200zk_group_groth16_prove(b200zk_group* grp, const b200zk_group_pk* pk, const uint64_t* z, const uint64_t* a, const uint64_t* b,
                                const uint64_t* c, const uint64_t r[4], const uint64_t s[4], uint8_t proof_out[128]) {
-    DeviceGuard dev_guard;
-    if (!grp || !pk || !z || !a || !b || !c || !r || !s || !proof_out) return B200ZK_ERR_ARG;
-    if (pk->n != grp->n) return gerr(grp, B200ZK_ERR_ARG, "proving key was sharded for a different group");
-    const int P = grp->n;
-    const unsigned log_m = pk->log_m;
-    unsigned log_rows, log_cols;
-    split_log(log_m, &log_rows, &log_cols);
-    const size_t rows = (size_t)1 << log_rows, cols = (size_t)1 << log_cols, m = pk->m, loc = m / P;
-    SlotLocks locks(grp);
-    // staging per device: a, b, c (column layout) + 2 temporaries (t2 ends up holding h), then this device's rows of z
-    std::vector<void*> va(P), vb(P), vc(P), t1(P), t2(P);
-    std::vector<const Fr*> zq(P), zl(P);
-    for (int g = 0; g < P; ++g) {
-        b200zk_ctx* ctx = grp->ctx[g];
-        const b200zk_group_pk::Shard& S = pk->shard[g];
-        G_CUDA_OK(grp, cudaSetDevice(ctx->device));
-        const size_t zrows = std::max(S.v1 - S.v0, (S.l1 - S.l0));
-        G_CUDA_OK(grp, ctx->slots[0].io_a.reserve((5 * loc + (S.v1 - S.v0) + (S.l1 - S.l0) + zrows) * sizeof(Fr)));
-        G_CUDA_OK(grp, ctx->slots[0].small.reserve(4096));
-        Fr* p = reinterpret_cast<Fr*>(ctx->slots[0].io_a.p);
-        va[g] = p; vb[g] = p + loc; vc[g] = p + 2 * loc; t1[g] = p + 3 * loc; t2[g] = p + 4 * loc;
-        cudaStream_t st = ctx->slots[0].stream;
-        Fr* dz = p + 5 * loc;
-        Fr* dzaux = dz + (S.v1 - S.v0);
-        zq[g] = dz; zl[g] = dzaux;
-        G_CUDA_OK(grp, cudaMemcpyAsync(dz, reinterpret_cast<const char*>(z) + S.v0 * 32, (S.v1 - S.v0) * 32, cudaMemcpyHostToDevice, st));
-        G_CUDA_OK(grp, cudaMemcpyAsync(dzaux, reinterpret_cast<const char*>(z) + (pk->n_inputs + S.l0) * 32, (S.l1 - S.l0) * 32, cudaMemcpyHostToDevice, st));
-    }
-    int rc = scatter_columns<Blob32>(grp, a, rows, cols, t1.data(), va.data());
-    if (!rc) rc = scatter_columns<Blob32>(grp, b, rows, cols, t1.data(), vb.data());
-    if (!rc) rc = scatter_columns<Blob32>(grp, c, rows, cols, t1.data(), vc.data());
-    if (rc) return rc;
-    auto fr = [](std::vector<void*>& v) { return reinterpret_cast<Fr* const*>(v.data()); };
-    return prove_columns(grp, pk, fr(va), fr(vb), fr(vc), fr(t1), fr(t2), zq.data(), zl.data(), r, s, proof_out);
+    return with_group(grp, [&]() -> int {
+        if (!pk || !z || !a || !b || !c || !r || !s || !proof_out) return B200ZK_ERR_ARG;
+        if (pk->n != grp->n) return gerr(grp, B200ZK_ERR_ARG, "proving key was sharded for a different group");
+        const int P = grp->n;
+        unsigned log_rows, log_cols;
+        split_log(pk->log_m, &log_rows, &log_cols);
+        const size_t rows = (size_t)1 << log_rows, cols = (size_t)1 << log_cols, loc = pk->m / P;
+        // the tail: this device's rows of z, z[v0, v1) then z[n_inputs + l0, n_inputs + l1), and as many Fr again as the longer of the two
+        Columns w(P);
+        int rc = carve_columns(grp, loc, [&](int g) {
+            const b200zk_group_pk::Shard& S = pk->shard[g];
+            return (S.v1 - S.v0) + (S.l1 - S.l0) + std::max(S.v1 - S.v0, S.l1 - S.l0);
+        }, w);
+        std::vector<const Fr*> zq(P), zl(P);
+        if (!rc) rc = each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) -> int {
+            const b200zk_group_pk::Shard& S = pk->shard[g];
+            B2_CUDA_OK(ctx, sl.small.reserve(4096));
+            zq[g] = w.z[g];
+            zl[g] = w.z[g] + (S.v1 - S.v0);
+            B2_CUDA_OK(ctx, cudaMemcpyAsync(w.z[g], reinterpret_cast<const char*>(z) + S.v0 * 32, (S.v1 - S.v0) * 32, cudaMemcpyHostToDevice, sl.stream));
+            B2_CUDA_OK(ctx, cudaMemcpyAsync(w.z[g] + (S.v1 - S.v0), reinterpret_cast<const char*>(z) + (pk->n_inputs + S.l0) * 32, (S.l1 - S.l0) * 32,
+                                            cudaMemcpyHostToDevice, sl.stream));
+            return B200ZK_OK;
+        });
+        if (!rc) rc = scatter_columns(grp, a, rows, cols, w.t1.data(), w.a.data());
+        if (!rc) rc = scatter_columns(grp, b, rows, cols, w.t1.data(), w.b.data());
+        if (!rc) rc = scatter_columns(grp, c, rows, cols, w.t1.data(), w.c.data());
+        if (rc) return rc;
+        return prove_columns(grp, pk, w, zq.data(), zl.data(), r, s, proof_out);
+    });
 }
 
 // ---- R1CS sharded by output slot + prove from the witness on device 0 ---------------------------------------------------------
@@ -660,118 +653,113 @@ void b200zk_group_r1cs_free(b200zk_group* grp, b200zk_group_r1cs* q) {
 int b200zk_group_r1cs_upload(b200zk_group* grp, const uint32_t* a_row_ptr, const uint32_t* a_col, const uint64_t* a_val,
                              const uint32_t* b_row_ptr, const uint32_t* b_col, const uint64_t* b_val, size_t num_constraints,
                              size_t num_inputs, size_t n_vars, unsigned log_m, int values_montgomery_depth, b200zk_group_r1cs** out) {
-    DeviceGuard dev_guard;
-    if (!grp || !out || !a_row_ptr || !b_row_ptr) return B200ZK_ERR_ARG;
-    *out = nullptr;
-    if (log_m > 27) return gerr(grp, B200ZK_ERR_DOMAIN, "log_m > 27: 2m exceeds the 2^28 subgroup (PolynomialDegreeTooLarge)");
-    const size_t m = (size_t)1 << log_m, nc = num_constraints;
-    if (nc + num_inputs > m) return gerr(grp, B200ZK_ERR_DOMAIN, "num_constraints + num_inputs exceeds the domain size");
-    if (num_inputs == 0 || num_inputs > n_vars) return gerr(grp, B200ZK_ERR_ARG, "need 1 <= num_inputs <= n_vars");
-    const int P = grp->n;
-    unsigned log_rows, log_cols;
-    split_log(log_m, &log_rows, &log_cols);
-    if (((size_t)1 << log_cols) < (size_t)P) return gerr(grp, B200ZK_ERR_ARG, "domain too small for this many GPUs");
-    const uint32_t* row_ptr[2] = {a_row_ptr, b_row_ptr};
-    const uint32_t* col[2] = {a_col, b_col};
-    const uint64_t* val[2] = {a_val, b_val};
-    for (int k = 0; k < 2; ++k) {
-        int rc = check_csr(grp, k ? "B" : "A", row_ptr[k], col[k], val[k], nc, n_vars);
-        if (rc) return rc;
-    }
-    SlotLocks locks(grp);
-    b200zk_group_r1cs* q = new b200zk_group_r1cs();
-    q->owner = grp; q->nc = nc; q->n_inputs = num_inputs; q->n_vars = n_vars; q->m = m; q->log_m = log_m;
-    q->shard.resize(P);
-    auto fail = [&](int rc) { b200zk_group_r1cs_free(grp, q); return rc; };
-    const size_t loc = m / P;
-    std::vector<uint32_t> lptr(loc + 1), lcol;
-    std::vector<uint64_t> lval;
-    for (int g = 0; g < P; ++g) {
-        b200zk_ctx* ctx = grp->ctx[g];
-        Slot& sl = ctx->slots[0];
-        if (cudaSetDevice(ctx->device) != cudaSuccess) return fail(gerr(grp, B200ZK_ERR_CUDA, "cudaSetDevice failed"));
-        b200zk_group_r1cs::Shard& S = q->shard[g];
+    return with_group(grp, [&]() -> int {
+        if (!out || !a_row_ptr || !b_row_ptr) return B200ZK_ERR_ARG;
+        *out = nullptr;
+        if (log_m > 27) return gerr(grp, B200ZK_ERR_DOMAIN, "log_m > 27: 2m exceeds the 2^28 subgroup (PolynomialDegreeTooLarge)");
+        const size_t m = (size_t)1 << log_m, nc = num_constraints;
+        if (nc + num_inputs > m) return gerr(grp, B200ZK_ERR_DOMAIN, "num_constraints + num_inputs exceeds the domain size");
+        if (num_inputs == 0 || num_inputs > n_vars) return gerr(grp, B200ZK_ERR_ARG, "need 1 <= num_inputs <= n_vars");
+        const int P = grp->n;
+        unsigned log_rows, log_cols;
+        split_log(log_m, &log_rows, &log_cols);
+        if (((size_t)1 << log_cols) < (size_t)P) return gerr(grp, B200ZK_ERR_ARG, "domain too small for this many GPUs");
+        const uint32_t* row_ptr[2] = {a_row_ptr, b_row_ptr};
+        const uint32_t* col[2] = {a_col, b_col};
+        const uint64_t* val[2] = {a_val, b_val};
         for (int k = 0; k < 2; ++k) {
-            // the slice's rows in slot order, gathered once on the host (index and word copies only)
-            fill_local_row_ptr(row_ptr[k], nc, log_rows, log_cols, P, g, lptr.data());
-            const size_t nnz = lptr[loc];
-            lcol.resize(nnz);
-            lval.resize(nnz * 4);
-            for (size_t j = 0; j < loc; ++j) {
-                const size_t i = slot_row(j, log_rows, log_cols, P, g);
-                if (i >= nc || row_ptr[k][i + 1] == row_ptr[k][i]) continue;
-                const size_t lo = row_ptr[k][i], n = row_ptr[k][i + 1] - lo;
-                memcpy(lcol.data() + lptr[j], col[k] + lo, n * sizeof(uint32_t));
-                memcpy(lval.data() + (size_t)lptr[j] * 4, val[k] + lo * 4, n * 32);
-            }
-            if (cudaMalloc(&S.ptr[k], (loc + 1) * sizeof(uint32_t)) != cudaSuccess || cudaMalloc(&S.col[k], nnz * sizeof(uint32_t) + 16) != cudaSuccess ||
-                cudaMalloc(&S.val[k], nnz * 32 + 16) != cudaSuccess)
-                return fail(gerr(grp, B200ZK_ERR_OOM, "constraint-matrix shard allocation failed"));
-            // pageable sources: each copy has consumed its source when the call returns, so the host vectors can be refilled
-            if (cudaMemcpyAsync(S.ptr[k], lptr.data(), (loc + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, sl.stream) != cudaSuccess ||
-                (nnz && cudaMemcpyAsync(S.col[k], lcol.data(), nnz * sizeof(uint32_t), cudaMemcpyHostToDevice, sl.stream) != cudaSuccess) ||
-                (nnz && cudaMemcpyAsync(S.val[k], lval.data(), nnz * 32, cudaMemcpyHostToDevice, sl.stream) != cudaSuccess))
-                return fail(gerr(grp, B200ZK_ERR_CUDA, "constraint-matrix upload failed"));
-            if (values_montgomery_depth != 0) {
-                const int to_mont = values_montgomery_depth < 0, times = to_mont ? -values_montgomery_depth : values_montgomery_depth;
-                int rc = gfrom(grp, g, fr_convert_dev(ctx, sl, S.val[k], S.val[k], nnz, to_mont, times));
-                if (rc) return fail(rc);
-            }
+            int rc = check_csr(grp, k ? "B" : "A", row_ptr[k], col[k], val[k], nc, n_vars);
+            if (rc) return rc;
         }
-    }
-    int rc = sync_all(grp);
-    if (rc) return fail(rc);
-    *out = q;
-    return B200ZK_OK;
+        b200zk_group_r1cs* q = new b200zk_group_r1cs();
+        q->owner = grp; q->nc = nc; q->n_inputs = num_inputs; q->n_vars = n_vars; q->m = m; q->log_m = log_m;
+        q->shard.resize(P);
+        const size_t loc = m / P;
+        std::vector<uint32_t> lptr(loc + 1), lcol;
+        std::vector<uint64_t> lval;
+        int rc = each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) -> int {
+            b200zk_group_r1cs::Shard& S = q->shard[g];
+            for (int k = 0; k < 2; ++k) {
+                // the slice's rows in slot order, gathered once on the host (index and word copies only)
+                fill_local_row_ptr(row_ptr[k], nc, log_rows, log_cols, P, g, lptr.data());
+                const size_t nnz = lptr[loc];
+                lcol.resize(nnz);
+                lval.resize(nnz * 4);
+                for (size_t j = 0; j < loc; ++j) {
+                    const size_t i = slot_row(j, log_rows, log_cols, P, g);
+                    if (i >= nc || row_ptr[k][i + 1] == row_ptr[k][i]) continue;
+                    const size_t lo = row_ptr[k][i], n = row_ptr[k][i + 1] - lo;
+                    memcpy(lcol.data() + lptr[j], col[k] + lo, n * sizeof(uint32_t));
+                    memcpy(lval.data() + (size_t)lptr[j] * 4, val[k] + lo * 4, n * 32);
+                }
+                if (cudaMalloc(&S.ptr[k], (loc + 1) * sizeof(uint32_t)) != cudaSuccess || cudaMalloc(&S.col[k], nnz * sizeof(uint32_t) + 16) != cudaSuccess ||
+                    cudaMalloc(&S.val[k], nnz * 32 + 16) != cudaSuccess)
+                    return set_error(ctx, B200ZK_ERR_OOM, "constraint-matrix shard allocation failed");
+                // pageable sources: each copy has consumed its source when the call returns, so the host vectors can be refilled
+                if (cudaMemcpyAsync(S.ptr[k], lptr.data(), (loc + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, sl.stream) != cudaSuccess ||
+                    (nnz && cudaMemcpyAsync(S.col[k], lcol.data(), nnz * sizeof(uint32_t), cudaMemcpyHostToDevice, sl.stream) != cudaSuccess) ||
+                    (nnz && cudaMemcpyAsync(S.val[k], lval.data(), nnz * 32, cudaMemcpyHostToDevice, sl.stream) != cudaSuccess))
+                    return set_error(ctx, B200ZK_ERR_CUDA, "constraint-matrix upload failed");
+                if (values_montgomery_depth != 0) {
+                    const int to_mont = values_montgomery_depth < 0, times = to_mont ? -values_montgomery_depth : values_montgomery_depth;
+                    B2_TRY(fr_convert_dev(ctx, sl, S.val[k], S.val[k], nnz, to_mont, times));
+                }
+            }
+            return B200ZK_OK;
+        });
+        if (!rc) rc = sync_all(grp);
+        if (rc) {
+            b200zk_group_r1cs_free(grp, q);
+            return rc;
+        }
+        *out = q;
+        return B200ZK_OK;
+    });
 }
 
 int b200zk_group_groth16_prove_r1cs_dev(b200zk_group* grp, const b200zk_group_pk* pk, const b200zk_group_r1cs* q, const void* d_z,
                                         const uint64_t r[4], const uint64_t s[4], uint8_t proof_out[128]) {
-    DeviceGuard dev_guard;
-    if (!grp || !pk || !q || !d_z || !r || !s || !proof_out) return B200ZK_ERR_ARG;
-    if (pk->owner != grp) return gerr(grp, B200ZK_ERR_ARG, "proving key was uploaded to a different group");
-    if (q->owner != grp) return gerr(grp, B200ZK_ERR_ARG, "constraint matrices were uploaded to a different group");
-    if (q->m != pk->m)
-        return gerr(grp, B200ZK_ERR_DOMAIN, "constraint matrices of domain " + std::to_string(q->m) + ", proving key of domain " + std::to_string(pk->m));
-    if (q->n_inputs != pk->n_inputs)
-        return gerr(grp, B200ZK_ERR_ARG, "constraint matrices with " + std::to_string(q->n_inputs) + " inputs, proving key with " + std::to_string(pk->n_inputs));
-    if (q->n_vars != pk->n_vars)
-        return gerr(grp, B200ZK_ERR_ARG, "constraint matrices over " + std::to_string(q->n_vars) + " variables, proving key over " + std::to_string(pk->n_vars));
-    const int P = grp->n;
-    unsigned log_rows, log_cols;
-    split_log(pk->log_m, &log_rows, &log_cols);
-    const size_t cg = ((size_t)1 << log_cols) / P, loc = pk->m / P, zbytes = pk->n_vars * sizeof(Fr);
-    SlotLocks locks(grp);
-    // the caller wrote z on device 0's slot-0 stream: every other device's copy of it waits for that point
-    b200zk_ctx* c0 = grp->ctx[0];
-    G_CUDA_OK(grp, cudaSetDevice(c0->device));
-    G_CUDA_OK(grp, cudaEventRecord(grp->ev_done[0], c0->slots[0].stream));
-    // per device: a, b, c (column layout, written by the mat-vec) + 2 temporaries (t2 ends up holding h), then (devices >= 1) z
-    std::vector<void*> va(P), vb(P), vc(P), t1(P), t2(P);
-    std::vector<const Fr*> zq(P), zl(P);
-    for (int g = 0; g < P; ++g) {
-        b200zk_ctx* ctx = grp->ctx[g];
-        Slot& sl = ctx->slots[0];
-        const b200zk_group_pk::Shard& S = pk->shard[g];
-        const b200zk_group_r1cs::Shard& Q = q->shard[g];
-        G_CUDA_OK(grp, cudaSetDevice(ctx->device));
-        G_CUDA_OK(grp, sl.io_a.reserve(5 * loc * sizeof(Fr) + (g ? zbytes : 0)));
-        G_CUDA_OK(grp, sl.small.reserve(4096));
-        Fr* p = reinterpret_cast<Fr*>(sl.io_a.p);
-        va[g] = p; vb[g] = p + loc; vc[g] = p + 2 * loc; t1[g] = p + 3 * loc; t2[g] = p + 4 * loc;
-        const Fr* z = reinterpret_cast<const Fr*>(d_z);
-        if (g) {
-            G_CUDA_OK(grp, cudaStreamWaitEvent(sl.stream, grp->ev_done[0], 0));
-            G_CUDA_OK(grp, cudaMemcpyPeerAsync(p + 5 * loc, ctx->device, d_z, c0->device, zbytes, sl.stream));
-            z = p + 5 * loc;
-        }
-        zq[g] = z + S.v0;
-        zl[g] = z + pk->n_inputs + S.l0;
-        G_TRY(grp, g, qap_slots_dev(ctx, sl, Q.ptr[0], Q.col[0], Q.val[0], Q.ptr[1], Q.col[1], Q.val[1], q->nc, q->n_inputs, z, log_rows, log_cols,
-                                    (size_t)g * cg, loc, va[g], vb[g], vc[g]));
-    }
-    auto fr = [](std::vector<void*>& v) { return reinterpret_cast<Fr* const*>(v.data()); };
-    return prove_columns(grp, pk, fr(va), fr(vb), fr(vc), fr(t1), fr(t2), zq.data(), zl.data(), r, s, proof_out);
+    return with_group(grp, [&]() -> int {
+        if (!pk || !q || !d_z || !r || !s || !proof_out) return B200ZK_ERR_ARG;
+        if (pk->owner != grp) return gerr(grp, B200ZK_ERR_ARG, "proving key was uploaded to a different group");
+        if (q->owner != grp) return gerr(grp, B200ZK_ERR_ARG, "constraint matrices were uploaded to a different group");
+        if (q->m != pk->m)
+            return gerr(grp, B200ZK_ERR_DOMAIN, "constraint matrices of domain " + std::to_string(q->m) + ", proving key of domain " + std::to_string(pk->m));
+        if (q->n_inputs != pk->n_inputs)
+            return gerr(grp, B200ZK_ERR_ARG, "constraint matrices with " + std::to_string(q->n_inputs) + " inputs, proving key with " + std::to_string(pk->n_inputs));
+        if (q->n_vars != pk->n_vars)
+            return gerr(grp, B200ZK_ERR_ARG, "constraint matrices over " + std::to_string(q->n_vars) + " variables, proving key over " + std::to_string(pk->n_vars));
+        const int P = grp->n;
+        unsigned log_rows, log_cols;
+        split_log(pk->log_m, &log_rows, &log_cols);
+        const size_t cg = ((size_t)1 << log_cols) / P, loc = pk->m / P, zbytes = pk->n_vars * sizeof(Fr);
+        // the caller wrote z on device 0's slot-0 stream: every other device's copy of it waits for that point
+        int rc = on_device(grp, 0, [&](b200zk_ctx* c0, Slot& s0) -> int {
+            B2_CUDA_OK(c0, cudaEventRecord(grp->ev_done[0], s0.stream));
+            return B200ZK_OK;
+        });
+        // the tail (devices >= 1): a copy of z.  a, b, c are written by the mat-vec.
+        Columns w(P);
+        if (!rc) rc = carve_columns(grp, loc, [&](int g) { return g ? pk->n_vars : 0; }, w);
+        std::vector<const Fr*> zq(P), zl(P);
+        if (!rc) rc = each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) -> int {
+            const b200zk_group_pk::Shard& S = pk->shard[g];
+            const b200zk_group_r1cs::Shard& Q = q->shard[g];
+            B2_CUDA_OK(ctx, sl.small.reserve(4096));
+            const Fr* z = reinterpret_cast<const Fr*>(d_z);
+            if (g) {
+                B2_CUDA_OK(ctx, cudaStreamWaitEvent(sl.stream, grp->ev_done[0], 0));
+                B2_CUDA_OK(ctx, cudaMemcpyPeerAsync(w.z[g], ctx->device, d_z, grp->ctx[0]->device, zbytes, sl.stream));
+                z = w.z[g];
+            }
+            zq[g] = z + S.v0;
+            zl[g] = z + pk->n_inputs + S.l0;
+            return qap_slots_dev(ctx, sl, Q.ptr[0], Q.col[0], Q.val[0], Q.ptr[1], Q.col[1], Q.val[1], q->nc, q->n_inputs, z, log_rows, log_cols,
+                                 (size_t)g * cg, loc, w.a[g], w.b[g], w.c[g]);
+        });
+        if (rc) return rc;
+        return prove_columns(grp, pk, w, zq.data(), zl.data(), r, s, proof_out);
+    });
 }
 
 }  // extern "C"
