@@ -139,6 +139,12 @@ SIGNATURES = {
     "b200zk_group_r1cs_free": (None, [c_vp, c_vp]),
     "b200zk_group_r1cs_local_row_ptr": (ctypes.c_int, [c_vp, ctypes.c_size_t, ctypes.c_uint, ctypes.c_int, ctypes.c_int, c_vp]),
     "b200zk_group_groth16_prove_r1cs_dev": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b200zk_group_zkey_load": (ctypes.c_int, [c_vp, c_vp, ctypes.c_size_t, ctypes.c_uint, ctypes.POINTER(c_vp)]),
+    "b200zk_group_zkey_free": (None, [c_vp, c_vp]),
+    "b200zk_group_zkey_info": (ctypes.c_int, [c_vp] + [ctypes.POINTER(ctypes.c_size_t)] * 4),
+    "b200zk_group_zkey_table_bytes": (ctypes.c_size_t, [c_vp]),
+    "b200zk_group_zkey_prove": (ctypes.c_int, [c_vp, c_vp, c_vp, ctypes.c_size_t, c_vp, c_vp, c_vp, ctypes.c_char_p,
+                                               ctypes.POINTER(ctypes.c_size_t), ctypes.c_char_p, ctypes.POINTER(ctypes.c_size_t)]),
     "b200zk_fr_op": (ctypes.c_int, [c_vp, ctypes.c_int, c_vp, c_vp, c_vp, ctypes.c_size_t]),
     "b200zk_test_field_op": (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_vp, c_vp, c_vp, ctypes.c_size_t]),
     "b200zk_test_arith": (ctypes.c_int, [c_vp, ctypes.c_int, c_vp, ctypes.c_size_t, c_vp]),

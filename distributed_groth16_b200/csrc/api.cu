@@ -607,25 +607,17 @@ int b200zk_zkey_load(b200zk_ctx* ctx, const void* zkey, size_t zkey_len, unsigne
     const uint8_t* file = reinterpret_cast<const uint8_t*>(zkey);
     sjf::Zkey h;
     std::string err;
-    if (!sjf::parse_zkey(file, zkey_len, &h, &err)) return set_error(ctx, B200ZK_ERR_ARG, err);
-    if (h.domain_size > (1u << 27)) {
-        return set_error(ctx, B200ZK_ERR_DOMAIN, "zkey domain size " + std::to_string(h.domain_size) +
-                                                     " exceeds 2^27: the h step needs twice the domain within Fr's 2^28 subgroup");
-    }
+    const int hrc = zkey_header(file, zkey_len, &h, &err);
+    if (hrc) return set_error(ctx, hrc, err);
     b200zk_zkey* zk = new b200zk_zkey();
     zk->n_vars = h.n_vars;
     zk->n_public = h.n_public;
     zk->domain_size = h.domain_size;
     int rc = with_slot(ctx, 0, [&](Slot& sl) { return zkey_matrices_dev(ctx, sl, file, h, zk); });
     if (!rc) {
-        // vk points in b200zk_pk_upload's order from the header's alpha_1 beta_1 beta_2 gamma_2 delta_1 delta_2; the queries go
-        // from the caller's bytes, which are already the device layout
-        const uint8_t* hp = file + h.hdr_points;
+        // the queries go from the caller's bytes, which are already the device layout
         uint64_t vk[56];
-        memcpy(vk, hp, 128);                    // alpha_1, beta_1
-        memcpy(vk + 16, hp + 384, 64);          // delta_1
-        memcpy(vk + 24, hp + 128, 128);         // beta_2
-        memcpy(vk + 40, hp + 448, 128);         // delta_2
+        zkey_vk_points(file, h, vk);
         rc = pk_build(ctx, file + h.a, file + h.b1, file + h.b2, file + h.l, file + h.h, h.n_vars, (size_t)h.n_public + 1, h.domain_size,
                       vk, cudaMemcpyHostToDevice, table_window, &zk->pk);
     }

@@ -1,9 +1,11 @@
-// b200zk-prove [--device N] <circuit.zkey> <witness.wtns> <proof.json> <public.json>
+// b200zk-prove [--device N | --devices I,J,...] <circuit.zkey> <witness.wtns> <proof.json> <public.json>
 //
 // snarkjs `groth16 prove` as one process, with the positional arguments of rapidsnark's prover: the zkey is loaded without
-// fixed-base tables (b200zk_zkey_load, table_window 0xFFFFFFFF: one proof does not pay back their build), r and s are drawn
-// from the OS, and proof.json / public.json are written as snarkjs writes them.  On any failure it prints the library's
-// message on stderr, exits non-zero and leaves neither output file behind.
+// fixed-base tables (table_window 0xFFFFFFFF: one proof does not pay back their build), r and s are drawn from the OS, and
+// proof.json / public.json are written as snarkjs writes them.  --device N proves on one GPU (b200zk_zkey_*), --devices on a
+// group of 1, 2, 4 or 8 of them (b200zk_group_zkey_*; an id may repeat, which emulates the group on fewer GPUs).  A usage
+// error exits 2 before any CUDA call.  On any other failure it prints the library's message on stderr, exits 1 and leaves
+// neither output file behind.
 #include <errno.h>
 #include <fcntl.h>
 #include <stdio.h>
@@ -14,6 +16,7 @@
 #include <unistd.h>
 
 #include <string>
+#include <vector>
 
 #include "../../include/b200zk.h"
 
@@ -53,18 +56,109 @@ int fail(const std::string& msg) {
     return 1;
 }
 
+// "0,1,2,3" -> ids; false for an empty or malformed list or a count other than 1, 2, 4 or 8
+bool parse_devices(const char* s, std::vector<int>* ids) {
+    for (const char* p = s;; ++p) {
+        char* end = nullptr;
+        if (*p < '0' || *p > '9') return false;
+        const long v = strtol(p, &end, 10);
+        if (v > 1 << 20) return false;
+        ids->push_back((int)v);
+        p = end;
+        if (*p == 0) break;
+        if (*p != ',') return false;
+    }
+    const size_t n = ids->size();
+    return n == 1 || n == 2 || n == 4 || n == 8;
+}
+
+// the two texts; on failure *err holds the library's message (context or group) or the failed create's code
+struct Outputs {
+    std::string proof_json, public_json;
+};
+
+int prove_one(int device, const Mapped& zkey, const Mapped& wtns, Outputs* out, std::string* err) {
+    b200zk_ctx* ctx = nullptr;
+    const int rc_ctx = b200zk_ctx_create(device, &ctx);
+    if (rc_ctx != B200ZK_OK) {
+        // no context, so no library message: the code says what kind of failure it was
+        *err = "could not create a context on CUDA device " + std::to_string(device) + ": b200zk_ctx_create returned " +
+               std::to_string(rc_ctx) + (rc_ctx == B200ZK_ERR_CUDA ? " (B200ZK_ERR_CUDA: the device is missing, or the CUDA "
+                                                                     "runtime could not set it up)" : "");
+        return rc_ctx;
+    }
+    b200zk_zkey* zk = nullptr;
+    out->proof_json.assign(B200ZK_PROOF_JSON_MAX, '\0');
+    int rc = b200zk_zkey_load(ctx, zkey.p == MAP_FAILED ? "" : zkey.p, zkey.len, 0xFFFFFFFFu, &zk);
+    if (rc == B200ZK_OK) {
+        size_t n_public = 0;
+        b200zk_zkey_info(zk, nullptr, &n_public, nullptr, nullptr);
+        out->public_json.assign(B200ZK_PUBLIC_JSON_MAX(n_public), '\0');
+        size_t proof_len = out->proof_json.size(), public_len = out->public_json.size();
+        const void* w = wtns.p == MAP_FAILED ? "" : wtns.p;
+        rc = b200zk_zkey_prove(ctx, zk, w, wtns.len, nullptr, nullptr, nullptr, &out->proof_json[0], &proof_len, &out->public_json[0],
+                               &public_len);
+        if (rc == B200ZK_OK) {
+            out->proof_json.resize(proof_len);
+            out->public_json.resize(public_len);
+        }
+    }
+    if (rc != B200ZK_OK) *err = b200zk_last_error(ctx);
+    b200zk_zkey_free(ctx, zk);
+    b200zk_ctx_destroy(ctx);
+    return rc;
+}
+
+int prove_group(const std::vector<int>& ids, const Mapped& zkey, const Mapped& wtns, Outputs* out, std::string* err) {
+    b200zk_group* grp = nullptr;
+    const int rc_grp = b200zk_group_create(ids.data(), (int)ids.size(), &grp);
+    if (rc_grp != B200ZK_OK) {
+        // no group, so no library message
+        *err = "could not create a group on the CUDA devices given: b200zk_group_create returned " + std::to_string(rc_grp) +
+               (rc_grp == B200ZK_ERR_CUDA ? " (B200ZK_ERR_CUDA: a device is missing, two devices cannot reach each other, or the "
+                                            "CUDA runtime could not set one up)" : "");
+        return rc_grp;
+    }
+    b200zk_group_zkey* zk = nullptr;
+    out->proof_json.assign(B200ZK_PROOF_JSON_MAX, '\0');
+    int rc = b200zk_group_zkey_load(grp, zkey.p == MAP_FAILED ? "" : zkey.p, zkey.len, 0xFFFFFFFFu, &zk);
+    if (rc == B200ZK_OK) {
+        size_t n_public = 0;
+        b200zk_group_zkey_info(zk, nullptr, &n_public, nullptr, nullptr);
+        out->public_json.assign(B200ZK_PUBLIC_JSON_MAX(n_public), '\0');
+        size_t proof_len = out->proof_json.size(), public_len = out->public_json.size();
+        const void* w = wtns.p == MAP_FAILED ? "" : wtns.p;
+        rc = b200zk_group_zkey_prove(grp, zk, w, wtns.len, nullptr, nullptr, nullptr, &out->proof_json[0], &proof_len,
+                                     &out->public_json[0], &public_len);
+        if (rc == B200ZK_OK) {
+            out->proof_json.resize(proof_len);
+            out->public_json.resize(public_len);
+        }
+    }
+    if (rc != B200ZK_OK) *err = b200zk_group_last_error(grp);
+    b200zk_group_zkey_free(grp, zk);
+    b200zk_group_destroy(grp);
+    return rc;
+}
+
 }  // namespace
 
 int main(int argc, char** argv) {
     int device = 0, a = 1;
+    std::vector<int> ids;
+    bool usage = false;
     if (argc == 7 && strcmp(argv[1], "--device") == 0) {
         char* end = nullptr;
         device = (int)strtol(argv[2], &end, 10);
-        if (!*argv[2] || *end) argc = 0;
+        usage = !*argv[2] || *end;
+        a = 3;
+    } else if (argc == 7 && strcmp(argv[1], "--devices") == 0) {
+        usage = !parse_devices(argv[2], &ids);
         a = 3;
     }
-    if (argc - a != 4) {
-        fprintf(stderr, "usage: b200zk-prove [--device N] <circuit.zkey> <witness.wtns> <proof.json> <public.json>\n");
+    if (usage || argc - a != 4) {
+        fprintf(stderr, "usage: b200zk-prove [--device N | --devices I,J,... (1, 2, 4 or 8 ids)] <circuit.zkey> <witness.wtns> "
+                        "<proof.json> <public.json>\n");
         return 2;
     }
     const char *zkey_path = argv[a], *wtns_path = argv[a + 1];
@@ -73,41 +167,13 @@ int main(int argc, char** argv) {
     Mapped zkey, wtns;
     if (!map_file(zkey_path, &zkey, &err) || !map_file(wtns_path, &wtns, &err)) return fail(err);
 
-    b200zk_ctx* ctx = nullptr;
-    const int rc_ctx = b200zk_ctx_create(device, &ctx);
-    if (rc_ctx != B200ZK_OK) {
-        // no context, so no library message: the code says what kind of failure it was
-        return fail("could not create a context on CUDA device " + std::to_string(device) + ": b200zk_ctx_create returned " +
-                    std::to_string(rc_ctx) + (rc_ctx == B200ZK_ERR_CUDA ? " (B200ZK_ERR_CUDA: the device is missing, or the CUDA "
-                                                                          "runtime could not set it up)" : ""));
-    }
-    b200zk_zkey* zk = nullptr;
-    std::string proof_json(B200ZK_PROOF_JSON_MAX, '\0'), public_json;
-    int rc = b200zk_zkey_load(ctx, zkey.p == MAP_FAILED ? "" : zkey.p, zkey.len, 0xFFFFFFFFu, &zk);
-    if (rc == B200ZK_OK) {
-        size_t n_public = 0;
-        b200zk_zkey_info(zk, nullptr, &n_public, nullptr, nullptr);
-        public_json.assign(B200ZK_PUBLIC_JSON_MAX(n_public), '\0');
-        size_t proof_len = proof_json.size(), public_len = public_json.size();
-        const void* w = wtns.p == MAP_FAILED ? "" : wtns.p;
-        rc = b200zk_zkey_prove(ctx, zk, w, wtns.len, nullptr, nullptr, nullptr, &proof_json[0], &proof_len, &public_json[0], &public_len);
-        if (rc == B200ZK_OK) {
-            proof_json.resize(proof_len);
-            public_json.resize(public_len);
-        }
-    }
-    if (rc != B200ZK_OK) {
-        err = b200zk_last_error(ctx);
-        b200zk_zkey_free(ctx, zk);
-        b200zk_ctx_destroy(ctx);
-        return fail(err);
-    }
-    b200zk_zkey_free(ctx, zk);
-    b200zk_ctx_destroy(ctx);
+    Outputs out;
+    const int rc = ids.empty() ? prove_one(device, zkey, wtns, &out, &err) : prove_group(ids, zkey, wtns, &out, &err);
+    if (rc != B200ZK_OK) return fail(err);
 
     const std::string proof_tmp = proof_path + ".tmp", public_tmp = public_path + ".tmp";
-    if (!write_tmp(proof_tmp, proof_json.data(), proof_json.size(), &err)) return fail(err);
-    if (!write_tmp(public_tmp, public_json.data(), public_json.size(), &err)) {
+    if (!write_tmp(proof_tmp, out.proof_json.data(), out.proof_json.size(), &err)) return fail(err);
+    if (!write_tmp(public_tmp, out.public_json.data(), out.public_json.size(), &err)) {
         unlink(proof_tmp.c_str());
         return fail(err);
     }

@@ -186,6 +186,22 @@ static inline unsigned ceil_log2(size_t n) {
     return l;
 }
 
+// The column layout of a 2^(log_rows + log_cols) vector over P = 2^(log_cols - log_cg) GPUs (group.cu): GPU g keeps the
+// cg = 2^log_cg columns [g cg, (g+1) cg), its local slot c rows + r holding global row r cols + g cg + c.  The one definition
+// of the map in both directions, for the host (slot_row, the sharded row_ptr) and the device (the group zkey's sort key).
+struct ColumnLayout {
+    uint32_t log_rows, log_cols, log_cg;
+    __host__ __device__ __forceinline__ size_t row(uint32_t g, size_t j) const {           // slot j of GPU g -> global row
+        return ((j & (((size_t)1 << log_rows) - 1)) << log_cols) + ((size_t)g << log_cg) + (j >> log_rows);
+    }
+    __host__ __device__ __forceinline__ uint32_t owner(uint32_t R) const {                 // global row -> its GPU
+        return (R & ((1u << log_cols) - 1)) >> log_cg;
+    }
+    __host__ __device__ __forceinline__ uint32_t slot(uint32_t R) const {                  // global row -> its owner's slot
+        return ((R & ((1u << log_cg) - 1)) << log_rows) + (R >> log_cols);
+    }
+};
+
 // ---- entry points implemented across translation units -------------------------------------
 // ntt.cu
 int ntt_dev(b200zk_ctx* ctx, Slot& sl, const Fr* d_in, Fr* d_out, unsigned log_n, bool inverse, bool coset,
@@ -288,7 +304,41 @@ int prove_dev(b200zk_ctx* ctx, const b200zk_pk* pk, const Fr* d_z, const Fr* d_a
               const uint64_t r[4], const uint64_t s[4], int mirror_bg1, uint8_t proof_out[128]);
 // zkey.cu (the header fields come from snarkjs_files.h's parse_zkey)
 namespace sjf { struct Zkey; }
+// parse_zkey and the 2^27 domain limit of every zkey load: B200ZK_OK, or the code with *err
+int zkey_header(const uint8_t* file, size_t len, sjf::Zkey* h, std::string* err);
+// the 56 vk limbs of b200zk_pk_upload from the header's points
+void zkey_vk_points(const uint8_t* file, const sjf::Zkey& h, uint64_t vk[56]);
 int zkey_matrices_dev(b200zk_ctx* ctx, Slot& sl, const uint8_t* file, const sjf::Zkey& h, b200zk_zkey* zk);
+// The group load's sort on one device: the checked records keyed owner-major over the layout cl, in one allocation `csr` (the
+// caller frees it): row_ptr of 2 m + 1 entries, GPU g's A rows at [2 g loc, (2 g + 1) loc] and B rows at [(2 g + 1) loc,
+// 2 (g + 1) loc] (loc = m / P), indexing col / val
+struct ZkeyCsr {
+    void* csr = nullptr;
+    uint32_t* row_ptr = nullptr;
+    uint32_t* col = nullptr;
+    Fr* val = nullptr;
+    uint32_t nc = 0;
+};
+int zkey_group_matrices_dev(b200zk_ctx* ctx, Slot& sl, const uint8_t* file, const sjf::Zkey& h, const ColumnLayout& cl, ZkeyCsr* out);
+// p[i] -= base, i < n, on the slot's stream
+int rebase_dev(b200zk_ctx* ctx, Slot& sl, uint32_t* p, size_t n, uint32_t base);
+// The host side of a prove from a .wtns, before any launch: parse, entry count, JSON buffer sizes (both lengths set when one
+// is short), r and s (drawn from getrandom when null).  B200ZK_OK, or the code with *err.
+struct WtnsJob {
+    const uint8_t* z = nullptr;          // n_vars canonical values in the caller's bytes
+    std::string pub;                     // public.json
+    uint64_t r[4], s[4];
+};
+int wtns_prologue(const uint8_t* wtns, size_t wtns_len, size_t n_vars, size_t n_public, const uint64_t* r_in, const uint64_t* s_in,
+                  const char* proof_json, size_t* proof_json_len, const char* public_json, size_t* public_json_len, WtnsJob* job,
+                  std::string* err);
+// the nv canonical values z -> Montgomery at d_z (refused, with a context error, when an entry is not below r)
+int witness_to_device(b200zk_ctx* ctx, Slot& sl, const uint8_t* z, size_t nv, Fr* d_z);
+// the scratch in sl.io_a that zkey_outputs_dev uses
+static const size_t JSON_SCRATCH = 768;
+// proof bytes and texts to the caller: proof_out, public.json, and proof.json from the points' encodings made on sl
+int zkey_outputs_dev(b200zk_ctx* ctx, Slot& sl, const uint8_t proof[128], const WtnsJob& job, uint8_t* proof_out, char* proof_json,
+                     size_t* proof_json_len, char* public_json, size_t* public_json_len);
 int zkey_prove_dev(b200zk_ctx* ctx, Slot& sl, const b200zk_zkey* zk, const uint8_t* wtns, size_t wtns_len, const uint64_t* r,
                    const uint64_t* s, uint8_t* proof_out, char* proof_json, size_t* proof_json_len, char* public_json,
                    size_t* public_json_len);

@@ -20,6 +20,7 @@
 // GPU g of P owns columns [g cols/P, (g+1) cols/P), each stored contiguously: local[c][r] = x[r cols + g cols/P + c].
 // A transform with (rows, cols) maps layout(cols) to layout(rows), so iNTT -> NTT chains need no redistribution.
 #include "common.cuh"
+#include "snarkjs_files.h"
 
 #include <algorithm>
 
@@ -64,6 +65,17 @@ struct b200zk_group_r1cs {
         void* val[2] = {};
     };
     std::vector<Shard> shard;
+};
+
+// A snarkjs Groth16 zkey resident on a group (b200zk_group_zkey_load): the sharded proving key, and per device one allocation
+// csr[g] behind A and B of its column-layout slice, row_ptr (2 loc + 1 entries: A's rows at [0, loc], B's at [loc, 2 loc])
+// then val then col, exactly b200zk_zkey's layout.  mats[g] views it as b200zk_group_r1cs shards (which own nothing here).
+struct b200zk_group_zkey {
+    const b200zk_group* owner = nullptr;
+    b200zk_group_pk* pk = nullptr;
+    size_t n_vars = 0, n_public = 0, domain_size = 0, num_constraints = 0;
+    std::vector<void*> csr;
+    std::vector<b200zk_group_r1cs::Shard> mats;
 };
 
 namespace {
@@ -324,7 +336,7 @@ int sharded_h(b200zk_group* grp, const Columns& w, unsigned log_m) {
 // Slot j of GPU g's column-layout slice holds global row (j mod rows) cols + g cols / P + j div rows (local[c rows + r] =
 // x[r cols + g cg + c]); qap.cu's global_row is the device twin
 size_t slot_row(size_t j, unsigned log_rows, unsigned log_cols, int P, int g) {
-    return ((j & (((size_t)1 << log_rows) - 1)) << log_cols) + (size_t)g * (((size_t)1 << log_cols) / P) + (j >> log_rows);
+    return ColumnLayout{log_rows, log_cols, log_cols - ceil_log2((size_t)P)}.row((uint32_t)g, j);
 }
 
 // The m / P + 1 entries of GPU g's slice CSR row_ptr from the global one (num_constraints + 1 entries; global rows >=
@@ -395,6 +407,113 @@ int prove_columns(b200zk_group* grp, const b200zk_group_pk* pk, const Columns& w
     });
     if (rc) return rc;
     return sync_all(grp);
+}
+
+// b200zk_group_groth16_prove_r1cs_dev after its checks, on A and B sharded as mats[g] (b200zk_group_r1cs's layout): the full
+// witness on device 0 is peer-copied to every other device, each device computes its column-layout slice of a, b, c, then
+// prove_columns.  z0(c0, s0, tail, &z) gives device 0's witness on its slot-0 stream: the caller's, or one it writes into
+// `tail`, n_vars Fr that are reserved on device 0 only when z0_in_tail.
+template <class Z0>
+int prove_r1cs_columns(b200zk_group* grp, const b200zk_group_pk* pk, const std::vector<b200zk_group_r1cs::Shard>& mats, size_t nc,
+                       size_t n_inputs, bool z0_in_tail, Z0&& z0, const uint64_t r[4], const uint64_t s[4], uint8_t proof_out[128]) {
+    const int P = grp->n;
+    unsigned log_rows, log_cols;
+    split_log(pk->log_m, &log_rows, &log_cols);
+    const size_t cg = ((size_t)1 << log_cols) / P, loc = pk->m / P, zbytes = pk->n_vars * sizeof(Fr);
+    // the tail (devices >= 1, and device 0 for z0_in_tail): a copy of z.  a, b, c are written by the mat-vec.
+    Columns w(P);
+    int rc = carve_columns(grp, loc, [&](int g) { return g || z0_in_tail ? pk->n_vars : 0; }, w);
+    // every other device's copy of z waits for the point where device 0's stream holds it
+    const Fr* z0p = nullptr;
+    if (!rc) rc = on_device(grp, 0, [&](b200zk_ctx* c0, Slot& s0) -> int {
+        B2_TRY(z0(c0, s0, w.z[0], &z0p));
+        B2_CUDA_OK(c0, cudaEventRecord(grp->ev_done[0], s0.stream));
+        return B200ZK_OK;
+    });
+    std::vector<const Fr*> zq(P), zl(P);
+    if (!rc) rc = each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) -> int {
+        const b200zk_group_pk::Shard& S = pk->shard[g];
+        const b200zk_group_r1cs::Shard& Q = mats[g];
+        B2_CUDA_OK(ctx, sl.small.reserve(4096));
+        const Fr* z = z0p;
+        if (g) {
+            B2_CUDA_OK(ctx, cudaStreamWaitEvent(sl.stream, grp->ev_done[0], 0));
+            B2_CUDA_OK(ctx, cudaMemcpyPeerAsync(w.z[g], ctx->device, z0p, grp->ctx[0]->device, zbytes, sl.stream));
+            z = w.z[g];
+        }
+        zq[g] = z + S.v0;
+        zl[g] = z + n_inputs + S.l0;
+        return qap_slots_dev(ctx, sl, Q.ptr[0], Q.col[0], Q.val[0], Q.ptr[1], Q.col[1], Q.val[1], nc, n_inputs, z, log_rows, log_cols,
+                             (size_t)g * cg, loc, w.a[g], w.b[g], w.c[g]);
+    });
+    if (rc) return rc;
+    return prove_columns(grp, pk, w, zq.data(), zl.data(), r, s, proof_out);
+}
+
+// The body of b200zk_group_pk_upload (the caller holds the slot locks), with the table window of b200zk_zkey_load: 0 = the
+// automatic policy, 0xFFFFFFFF = no tables, else c on every shard.  The queries are host bytes.
+int group_pk_build(b200zk_group* grp, const void* a_query, const void* b_g1_query, const void* b_g2_query, const void* l_query,
+                   const void* h_query, size_t n_vars, size_t n_inputs, size_t m, const uint64_t* vk_points, unsigned table_window,
+                   b200zk_group_pk** out) {
+    if (n_vars == 0 || n_inputs == 0 || n_inputs > n_vars) return gerr(grp, B200ZK_ERR_ARG, "need 1 <= n_inputs <= n_vars");
+    if (m == 0 || (m & (m - 1))) return gerr(grp, B200ZK_ERR_DOMAIN, "h_query length must be a power of two");
+    const int P = grp->n;
+    const unsigned log_m = ceil_log2(m);
+    unsigned log_rows, log_cols;
+    split_log(log_m, &log_rows, &log_cols);
+    const size_t rows = (size_t)1 << log_rows, cols = (size_t)1 << log_cols;
+    if (cols < (size_t)P) return gerr(grp, B200ZK_ERR_ARG, "domain too small for this many GPUs");
+    b200zk_group_pk* pk = new b200zk_group_pk();
+    pk->n = P; pk->n_vars = n_vars; pk->n_inputs = n_inputs; pk->m = m; pk->log_m = log_m; pk->owner = grp;
+    pk->shard.resize(P);
+    const size_t n_aux = n_vars - n_inputs;
+    // table_window as b200zk_pk_precompute's c: 0 is the automatic policy, which B200ZK_PK_TABLES=0 turns off
+    const bool want_tables = table_window != 0xFFFFFFFFu && (table_window != 0 || pk_tables_enabled());
+    int rc = each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) -> int {
+        b200zk_group_pk::Shard& S = pk->shard[g];
+        S.v0 = cut(n_vars, g, P); S.v1 = cut(n_vars, g + 1, P);
+        S.l0 = cut(n_aux, g, P); S.l1 = cut(n_aux, g + 1, P);
+        S.hn = m / P;
+        const size_t cnt[5] = {S.v1 - S.v0, S.v1 - S.v0, S.v1 - S.v0, S.l1 - S.l0, S.hn};
+        const size_t psz[5] = {64, 64, 128, 64, 64};
+        const void* src[4] = {reinterpret_cast<const char*>(a_query) + S.v0 * 64, reinterpret_cast<const char*>(b_g1_query) + S.v0 * 64,
+                              reinterpret_cast<const char*>(b_g2_query) + S.v0 * 128,
+                              l_query ? reinterpret_cast<const char*>(l_query) + S.l0 * 64 : nullptr};
+        for (int k = 0; k < 5; ++k) {
+            if (cudaMalloc(&S.q[k], cnt[k] * psz[k] + 16) != cudaSuccess) return set_error(ctx, B200ZK_ERR_OOM, "proving-key shard allocation failed");
+            if (k < 4 && cnt[k] && cudaMemcpyAsync(S.q[k], src[k], cnt[k] * psz[k], cudaMemcpyHostToDevice, sl.stream) != cudaSuccess)
+                return set_error(ctx, B200ZK_ERR_CUDA, "proving-key upload failed");
+        }
+        {   // h_query in the column layout of the h this device will compute: local[c][r] = h_query[r cols + g cg + c]
+            const size_t cg = cols / P;
+            if (sl.io_a.reserve(S.hn * 64) != cudaSuccess) return set_error(ctx, B200ZK_ERR_OOM, "staging allocation failed");
+            if (cudaMemcpy2DAsync(sl.io_a.p, cg * 64, reinterpret_cast<const char*>(h_query) + g * cg * 64, cols * 64, cg * 64, rows,
+                                  cudaMemcpyHostToDevice, sl.stream) != cudaSuccess)
+                return set_error(ctx, B200ZK_ERR_CUDA, "h_query upload failed");
+            B2_TRY(transpose_dev<Blob64>(ctx, sl.stream, sl.io_a.p, S.q[4], rows, cg));
+        }
+        if (want_tables) {          // B200ZK_PK_TABLE_WINDOW is not read here
+            size_t bytes = 0;
+            B2_TRY(pk_tables_build(ctx, sl, S.q, cnt, table_window, S.tab, S.tab_c, &bytes));
+            pk->table_bytes += bytes;
+        }
+        return B200ZK_OK;
+    });
+    // device 0 keeps the vk points for the final assembly (queries of the tiny pk object are never read: include_zero_terms = 0)
+    if (!rc) rc = on_device(grp, 0, [&](b200zk_ctx* c0, Slot& s0) -> int {
+        pk->pk0 = new b200zk_pk();
+        pk->pk0->n_vars = n_vars; pk->pk0->n_inputs = n_inputs; pk->pk0->m = m;
+        if (cudaMalloc(&pk->pk0->vk, 56 * 8) != cudaSuccess || cudaMemcpyAsync(pk->pk0->vk, vk_points, 56 * 8, cudaMemcpyHostToDevice, s0.stream) != cudaSuccess)
+            return set_error(c0, B200ZK_ERR_CUDA, "vk upload failed");
+        return B200ZK_OK;
+    });
+    if (!rc) rc = sync_all(grp);
+    if (rc) {
+        b200zk_group_pk_free(grp, pk);
+        return rc;
+    }
+    *out = pk;
+    return B200ZK_OK;
 }
 
 }  // namespace
@@ -528,64 +647,7 @@ int b200zk_group_pk_upload(b200zk_group* grp, const uint64_t* a_query, const uin
                            const uint64_t* vk_points, b200zk_group_pk** out) {
     return with_group(grp, [&]() -> int {
         if (!out || !a_query || !b_g1_query || !b_g2_query || !h_query || !vk_points) return B200ZK_ERR_ARG;
-        if (n_vars == 0 || n_inputs == 0 || n_inputs > n_vars) return gerr(grp, B200ZK_ERR_ARG, "need 1 <= n_inputs <= n_vars");
-        if (m == 0 || (m & (m - 1))) return gerr(grp, B200ZK_ERR_DOMAIN, "h_query length must be a power of two");
-        const int P = grp->n;
-        const unsigned log_m = ceil_log2(m);
-        unsigned log_rows, log_cols;
-        split_log(log_m, &log_rows, &log_cols);
-        const size_t rows = (size_t)1 << log_rows, cols = (size_t)1 << log_cols;
-        if (cols < (size_t)P) return gerr(grp, B200ZK_ERR_ARG, "domain too small for this many GPUs");
-        b200zk_group_pk* pk = new b200zk_group_pk();
-        pk->n = P; pk->n_vars = n_vars; pk->n_inputs = n_inputs; pk->m = m; pk->log_m = log_m; pk->owner = grp;
-        pk->shard.resize(P);
-        const size_t n_aux = n_vars - n_inputs;
-        const bool want_tables = pk_tables_enabled();
-        int rc = each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) -> int {
-            b200zk_group_pk::Shard& S = pk->shard[g];
-            S.v0 = cut(n_vars, g, P); S.v1 = cut(n_vars, g + 1, P);
-            S.l0 = cut(n_aux, g, P); S.l1 = cut(n_aux, g + 1, P);
-            S.hn = m / P;
-            const size_t cnt[5] = {S.v1 - S.v0, S.v1 - S.v0, S.v1 - S.v0, S.l1 - S.l0, S.hn};
-            const size_t psz[5] = {64, 64, 128, 64, 64};
-            const void* src[4] = {reinterpret_cast<const char*>(a_query) + S.v0 * 64, reinterpret_cast<const char*>(b_g1_query) + S.v0 * 64,
-                                  reinterpret_cast<const char*>(b_g2_query) + S.v0 * 128,
-                                  l_query ? reinterpret_cast<const char*>(l_query) + S.l0 * 64 : nullptr};
-            for (int k = 0; k < 5; ++k) {
-                if (cudaMalloc(&S.q[k], cnt[k] * psz[k] + 16) != cudaSuccess) return set_error(ctx, B200ZK_ERR_OOM, "proving-key shard allocation failed");
-                if (k < 4 && cnt[k] && cudaMemcpyAsync(S.q[k], src[k], cnt[k] * psz[k], cudaMemcpyHostToDevice, sl.stream) != cudaSuccess)
-                    return set_error(ctx, B200ZK_ERR_CUDA, "proving-key upload failed");
-            }
-            {   // h_query in the column layout of the h this device will compute: local[c][r] = h_query[r cols + g cg + c]
-                const size_t cg = cols / P;
-                if (sl.io_a.reserve(S.hn * 64) != cudaSuccess) return set_error(ctx, B200ZK_ERR_OOM, "staging allocation failed");
-                if (cudaMemcpy2DAsync(sl.io_a.p, cg * 64, reinterpret_cast<const char*>(h_query) + g * cg * 64, cols * 64, cg * 64, rows,
-                                      cudaMemcpyHostToDevice, sl.stream) != cudaSuccess)
-                    return set_error(ctx, B200ZK_ERR_CUDA, "h_query upload failed");
-                B2_TRY(transpose_dev<Blob64>(ctx, sl.stream, sl.io_a.p, S.q[4], rows, cg));
-            }
-            if (want_tables) {          // automatic windows only: B200ZK_PK_TABLE_WINDOW is not read here
-                size_t bytes = 0;
-                B2_TRY(pk_tables_build(ctx, sl, S.q, cnt, 0, S.tab, S.tab_c, &bytes));
-                pk->table_bytes += bytes;
-            }
-            return B200ZK_OK;
-        });
-        // device 0 keeps the vk points for the final assembly (queries of the tiny pk object are never read: include_zero_terms = 0)
-        if (!rc) rc = on_device(grp, 0, [&](b200zk_ctx* c0, Slot& s0) -> int {
-            pk->pk0 = new b200zk_pk();
-            pk->pk0->n_vars = n_vars; pk->pk0->n_inputs = n_inputs; pk->pk0->m = m;
-            if (cudaMalloc(&pk->pk0->vk, 56 * 8) != cudaSuccess || cudaMemcpyAsync(pk->pk0->vk, vk_points, 56 * 8, cudaMemcpyHostToDevice, s0.stream) != cudaSuccess)
-                return set_error(c0, B200ZK_ERR_CUDA, "vk upload failed");
-            return B200ZK_OK;
-        });
-        if (!rc) rc = sync_all(grp);
-        if (rc) {
-            b200zk_group_pk_free(grp, pk);
-            return rc;
-        }
-        *out = pk;
-        return B200ZK_OK;
+        return group_pk_build(grp, a_query, b_g1_query, b_g2_query, l_query, h_query, n_vars, n_inputs, m, vk_points, 0, out);
     });
 }
 
@@ -729,36 +791,128 @@ int b200zk_group_groth16_prove_r1cs_dev(b200zk_group* grp, const b200zk_group_pk
             return gerr(grp, B200ZK_ERR_ARG, "constraint matrices with " + std::to_string(q->n_inputs) + " inputs, proving key with " + std::to_string(pk->n_inputs));
         if (q->n_vars != pk->n_vars)
             return gerr(grp, B200ZK_ERR_ARG, "constraint matrices over " + std::to_string(q->n_vars) + " variables, proving key over " + std::to_string(pk->n_vars));
+        return prove_r1cs_columns(grp, pk, q->shard, q->nc, q->n_inputs, false, [&](b200zk_ctx*, Slot&, Fr*, const Fr** z) {
+            *z = reinterpret_cast<const Fr*>(d_z);         // the caller wrote it on device 0's slot-0 stream
+            return B200ZK_OK;
+        }, r, s, proof_out);
+    });
+}
+
+// ---- a snarkjs zkey resident on the group (the group twin of b200zk_zkey_*, zkey.cu) -------------------------------------------
+void b200zk_group_zkey_free(b200zk_group* grp, b200zk_group_zkey* zk) {
+    DeviceGuard dev_guard;
+    if (!zk) return;
+    for (size_t g = 0; g < zk->csr.size(); ++g) {
+        if (grp && g < grp->ctx.size()) cudaSetDevice(grp->ctx[g]->device);
+        if (zk->csr[g]) cudaFree(zk->csr[g]);
+    }
+    b200zk_group_pk_free(grp, zk->pk);
+    delete zk;
+}
+
+int b200zk_group_zkey_load(b200zk_group* grp, const void* zkey, size_t zkey_len, unsigned table_window, b200zk_group_zkey** out) {
+    return with_group(grp, [&]() -> int {
+        if (!zkey || !out) return gerr(grp, B200ZK_ERR_ARG, "zkey_load: null pointer");
+        *out = nullptr;
+        const uint8_t* file = reinterpret_cast<const uint8_t*>(zkey);
+        sjf::Zkey h;
+        std::string err;
+        const int hrc = zkey_header(file, zkey_len, &h, &err);
+        if (hrc) return gerr(grp, hrc, err);
         const int P = grp->n;
+        const size_t m = h.domain_size;
         unsigned log_rows, log_cols;
-        split_log(pk->log_m, &log_rows, &log_cols);
-        const size_t cg = ((size_t)1 << log_cols) / P, loc = pk->m / P, zbytes = pk->n_vars * sizeof(Fr);
-        // the caller wrote z on device 0's slot-0 stream: every other device's copy of it waits for that point
+        split_log(ceil_log2(m), &log_rows, &log_cols);
+        if (((size_t)1 << log_cols) < (size_t)P) return gerr(grp, B200ZK_ERR_ARG, "domain too small for this many GPUs");
+        const ColumnLayout cl{log_rows, log_cols, log_cols - ceil_log2((size_t)P)};
+        const size_t loc = m / P, L = 2 * loc + 1, ptr_bytes = (L * 4 + 15) & ~(size_t)15;
+        b200zk_group_zkey* zk = new b200zk_group_zkey();
+        zk->owner = grp; zk->n_vars = h.n_vars; zk->n_public = h.n_public; zk->domain_size = m;
+        zk->csr.assign(P, nullptr);
+        zk->mats.resize(P);
+        // the sort on device 0, keyed owner-major: GPU g's A and B are entries [2 g loc, 2 (g + 1) loc] of its row_ptr
+        ZkeyCsr all;
+        std::vector<uint32_t> start(P + 1);
         int rc = on_device(grp, 0, [&](b200zk_ctx* c0, Slot& s0) -> int {
-            B2_CUDA_OK(c0, cudaEventRecord(grp->ev_done[0], s0.stream));
+            B2_TRY(zkey_group_matrices_dev(c0, s0, file, h, cl, &all));
+            B2_CUDA_OK(c0, cudaMemcpy2DAsync(start.data(), 4, all.row_ptr, 2 * loc * 4, 4, P + 1, cudaMemcpyDeviceToHost, s0.stream));
+            B2_CUDA_OK(c0, cudaStreamSynchronize(s0.stream));
             return B200ZK_OK;
         });
-        // the tail (devices >= 1): a copy of z.  a, b, c are written by the mat-vec.
-        Columns w(P);
-        if (!rc) rc = carve_columns(grp, loc, [&](int g) { return g ? pk->n_vars : 0; }, w);
-        std::vector<const Fr*> zq(P), zl(P);
+        zk->num_constraints = all.nc;
+        // every GPU's slice into one allocation of its own, row_ptr rebased to start at 0
         if (!rc) rc = each_device(grp, [&](int g, b200zk_ctx* ctx, Slot& sl) -> int {
-            const b200zk_group_pk::Shard& S = pk->shard[g];
-            const b200zk_group_r1cs::Shard& Q = q->shard[g];
-            B2_CUDA_OK(ctx, sl.small.reserve(4096));
-            const Fr* z = reinterpret_cast<const Fr*>(d_z);
-            if (g) {
-                B2_CUDA_OK(ctx, cudaStreamWaitEvent(sl.stream, grp->ev_done[0], 0));
-                B2_CUDA_OK(ctx, cudaMemcpyPeerAsync(w.z[g], ctx->device, d_z, grp->ctx[0]->device, zbytes, sl.stream));
-                z = w.z[g];
+            const size_t nnz = start[g + 1] - start[g];
+            B2_CUDA_OK(ctx, cudaMalloc(&zk->csr[g], ptr_bytes + nnz * 36 + 16));
+            uint32_t* row_ptr = reinterpret_cast<uint32_t*>(zk->csr[g]);
+            Fr* val = reinterpret_cast<Fr*>(reinterpret_cast<char*>(zk->csr[g]) + ptr_bytes);
+            uint32_t* col = reinterpret_cast<uint32_t*>(val + nnz);
+            const int d0 = grp->ctx[0]->device;
+            B2_CUDA_OK(ctx, cudaMemcpyPeerAsync(row_ptr, ctx->device, all.row_ptr + (size_t)g * 2 * loc, d0, L * 4, sl.stream));
+            if (nnz) {
+                B2_CUDA_OK(ctx, cudaMemcpyPeerAsync(val, ctx->device, all.val + start[g], d0, nnz * sizeof(Fr), sl.stream));
+                B2_CUDA_OK(ctx, cudaMemcpyPeerAsync(col, ctx->device, all.col + start[g], d0, nnz * 4, sl.stream));
             }
-            zq[g] = z + S.v0;
-            zl[g] = z + pk->n_inputs + S.l0;
-            return qap_slots_dev(ctx, sl, Q.ptr[0], Q.col[0], Q.val[0], Q.ptr[1], Q.col[1], Q.val[1], q->nc, q->n_inputs, z, log_rows, log_cols,
-                                 (size_t)g * cg, loc, w.a[g], w.b[g], w.c[g]);
+            B2_TRY(rebase_dev(ctx, sl, row_ptr, L, start[g]));
+            b200zk_group_r1cs::Shard& Q = zk->mats[g];
+            Q.ptr[0] = row_ptr; Q.ptr[1] = row_ptr + loc;
+            Q.col[0] = Q.col[1] = col;
+            Q.val[0] = Q.val[1] = val;
+            return B200ZK_OK;
         });
+        if (!rc) rc = sync_all(grp);
+        if (all.csr) {                                  // device 0 keeps only its own share
+            cudaSetDevice(grp->ctx[0]->device);
+            cudaFree(all.csr);
+        }
+        if (!rc) {
+            uint64_t vk[56];
+            zkey_vk_points(file, h, vk);
+            rc = group_pk_build(grp, file + h.a, file + h.b1, file + h.b2, file + h.l, file + h.h, h.n_vars, (size_t)h.n_public + 1, m, vk,
+                                table_window, &zk->pk);
+        }
+        if (rc) {
+            b200zk_group_zkey_free(grp, zk);
+            return rc;
+        }
+        *out = zk;
+        return B200ZK_OK;
+    });
+}
+
+int b200zk_group_zkey_info(const b200zk_group_zkey* zk, size_t* n_vars, size_t* n_public, size_t* domain_size, size_t* num_constraints) {
+    if (!zk) return B200ZK_ERR_ARG;
+    if (n_vars) *n_vars = zk->n_vars;
+    if (n_public) *n_public = zk->n_public;
+    if (domain_size) *domain_size = zk->domain_size;
+    if (num_constraints) *num_constraints = zk->num_constraints;
+    return B200ZK_OK;
+}
+
+size_t b200zk_group_zkey_table_bytes(const b200zk_group_zkey* zk) { return zk && zk->pk ? zk->pk->table_bytes : 0; }
+
+int b200zk_group_zkey_prove(b200zk_group* grp, const b200zk_group_zkey* zk, const void* wtns, size_t wtns_len, const uint64_t r[4],
+                            const uint64_t s[4], uint8_t proof_out[128], char* proof_json, size_t* proof_json_len, char* public_json,
+                            size_t* public_json_len) {
+    return with_group(grp, [&]() -> int {
+        if (!zk || !wtns || (proof_json && !proof_json_len) || (public_json && !public_json_len))
+            return gerr(grp, B200ZK_ERR_ARG, "zkey_prove: null key or witness, or a JSON buffer without its length");
+        if (zk->owner != grp) return gerr(grp, B200ZK_ERR_ARG, "zkey was loaded on a different group");
+        WtnsJob job;
+        std::string err;
+        const int prc = wtns_prologue(reinterpret_cast<const uint8_t*>(wtns), wtns_len, zk->n_vars, zk->n_public, r, s, proof_json,
+                                      proof_json_len, public_json, public_json_len, &job, &err);
+        if (prc) return gerr(grp, prc, err);
+        uint8_t proof[128];
+        int rc = prove_r1cs_columns(grp, zk->pk, zk->mats, zk->num_constraints, zk->n_public + 1, true,
+                                    [&](b200zk_ctx* c0, Slot& s0, Fr* tail, const Fr** z) {
+            *z = tail;
+            return witness_to_device(c0, s0, job.z, zk->n_vars, tail);
+        }, job.r, job.s, proof);
         if (rc) return rc;
-        return prove_columns(grp, pk, w, zq.data(), zl.data(), r, s, proof_out);
+        return on_device(grp, 0, [&](b200zk_ctx* c0, Slot& s0) {
+            return zkey_outputs_dev(c0, s0, proof, job, proof_out, proof_json, proof_json_len, public_json, public_json_len);
+        });
     });
 }
 

@@ -33,6 +33,7 @@ typedef struct b200zk_group b200zk_group;         /* several GPUs of one box, on
 typedef struct b200zk_group_pk b200zk_group_pk;   /* a proving key sharded over a group */
 typedef struct b200zk_group_r1cs b200zk_group_r1cs;   /* a circuit's A and B sharded over a group by QAP output slot */
 typedef struct b200zk_zkey b200zk_zkey;   /* a snarkjs Groth16 .zkey resident in HBM: b200zk_pk + A, B in CSR */
+typedef struct b200zk_group_zkey b200zk_group_zkey;   /* the same resident on a group: b200zk_group_pk + A, B sharded by slot */
 
 enum {
     B200ZK_OK = 0,
@@ -436,6 +437,33 @@ int  b200zk_group_r1cs_local_row_ptr(const uint32_t* row_ptr, size_t num_constra
  * (B200ZK_ERR_DOMAIN). */
 int  b200zk_group_groth16_prove_r1cs_dev(b200zk_group* group, const b200zk_group_pk* pk, const b200zk_group_r1cs* matrices,
                                          const void* d_z, const uint64_t r[4], const uint64_t s[4], uint8_t proof_out[128]);
+
+/* ---- snarkjs `groth16 prove` from the files' bytes on a group (csrc/group.cu, csrc/zkey.cu): b200zk_zkey_* sharded -------
+ * b200zk_group_zkey_load: b200zk_zkey_load on a group.  The header checks, messages and codes are b200zk_zkey_load's
+ * (B200ZK_ERR_ARG / B200ZK_ERR_DOMAIN before any launch); a domain whose cols = 2^floor(log m / 2) is below the group size is
+ * refused before any launch with B200ZK_ERR_ARG, "domain too small for this many GPUs".  The coefficient section is sorted
+ * once on GPU 0, keyed (owner GPU, matrix, slot), so that every GPU's A and B are one contiguous slice, which is copied to
+ * that GPU; the layout is b200zk_group_r1cs_upload's (local slot c rows + r is global row r cols + g cg + c).  The point
+ * sections are sharded from the caller's bytes as b200zk_group_pk_upload shards them (a, b1, b2, l by index range, h in the
+ * column layout); the vk points come from the header.  table_window as b200zk_zkey_load's, on every shard: 0 = the
+ * automatic policy (B200ZK_PK_TABLES), 0xFFFFFFFF = no tables, else the window c.  The caller may unmap the file on return.
+ * Device memory, n coefficient records, m the domain size, P GPUs: peak on GPU 0 while sorting about 80 n + 16 m bytes (raw
+ * records, counters, the whole CSR and its own slice); held afterwards by GPU g, 36 bytes per record it owns + 8 m / P + 4
+ * bytes, plus its proving-key shard and tables (in an emulated group, `b200zk_group_create` with one device id repeated,
+ * every rank's share is on that device).  Errors: b200zk_group_last_error, "device N: " before device-side messages. */
+int    b200zk_group_zkey_load(b200zk_group* group, const void* zkey, size_t zkey_len, unsigned table_window,
+                              b200zk_group_zkey** out);
+void   b200zk_group_zkey_free(b200zk_group* group, b200zk_group_zkey* zk);
+int    b200zk_group_zkey_info(const b200zk_group_zkey* zk, size_t* n_vars, size_t* n_public, size_t* domain_size,
+                              size_t* num_constraints);
+size_t b200zk_group_zkey_table_bytes(const b200zk_group_zkey* zk);
+/* b200zk_zkey_prove on a group: the same arguments, texts, bytes, codes, messages and *_len outputs.  The witness goes to
+ * GPU 0, is checked and converted there and peer-copied to the other GPUs; then the sharded QAP, h and MSMs of
+ * b200zk_group_groth16_prove_r1cs_dev, and the JSON encodings on GPU 0.  A key loaded on another group: B200ZK_ERR_ARG
+ * before any launch. */
+int    b200zk_group_zkey_prove(b200zk_group* group, const b200zk_group_zkey* zk, const void* wtns, size_t wtns_len,
+                               const uint64_t r[4], const uint64_t s[4], uint8_t proof_out[128], char* proof_json,
+                               size_t* proof_json_len, char* public_json, size_t* public_json_len);
 
 /* ---- the parties' local share arithmetic (n-party compatibility mirrors, SURVEY 8f4) ----------------------------------
  * Element-wise Fr operation on host buffers of n x 4 Montgomery limbs: op 0 = a * b (share-wise product of two sharings,
